@@ -2,6 +2,7 @@
 """bench.py -- BASELINE.json's metric on BASELINE.json's configs.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config fwd|fwdbwd|cascade|train8]
+                    [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W      (one rank per GPU)
 
 --config fwd (default, BASELINE configs[1], the judged line): image-pairs/sec of the MaskFlownet-S forward at 1024x448,
@@ -11,16 +12,15 @@ and out; every contraction (correlations, deformable warp, all 3x3 / transposed 
 kernels with each operand split into bf16 hi + bf16 lo (hi*hi + hi*lo + lo*hi, fp32 accumulation: ~2^-17 relative, inside
 the 1e-4 bound of north_star; no cuDNN / cuBLAS kernel runs in the step).
   value            device-resident inputs, the step replayed from a CUDA graph (network.FlowPredictor), K steps, CUDA events
-  value_sustained  the same loop repeated until >= --sustain-seconds inside the same protocol (power-capped clocks)
+  value_sustained  with --sustain-seconds S > 0: the same loop repeated until >= S seconds (power-capped clocks)
   e2e              the public serving API (network.PipelinedFlowPredictor) with HOST buffers: pinned uint8 H2D and pinned
                    fp32 flow D2H inside the timed region, overlapped with the forward on copy streams
   roofline         level-2 correlation launch timed inside an eager step with CUDA events (+ every correlation and warp
-                   launch; K3 against HBM bytes and bf16 flops); `traffic` = dram bytes per launch from the committed ncu
-                   capture of the same kernel (static: ncu cannot run inside the timed region)
+                   launch; K3 against HBM bytes and bf16 flops)
   cpu_baseline     oracle port of the whole forward on the host cores + the correlation-only table of BASELINE.md section 3
                    (1-thread literal MXNet loop nest / OpenMP all cores / torch-CPU) per pair, configs[0] first
 --config fwdbwd  (configs[2])  MaskFlownet-S forward + MultiscaleEpe + backward, batch 8, 512x384 (3x3 convolutions: forward
-                               on the tcgen05 kernel, backward cuDNN fp32 -- `--train-tc-forward 0` = cuDNN both ways;
+                               on the wgmma kernel, backward cuDNN fp32 -- `--train-tc-forward 0` = cuDNN both ways;
                                MultiscaleEpe = the fused kernels of csrc/loss.cu)
 --config cascade (configs[3])  MaskFlownet (S head + dual pyramid, md=2 correlations) forward, batch 4, 1024x448
 --config train8  (configs[4])  training step, batch 4 per GPU (32 on 8 GPUs), 960x540 padded to 960x576 like
@@ -29,6 +29,12 @@ the 1e-4 bound of north_star; no cuDNN / cuBLAS kernel runs in the step).
 --impl reference times the CPU arm: the reference's own CPU path cannot run here (MXNet is not installable, SURVEY.md
 section 8c), so it is the oracle port (oracle/network_ref.py: torch-CPU convolutions + the C oracle's OpenMP correlation /
 deformable convolution) on the host threads, one image pair per step (a bounded sample of the same workload).
+
+--dump-outputs DIR  after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy (float32):
+                    fwd / cascade / --impl reference: flow.npy (the full-resolution flow); fwdbwd / train8: loss.npy (the
+                    per-sample loss) and grad.npy (the flat gradient bucket of all parameters, in model.parameters() order;
+                    train8: after the all-reduce and its 1/global-batch scale).
+                    Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -51,23 +57,9 @@ ARITH = "f32 I/O; bf16 hi+lo split operands (hi*hi+hi*lo+lo*hi) on tensor cores,
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 1590.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md 6.65 TB/s, 1.59 PFLOP/s)"
-
-
-def dram_traffic(kernel_name: str):
-    """dram read+write bytes per launch of the named kernel from the committed ncu captures (profiles/r0?_dram_traffic.json)."""
-    for fn in ("r02_dram_traffic.json", "r01_dram_traffic.json"):
-        try:
-            for key, rec in json.load(open(os.path.join(ROOT, "profiles", fn))).items():
-                if not key.startswith("_") and key in (kernel_name or ""):
-                    return int(rec["dram_read_bytes"]) + int(rec["dram_write_bytes"]), f"static: profiles/{fn} (ncu --set full)"
-        except (OSError, ValueError, KeyError):
-            pass
-    return None, "no ncu capture of this kernel committed"
+    """HBM GB/s and dense bf16 TFLOP/s the fractions are taken against: NVIDIA's H100 SXM data sheet (700 W part); a card
+    with a lower power limit reaches less."""
+    return 3350.0, 989.0, "H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16)"
 
 
 class ClockSampler(threading.Thread):
@@ -142,12 +134,15 @@ def usable_host_threads() -> int:
 
 def cpu_arm(steps: int, warmup: int, max_threads: int, H=448, W=1024):
     """Oracle port of the same forward on the host cores; one pair per step.  The thread count is the fastest of a short
-    probe over {8, 16, 32, 64, all usable} (more threads only add contention on the small pyramid levels)."""
+    probe over {8, 16, 32, 64, all usable} (more threads only add contention on the small pyramid levels).
+    Returns (pairs/s, s/step, threads, flow of the last step)."""
     from oracle import cref, network_ref
     from maskflownet_b200.network import MaskFlownetS
+    torch.manual_seed(0)
     model = MaskFlownetS()
     params = {k: v.detach() for k, v in model.named_parameters()}
     a, b = synthetic_pairs(1, 0, H, W)
+    last = [None]
 
     def run(n, threads):
         torch.set_num_threads(threads)
@@ -155,7 +150,7 @@ def cpu_arm(steps: int, warmup: int, max_threads: int, H=448, W=1024):
         t0 = time.perf_counter()
         with torch.no_grad():
             for _ in range(n):
-                network_ref.predict_flow(params, a, b, threads=threads)
+                last[0] = network_ref.predict_flow(params, a, b, threads=threads)
         return (time.perf_counter() - t0) / n
 
     cands = sorted({t for t in (8, 16, 32, 64, max_threads) if t <= max_threads})
@@ -164,7 +159,7 @@ def cpu_arm(steps: int, warmup: int, max_threads: int, H=448, W=1024):
     for _ in range(max(0, warmup - 1)):
         run(1, best)
     sec = run(steps, best)
-    return 1.0 / sec, sec, best
+    return 1.0 / sec, sec, best, last[0]
 
 
 def cpu_corr_table(max_threads: int):
@@ -231,18 +226,26 @@ def barrier(c):
 
 def timed(c, fn, K, sync_extra=None):
     """EXACTLY K calls of fn bracketed by barrier + synchronize; 256 MiB L2 flush before every call (inside the region);
-    device time from CUDA events, max over ranks."""
+    device time from CUDA events, max over ranks.  The last call's result is kept in c.last."""
     barrier(c)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(K):
         c.flush.zero_()
-        fn()
+        c.last = fn()
     if sync_extra is not None:
         sync_extra()      # copy streams joined into the timed region (their work must finish before e1)
     e1.record()
     barrier(c)
     return c.mdist.max_over_ranks(e0.elapsed_time(e1), c.dev)
+
+
+def dump_outputs(directory, arrays):
+    """Writes each array as <directory>/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), t.detach().float().cpu().numpy().astype(np.float32))
 
 
 def base_line(metric, value, K, Wm, ms_total, world, config):
@@ -298,6 +301,7 @@ def bench_fwd(args, K, Wm):
         ms_total = timed(c, step_graph, K)
         torch.cuda.profiler.stop()
         clocks = sampler.finish()
+        last_flow = c.last.clone()      # the graph's output buffer is overwritten by later replays
         # ---- e2e: host buffers through the serving API; copies inside the timed region ----
         ms_e2e = timed(c, step_e2e, K, sync_extra=lambda: (torch.cuda.current_stream().wait_stream(serve.d2h),
                                                            torch.cuda.current_stream().wait_stream(serve.h2d)))
@@ -351,7 +355,6 @@ def bench_fwd(args, K, Wm):
         return 18 * LEVEL_C[L] ** 2 * BATCH * (H >> L) * (W >> L)
     t2 = kt.get(("corr", 2))
     achieved = corr_bytes(2) / (t2 * 1e-3) / 1e9 if t2 else None
-    traffic, traffic_src = dram_traffic(corr_kernel)
     corr_levels = {f"L{L}": {"ms": round(kt[("corr", L)], 5), "alg_bytes": corr_bytes(L),
                              "gbs": round(corr_bytes(L) / kt[("corr", L)] / 1e6, 1),
                              "frac": round(corr_bytes(L) / kt[("corr", L)] / 1e6 / hbm, 4)} for L in (6, 5, 4, 3, 2) if ("corr", L) in kt}
@@ -384,8 +387,7 @@ def bench_fwd(args, K, Wm):
         line["value_sustained"] = sust
     line["roofline"] = {"kernel": f"{corr_kernel} (level-2 correlation, N=8 C=32 112x256, md=4)", "bound": "hbm",
                         "achieved": round(achieved, 1) if achieved else None, "peak": hbm, "unit": "GB/s",
-                        "frac": round(achieved / hbm, 4) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
-                        "peak_source": peak_kind, "alg_bytes_per_launch": corr_bytes(2),
+                        "frac": round(achieved / hbm, 4) if achieved else None, "peak_source": peak_kind, "alg_bytes_per_launch": corr_bytes(2),
                         "launch_ms_in_step": round(t2, 5) if t2 else None,
                         "launch_ms_isolated_cold_l2": round(sum(iso) / len(iso), 5),
                         "corr_levels": corr_levels, "corr_sum_ms": round(corr_sum_ms, 5),
@@ -394,7 +396,7 @@ def bench_fwd(args, K, Wm):
     if c.rank == 0 and c.world == 1 and args.cpu_sample_steps > 0:
         host_threads = usable_host_threads()
         try:
-            val, sec, used = cpu_arm(args.cpu_sample_steps, 1, host_threads)
+            val, sec, used, _ = cpu_arm(args.cpu_sample_steps, 1, host_threads)
             line["cpu_baseline"] = {"value": round(val, 4), "unit": "pairs/s", "cores": used, "kind": "port",
                                     "sample": f"{args.cpu_sample_steps} steps x 1 pair at 1024x448 on {used} of "
                                               f"{host_threads} host threads (oracle/network_ref.py)"}
@@ -403,6 +405,8 @@ def bench_fwd(args, K, Wm):
             line["cpu_baseline"] = {"value": None, "unit": "pairs/s", "cores": host_threads, "kind": "port",
                                     "sample": f"failed: {e}"}
     if c.rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"flow": last_flow})
         print(json.dumps(line), flush=True)
     if c.world > 1:
         torch.distributed.destroy_process_group()
@@ -478,7 +482,7 @@ def bench_other(args, K, Wm):
         extra["grad_bucket_mb"] = round(bucket.numel * 4 / 1e6, 1)
 
     def step_resident():
-        step(a_d, b_d, flow_d)
+        return step(a_d, b_d, flow_d)
 
     def step_e2e():
         x1, x2 = a_h.to(c.dev, non_blocking=True), b_h.to(c.dev, non_blocking=True)
@@ -495,6 +499,9 @@ def bench_other(args, K, Wm):
     torch.cuda.profiler.start()           # ncu --profile-from-start off: the launch list of the timed region only
     ms_total = timed(c, step_resident, K)
     torch.cuda.profiler.stop()
+    last_out = {"flow" if cfg == "cascade" else "loss": c.last.clone()}
+    if cfg != "cascade":
+        last_out["grad"] = bucket.flat.clone()      # the last timed step's gradients (later steps overwrite the bucket)
     launches = _lib.launch_count() - n0
     ar_ms = sum(x.elapsed_time(y) for x, y in t_ar) / len(t_ar) if t_ar else None
     ms_e2e = timed(c, step_e2e, K)
@@ -503,7 +510,7 @@ def bench_other(args, K, Wm):
     tc_fwd = bool(getattr(model, "train_tc_forward", False))
     config = {"workload": workload, "arithmetic": ARITH if cfg == "cascade" else
               "forward/backward of the hot path (correlation, fused warp): our exact-fp32 / bf16-split kernels; 3x3 convolutions: "
-              + ("forward on the tcgen05 kernel (f32 I/O, bf16 hi/lo split MMA, fp32 accumulate), backward aten.convolution_backward "
+              + ("forward on the wgmma kernel (f32 I/O, bf16 hi/lo split MMA, fp32 accumulate), backward aten.convolution_backward "
                  "(cuDNN fp32, TF32 off)" if tc_fwd else "torch autograd both ways (cuDNN fp32, TF32 off)")
               + "; MultiscaleEpe: fused forward / backward kernels (csrc/loss.cu)",
               "train_tc_forward": tc_fwd,
@@ -523,6 +530,8 @@ def bench_other(args, K, Wm):
         extra["nccl_ranks"] = c.world
     line.update(extra)
     if c.rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_out)
         print(json.dumps(line), flush=True)
     if c.world > 1:
         torch.distributed.destroy_process_group()
@@ -536,10 +545,13 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="fwd", choices=["fwd", "fwdbwd", "cascade", "train8"])
     ap.add_argument("--cpu-sample-steps", type=int, default=32)   # ~10 s of host work on a 16-thread box
-    ap.add_argument("--sustain-seconds", type=float, default=3.0)
+    ap.add_argument("--sustain-seconds", type=float, default=0.0,
+                    help="fwd: also time the graph loop for >= this many seconds (value_sustained); 0 = off")
     ap.add_argument("--train-tc-forward", type=int, default=-1,
-                    help="fwdbwd / train8: 1 = the 3x3 convolutions' forward on the tcgen05 kernel (cuDNN backward), 0 = cuDNN "
+                    help="fwdbwd / train8: 1 = the 3x3 convolutions' forward on the wgmma kernel (cuDNN backward), 0 = cuDNN "
                          "both ways, -1 = the model's default")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     K, Wm = args.steps, max(args.warmup, 0)
     rank = int(os.environ.get("RANK", "0"))
@@ -548,7 +560,9 @@ def main():
     if args.impl == "reference":
         if rank != 0:
             return
-        val, sec, used = cpu_arm(max(1, K), max(1, min(Wm, 1)), host_threads)
+        val, sec, used, flow = cpu_arm(max(1, K), max(1, min(Wm, 1)), host_threads)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"flow": flow})
         line = {"impl": "reference", "metric": "image-pairs/sec (MaskFlownet-S forward, 1024x448)", "value": round(val, 4),
                 "unit": "pairs/s", "n_gpus": args.gpus, "steps": K, "warmup": Wm, "ms_per_step": round(sec * 1e3, 2),
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",

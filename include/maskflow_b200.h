@@ -1,5 +1,5 @@
 /*
- * maskflow_b200.h -- C ABI of libmaskflow_b200.so: the MaskFlownet hot path on NVIDIA B200 (sm_100a).
+ * maskflow_b200.h -- C ABI of libmaskflow_b200.so: the MaskFlownet hot path on NVIDIA H100 (sm_90a).
  *
  * The reference (microsoft/MaskFlownet) reaches this path through Apache MXNet's operator registry
  * (the `F` namespace handed to HybridBlock.hybrid_forward).  Each entry point below replaces one MXNet
@@ -218,7 +218,7 @@ MFN_API int mfn_image_warp_concat_forward(const float* im1, const float* im2, co
  * needs no concat copies.  fp32-accurate tensor-core arithmetic (bf16 hi/lo split, 3 MMAs per product, fp32 accumulate).
  * Weights are packed once per layer: mfn_conv3x3_packed_bytes() -> caller allocates -> mfn_conv3x3_pack_weights().
  * Cout <= 256.  leaky_slope = 1 disables the activation.
- * Two kernels serve it: tcgen05.mma with TMEM accumulators (csrc/conv3x3_umma.cu, default; tuning key "conv_umma") and
+ * Two kernels serve it: warpgroup MMAs (csrc/conv3x3_wgmma.cu, default; tuning key "conv_wgmma") and
  * the mma.sync kernel (csrc/conv3x3.cu, stride 1, Cout <= 128); the packed buffer holds both weight images.
  * mfn_conv3x3_forward_ex adds
  *   - stride 2 (pad 1, dilation 1) = the feature pyramid's down-sampling convolutions conv{L}a / conv{L}x

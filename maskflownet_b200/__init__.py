@@ -1,4 +1,4 @@
-"""maskflownet_b200 -- Blackwell-native (sm_100a) implementation of the MaskFlownet hot path:
+"""maskflownet_b200 -- Hopper-native (sm_90a) implementation of the MaskFlownet hot path:
 the local correlation cost volume and the flow-guided deformable feature warp x occlusion mask that feeds it.
 
   maskflownet_b200.ops      tensor-level operators backed by libmaskflow_b200.so (C ABI: include/maskflow_b200.h)

@@ -52,7 +52,7 @@ class MaskflowError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources in-tree with nvcc for sm_100a (no GPU needed).  Returns the .so path."""
+    """Compile the CUDA sources in-tree with nvcc for sm_90a (no GPU needed).  Returns the .so path."""
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     res = subprocess.run(cmd, capture_output=not verbose, text=True)
     if res.returncode != 0:

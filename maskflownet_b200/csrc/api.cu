@@ -53,7 +53,6 @@ extern "C" int mfn_set_tuning(const char* key, int value) {
   else if (!strcmp(key, "warp_lin_fch")) mfn::tuning().warp_lin_fch = value;
   else if (!strcmp(key, "conv_as")) mfn::tuning().conv_as = value;
   else if (!strcmp(key, "conv_splitk")) mfn::tuning().conv_splitk = value;
-  else if (!strcmp(key, "conv_nacc")) mfn::tuning().conv_nacc = value;
   else if (!strcmp(key, "corr_rb_twb")) mfn::tuning().corr_rb_twb = value;
   else if (!strcmp(key, "corr_rb_rows")) mfn::tuning().corr_rb_rows = value;
   else if (!strcmp(key, "corr_tma")) mfn::tuning().corr_tma = value;
@@ -61,9 +60,9 @@ extern "C" int mfn_set_tuning(const char* key, int value) {
   else if (!strcmp(key, "corr_ts_hi")) mfn::tuning().corr_ts_hi = value;
   else if (!strcmp(key, "corr_dbg")) mfn::tuning().corr_dbg = value;
   else if (!strcmp(key, "corr_ring_th")) mfn::tuning().corr_ring_th = value;
-  else if (!strcmp(key, "conv_umma")) mfn::tuning().conv_umma = value;
+  else if (!strcmp(key, "conv_wgmma")) mfn::tuning().conv_wgmma = value;
   else if (!strcmp(key, "conv_grid_cap")) mfn::tuning().conv_grid_cap = value;
-  else if (!strcmp(key, "conv_umma_min_w")) mfn::tuning().conv_umma_min_w = value;
+  else if (!strcmp(key, "conv_wgmma_min_w")) mfn::tuning().conv_wgmma_min_w = value;
   else return mfn::fail(MFN_ERR_INVALID_ARG, "mfn_set_tuning: unknown key '%s'", key);
   return MFN_OK;
 }

@@ -21,6 +21,7 @@
 // the CPU -- test infrastructure for the kernel source, never a product path (the shim has no launcher, no C ABI).
 #ifdef MFN_HOST_EMULATION
 #include "cuda_shim.h"
+#include "device_caps.h"
 #else
 #include "common.cuh"
 #endif
@@ -75,8 +76,7 @@ __device__ __forceinline__ Taps sampler_taps(float gx, float gy, int H, int W) {
 }
 
 // uint8 sources are read as value / 255 (network/pipeline.py:100).  The 28 taps of a pixel would cost 28 IEEE divisions
-// (~10 instructions each; the first version of the kernel spent most of its issue slots there: 0.18 ms for 8 x 448 x 832
-// target pixels, profiles/r02_train_side_bench.jsonl): the 256 possible quotients are tabulated once per block instead --
+// (~10 instructions each; the first version of the kernel spent most of its issue slots there): the 256 possible quotients are tabulated once per block instead --
 // the same correctly rounded values, one shared-memory load per tap.
 template <typename T>
 __device__ __forceinline__ float ld(const T* p, int o, const float* lut) {
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(256)
 
 static inline unsigned grid_of(long long total) {
   long long b = (total + 255) / 256;
-  return (unsigned)(b < 1 ? 1 : (b > 148LL * 32 ? 148LL * 32 : b));
+  return (unsigned)(b < 1 ? 1 : (b > (long long)kNumSMs * 32 ? (long long)kNumSMs * 32 : b));
 }
 
 }  // namespace aug
@@ -370,7 +370,7 @@ extern "C" int mfn_color_augment_forward(const float* img1, const float* img2, c
   int rc = check_launch("color_sum_kernel");
   if (rc) return rc;
   int bps = (HW + 255) / 256;
-  const int cap = (148 * 16 + 2 * N - 1) / (2 * N);
+  const int cap = (kNumSMs * 16 + 2 * N - 1) / (2 * N);
   if (bps > cap) bps = cap;
   if (bps < 1) bps = 1;
   color_apply_kernel<<<dim3(bps, N, 2), 256, 0, st>>>(img1, img2, noise1, noise2, params, noise_sigma, (unsigned long long)seed,

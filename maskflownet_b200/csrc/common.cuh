@@ -1,9 +1,10 @@
-// common.cuh -- shared host/device helpers for libmaskflow_b200 (sm_100a only).
+// common.cuh -- shared host/device helpers for libmaskflow_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/maskflow_b200.h"
+#include "device_caps.h"
 
 namespace mfn {
 
@@ -16,15 +17,14 @@ void note_kernel(const char* name);
 struct Tuning {
   int corr_grid_cap = 0;      // > 0: cap the persistent grid of the MMA correlation kernels (tests force long tile runs)
   int corr_disable_ring = 0;  // 1: use the tile kernel even for C <= 32
-  int conv_umma = 1;          // 1: 3x3 convolutions run on tcgen05 / TMEM (conv3x3_umma.cu), 0: mma.sync kernel
-  int conv_grid_cap = 0;      // persistent tcgen05 convolution: CTAs (0 = one per SM); tests force long per-CTA tile runs
-  int conv_umma_min_w = 1;    // narrower images stay on the mma.sync kernel (a 128-pixel M tile would be mostly padding)
+  int conv_wgmma = 1;          // 1: 3x3 convolutions run on wgmma (conv3x3_wgmma.cu), 0: mma.sync kernel
+  int conv_grid_cap = 0;      // persistent wgmma convolution: CTAs (0 = one per SM); tests force long per-CTA tile runs
+  int conv_wgmma_min_w = 1;    // narrower images stay on the mma.sync kernel (a 128-pixel M tile would be mostly padding)
   int corr_ring_th = 8;       // tile height of the strip-marching kernel: 4 (8 warps, 2 CTAs/SM) or 8 (16 warps, 1 CTA/SM)
   int corr_rb = 1;            // 1: C > 32 correlations run on the row-block kernel (corr_rb.cu); 2: also C <= 32 when the TMA kernel declines; 0: chunked tile kernel
   int warp_lin_fch = 0;       // > 0: channels per thread of warp_lin_kernel (a multiple of 8; default: 16 / 32 / 64 by level size)
-  int conv_as = 0;            // 2: wide tcgen05 layers keep 2 input stages (more weight stages); default 3
+  int conv_as = 0;            // 2: wide wgmma layers keep 2 input stages (more weight stages); default 3
   int conv_splitk = 1;        // 0: never split K; 1: plan decides (<= 8 parts); k > 1: cap on the number of parts
-  int conv_nacc = 0;          // > 0: cap on the tcgen05 convolution's TMEM accumulator ring (default: as many as fit, <= 8)
   int corr_rb_twb = 0;        // 2: force 16-pixel strips in the row-block kernel (two CTAs per SM when the tile fits 113 KB)
   int corr_rb_rows = 0;       // > 0: start the row-block kernel's RB search at this value (4 / 2 / 1)
   int corr_tma = 1;           // 1: C <= 32 correlations run on the TMA pipeline kernel (corr_tma.cu) when the shape fits
@@ -43,7 +43,6 @@ static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStre
 
 static inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per function AND per device (a process may drive several GPUs: ops._call
 // switches the device per tensor): remember the largest opt-in per device, re-issue it when a launch needs more.
@@ -60,7 +59,7 @@ static inline cudaError_t ensure_dyn_smem(K kernel, int bytes, SmemOptIn& st) {
   return e;
 }
 
-// warp_lin.cu: K3 through linearity, exact for both border rules; -1 = the extended tcgen05 convolution does not fit
+// warp_lin.cu: K3 through linearity, exact for both border rules; -1 = the extended wgmma convolution does not fit
 long long warp_lin_workspace_bytes(int N, int F, int H, int W);
 int launch_warp_lin(const float* x, const float* flow_c, const float* mask_c, const float* weight, const void* packed_weight,
                     const float* bias, const float* tradeoff, void* workspace, float* out, float* fup, float* mup, int N,

@@ -1,4 +1,4 @@
-// conv3x3.cu -- decoder dense-block convolution (SURVEY.md section 8f, row N2) for sm_100a.
+// conv3x3.cu -- decoder dense-block convolution (SURVEY.md section 8f, row N2) for sm_90a.
 //
 // Serves mfn_conv3x3_forward: the 3x3 / stride 1 / pad 1 convolutions of the reference's decoder and context network
 //   x = concat(leaky(convL_i(x)), x)        network/MaskFlownet.py:219-223, 237-241, ... (conv block: :166-175)
@@ -278,9 +278,9 @@ static int launch_conv(const float* x, long long x_bs, const unsigned char* wpac
                   : launch_conv_impl<WC, NTN, true>(x, x_bs, wpack, bias, out, out_bs, N, Cin, H, W, Cout, dil, slope, lin_prefix, st);
 }
 
-// bytes of the mma.sync weight image (first region of the packed buffer; the tcgen05 image follows it)
+// bytes of the mma.sync weight image (first region of the packed buffer; the wgmma image follows it)
 long long conv3x3_sync_packed_bytes(int Cin, int Cout) {
-  if (Cout > 128) return 0;   // the mma.sync kernels stop at 128 output channels; wider layers exist only in the tcgen05 image
+  if (Cout > 128) return 0;   // the mma.sync kernels stop at 128 output channels; wider layers exist only in the wgmma image
   return (long long)((Cin + 31) / 32) * 9 * 2 * c3::cout_pad(Cout) * c3::PXB;
 }
 
@@ -288,7 +288,7 @@ long long conv3x3_sync_packed_bytes(int Cin, int Cout) {
 
 extern "C" long long mfn_conv3x3_packed_bytes(int Cin, int Cout) {
   if (Cin <= 0 || Cout <= 0) return 0;
-  return mfn::conv3x3_sync_packed_bytes(Cin, Cout) + mfn::conv3x3_umma_packed_bytes(Cin, Cout);
+  return mfn::conv3x3_sync_packed_bytes(Cin, Cout) + mfn::conv3x3_wgmma_packed_bytes(Cin, Cout);
 }
 
 extern "C" int mfn_conv3x3_pack_weights(const float* weight, void* packed, int Cin, int Cout, void* stream) {
@@ -307,7 +307,7 @@ extern "C" int mfn_conv3x3_pack_weights(const float* weight, void* packed, int C
     const int rc = check_launch("conv3x3_pack_kernel");
     if (rc) return rc;
   }
-  return conv3x3_umma_pack(weight, static_cast<unsigned char*>(packed) + conv3x3_sync_packed_bytes(Cin, Cout), Cin, Cout,
+  return conv3x3_wgmma_pack(weight, static_cast<unsigned char*>(packed) + conv3x3_sync_packed_bytes(Cin, Cout), Cin, Cout,
                            as_stream(stream));
 }
 
@@ -331,8 +331,8 @@ extern "C" long long mfn_conv3x3_workspace_bytes(int N, int Cin, int H, int W, i
   if (N <= 0 || Cin <= 0 || H <= 0 || W <= 0 || Cout <= 0 || Cout > 256 || dilation < 1 ||
       !(stride == 1 || (stride == 2 && dilation == 1)))
     return 0;
-  if (!(tuning().conv_umma && W >= tuning().conv_umma_min_w) && Cout <= 128 && stride == 1) return 0;   // mma.sync kernel
-  return conv3x3_umma_workspace_bytes(N, Cin, H, W, Cout, stride, dilation);
+  if (!(tuning().conv_wgmma && W >= tuning().conv_wgmma_min_w) && Cout <= 128 && stride == 1) return 0;   // mma.sync kernel
+  return conv3x3_wgmma_workspace_bytes(N, Cin, H, W, Cout, stride, dilation);
 }
 
 extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, const void* packed_weight,
@@ -363,8 +363,8 @@ extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, 
   const unsigned char* wp = static_cast<const unsigned char*>(packed_weight);
   cudaStream_t st = as_stream(stream);
   const bool sync_ok = Cout <= 128 && stride == 1 && mode == MFN_CONV_OUT_NCHW;   // what the mma.sync kernels cover
-  if ((tuning().conv_umma && W >= tuning().conv_umma_min_w) || !sync_ok) {   // tcgen05 / TMEM kernel
-    const int rc = conv3x3_umma_launch(x, xbs, wp + conv3x3_sync_packed_bytes(Cin, Cout), bias, out, obs, N, Cin, H, W,
+  if ((tuning().conv_wgmma && W >= tuning().conv_wgmma_min_w) || !sync_ok) {   // wgmma kernel
+    const int rc = conv3x3_wgmma_launch(x, xbs, wp + conv3x3_sync_packed_bytes(Cin, Cout), bias, out, obs, N, Cin, H, W,
                                        Cout, stride, dilation, out_mode, leaky_slope, st, 0, static_cast<float*>(workspace),
                                        workspace_bytes);
     if (rc != -1) return rc;

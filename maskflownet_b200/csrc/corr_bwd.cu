@@ -1,4 +1,4 @@
-// corr_bwd.cu -- correlation backward (K2) for sm_100a.
+// corr_bwd.cu -- correlation backward (K2) for sm_90a.
 //
 // Serves mfn_correlation_backward: the gradient of F.Correlation (network/MaskFlownet.py:193-195, 440-441) that the
 // reference obtains implicitly from autograd.record() / loss.backward() (network/pipeline.py:97,112-113).
@@ -15,7 +15,7 @@ namespace mfn {
 namespace k2 {
 // CTA = 4 rows x 32 pixels; thread = one 4-pixel quad x CPT channels (CPT = 1: 56 KB of shared memory, four CTAs per SM --
 // measured faster than CPT = 4 with two CTAs per SM: the kernel is bound by the latency of its tile loads, not by the
-// shared-memory traffic of the stencil, profiles/r02_ncu_corr_bwd_L2_summary.txt).
+// shared-memory traffic of the stencil).
 constexpr int TH = 4, TW = 32, CPT = 1, CK = 8 * CPT, NT = 256;
 }
 
@@ -40,8 +40,8 @@ __global__ void __launch_bounds__(k2::NT)
   const float* gon = go + (size_t)n * obs;
   const float* fon = fwd_out ? fwd_out + (size_t)n * obs : nullptr;
   // G tile: thread (warp w, lane) owns column xx = lane of the tile rows j = w + 8k, j = q * TH + rr  (rr = w & 3 and
-  // q = (w >> 2) + 2k).  Loads are issued in batches of 8 before any of them is consumed (the round-1 loop consumed each
-  // load at once: 65 % of the kernel's stall samples were that dependency, profiles/r02_ncu_corr_bwd_L2_summary.txt).
+  // q = (w >> 2) + 2k).  Loads are issued in batches of 8 before any of them is consumed (a loop that consumes each load
+  // at once stalls on that dependency).
   {
     const int w = tid >> 5, xx = tid & 31, rr = w & 3;
     constexpr int KQ = (D + 1) / 2;

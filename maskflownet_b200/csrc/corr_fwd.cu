@@ -1,4 +1,4 @@
-// corr_fwd.cu -- correlation cost-volume forward kernels (K1) for sm_100a.
+// corr_fwd.cu -- correlation cost-volume forward kernels (K1) for sm_90a.
 //
 // Serves mfn_correlation_forward (include/maskflow_b200.h), i.e. the reference's
 //   F.Correlation(im1, im2, pad_size=md, kernel_size=1, max_displacement=md, stride1=1, stride2=1,
@@ -935,7 +935,7 @@ static int launch_generic(const float* d1, const float* d2, float* out, int N, i
   const long long total = (long long)N * D * OH * OW;
   const int threads = 256;
   long long blocks = (total + threads - 1) / threads;
-  if (blocks > 148LL * 64) blocks = 148LL * 64;
+  if (blocks > (long long)kNumSMs * 64) blocks = (long long)kNumSMs * 64;
   corr_generic_kernel<<<(unsigned)blocks, threads, 0, st>>>(d1, d2, out, N, C, H, W, pad, ks, md, s1, s2, mul,
                                                            D, OH, OW, obs, slope);
   return check_launch("corr_generic_kernel");
@@ -1023,8 +1023,8 @@ static int launch_mma(const float* d1, const float* d2, float* out, int N, int C
     if (rc != -1) return rc;
   }
   // row-block kernel (corr_rb.cu, all channels resident, one CTA per output row block): wins only on the smallest level
-  // (level 6: 7 x 16, where the chunked tile kernel below has 16 tiles of 7 channel chunks); measured slower elsewhere
-  // (profiles/r02_kbench_corr.jsonl), so levels 3-5 stay on the tile kernel.
+  // (level 6: 7 x 16, where the chunked tile kernel below has 16 tiles of 7 channel chunks); it was measured slower
+  // elsewhere, so levels 3-5 stay on the tile kernel.
   if (tuning().corr_rb && C > 32 && (long long)N * H * W <= 1024) {
     const int rc = launch_corr_rb(MD, d1, d2, out, N, C, H, W, obs, slope, st);
     if (rc != -1) return rc;

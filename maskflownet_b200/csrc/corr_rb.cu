@@ -1,5 +1,5 @@
 // corr_rb.cu -- correlation cost-volume forward (K1) for C > 32 (levels 3..6 of the S head and of the cascade) and for the
-// shapes the TMA kernel cannot take (W % 4 != 0): "row-block" kernel, sm_100a.
+// shapes the TMA kernel cannot take (W % 4 != 0): "row-block" kernel, sm_90a.
 //
 // Serves mfn_correlation_forward (include/maskflow_b200.h) for the reference regime
 //   F.Correlation(pad_size=md, kernel_size=1, max_displacement=md, stride1=1, stride2=1, is_multiply=1) + LeakyReLU
@@ -15,7 +15,7 @@
 //   phase 2  warp = (8-pixel block, subset of the RB + 2 md data2 rows): per data2 row one ldmatrix sweep over K feeds the
 //            mma.sync.m16n8k16 chains of every pixel row it serves (banded formulation: 16 data2 positions x 8 pixels -> all
 //            dx of one dy; hi*lo + lo*hi + hi*hi, fp32 accumulate); LeakyReLU; per-warp staging; 32-byte plane-row stores.
-// RB (4 / 2 / 1) and the strip width (32 / 16 pixels) are chosen by the host so that the grid covers the 148 SMs.
+// RB (4 / 2 / 1) and the strip width (32 / 16 pixels) are chosen by the host so that the grid covers all SMs.
 #include <cuda_bf16.h>
 
 #include "common.cuh"

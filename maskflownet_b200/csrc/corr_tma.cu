@@ -1,5 +1,5 @@
 // corr_tma.cu -- correlation cost-volume forward (K1), the production kernel for C <= 32 (level 2 of the S head and of the
-// cascade: 55 % of the path's bytes).  sm_100a only.
+// cascade: 55 % of the path's bytes).  sm_90a only.
 //
 // Serves mfn_correlation_forward (include/maskflow_b200.h) for the reference regime
 //   F.Correlation(pad_size=md, kernel_size=1, max_displacement=md, stride1=1, stride2=1, is_multiply=1) + LeakyReLU
@@ -10,7 +10,7 @@
 //   HBM --TMA tensor loads--> raw fp32 ring --converter warps--> split-bf16 rings --MMA warps--> staging --TMA tensor stores--> HBM
 //
 //   * work unit   = 4 image rows x 32 pixels of one (n, x-strip) column; a CTA owns a contiguous run of units in
-//                   (strip, row-group) order (all 148 SMs get the same number of units +-1) and marches down the strips.
+//                   (strip, row-group) order (all SMs get the same number of units +-1) and marches down the strips.
 //   * producer    (1 thread): cp.async.bulk.tensor 4-D loads of [8 channels][4 rows][40 px] data2 boxes (4-pixel x halo) and
 //                   [8 channels][4 rows][32 px] data1 boxes straight from the NCHW tensors.  Out-of-image rows / columns /
 //                   channels are zero-filled by the TMA unit: that IS the operator's pad_size, no padded temporaries.
@@ -326,8 +326,8 @@ __global__ void __launch_bounds__(ct::NTHREADS, 1)
       // One step = data2 row t (image row y0 - MD + t), serving pixel rows r with dy index d = t - r.  The G - 3 steps in
       // which all four pixel rows are served run as a RUNTIME loop (unrolled by two for the fragment double buffer); only
       // the three ramp-up and three ramp-down steps are unrolled with their compile-time row sets.  The fully unrolled walk
-      // (12 x ~105 instructions, 20 KB) plus the other roles' code overflowed the 32 KB instruction cache level: 15 % of the
-      // stall samples were "no instruction" (profiles/r02_ncu_corr_tma_L2_summary.txt).
+      // (12 x ~105 instructions, 20 KB) plus the other roles' code overflowed the instruction cache: the warps stalled
+      // on instruction fetch.
       auto step = [&](const int t, const bool all, const uint32_t (&fh)[2][4], const uint32_t (&fl)[2][4], uint32_t (&nh)[2][4],
                       uint32_t (&nl)[2][4]) {
         if (t + 1 < NLR) frag(LR0 + t + 1, nh, nl);

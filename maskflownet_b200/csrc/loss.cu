@@ -17,6 +17,7 @@
 // Algorithmic bytes: forward 4*N*H*W*3 (flow + mask) + the coarse tensors; backward the same per scale from L2.
 #ifdef MFN_HOST_EMULATION
 #include "cuda_shim.h"
+#include "device_caps.h"
 #else
 #include "common.cuh"
 #endif
@@ -268,7 +269,7 @@ extern "C" int mfn_multiscale_epe_backward(const float* flow, const float* mask,
   if (rc) return rc;
   const long long warps = A.first_warp[A.num];
   long long blocks = (warps + 7) / 8;     // 8 warps per block
-  if (blocks > 148LL * 64) blocks = 148LL * 64;
+  if (blocks > (long long)kNumSMs * 64) blocks = (long long)kNumSMs * 64;
   epe::epe_backward_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(flow, mask, A, eps, q, grad_loss, mask_sum, N, H, W);
   return check_launch("epe_backward_kernel");
 }

@@ -44,16 +44,16 @@ __host__ __device__ __forceinline__ int swz(int p, int c) { return p * PXB + ((c
 __host__ __device__ constexpr int cout_pad(int cout) { return cout <= 32 ? 32 : (cout <= 64 ? 64 : (cout <= 96 ? 96 : 128)); }
 }  // namespace c3
 
-// tcgen05 / TMEM implementation of the same convolution (conv3x3_umma.cu); its weight image follows the mma.sync image
-// inside the packed buffer.  conv3x3_umma_launch returns -1 when the shape does not fit (caller falls back).
+// wgmma implementation of the same convolution (conv3x3_wgmma.cu); its weight image follows the mma.sync image
+// inside the packed buffer.  conv3x3_wgmma_launch returns -1 when the shape does not fit (caller falls back).
 long long conv3x3_sync_packed_bytes(int Cin, int Cout);
-long long conv3x3_umma_packed_bytes(int Cin, int Cout);
-int conv3x3_umma_pack(const float* weight, unsigned char* packed, int Cin, int Cout, cudaStream_t st);
-int conv3x3_umma_launch(const float* x, long long x_bs, const unsigned char* wpack, const float* bias, float* out,
+long long conv3x3_wgmma_packed_bytes(int Cin, int Cout);
+int conv3x3_wgmma_pack(const float* weight, unsigned char* packed, int Cin, int Cout, cudaStream_t st);
+int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wpack, const float* bias, float* out,
                         long long out_bs, int N, int Cin, int H, int W, int Cout, int stride, int dil, int out_mode,
                         float slope, cudaStream_t st, int ext = 0, float* ws = nullptr, long long ws_bytes = 0);
 // split-K over the input-channel chunks for layers with fewer tiles than SMs: the plan (1 = none) and the fp32 workspace
-// the caller has to lend to conv3x3_umma_launch for it
-long long conv3x3_umma_workspace_bytes(int N, int Cin, int H, int W, int Cout, int stride, int dil);
+// the caller has to lend to conv3x3_wgmma_launch for it
+long long conv3x3_wgmma_workspace_bytes(int N, int Cin, int H, int W, int Cout, int stride, int dil);
 
 }  // namespace mfn

@@ -116,7 +116,7 @@ __global__ void scale_kernel(float* v, int n, float s) {
 
 static inline unsigned grid_of(long long total) {
   long long b = (total + 255) / 256;
-  return (unsigned)(b < 1 ? 1 : (b > 148LL * 32 ? 148LL * 32 : b));
+  return (unsigned)(b < 1 ? 1 : (b > (long long)kNumSMs * 32 ? (long long)kNumSMs * 32 : b));
 }
 
 }  // namespace mfn
@@ -133,7 +133,7 @@ extern "C" int mfn_preprocess_forward(const void* img1, const void* img2, int is
   const int planes = N * C;
   cudaError_t ce = cudaMemsetAsync(rgb_mean, 0, sizeof(float) * planes, st);
   if (ce != cudaSuccess) return fail((int)ce, "mfn_preprocess_forward: cudaMemsetAsync: %s", cudaGetErrorString(ce));
-  int slices = (148 * 4 + planes - 1) / planes;
+  int slices = (kNumSMs * 4 + planes - 1) / planes;
   if (slices < 1) slices = 1;
   // rgb_mean first accumulates the per-plane sums (atomics over `slices` partial sums), is read as such by the resampling
   // kernel, and is turned into the means by a last tiny launch

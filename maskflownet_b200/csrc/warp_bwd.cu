@@ -1,4 +1,4 @@
-// warp_bwd.cu -- backward of the flow-guided feature warp (K4) for sm_100a.
+// warp_bwd.cu -- backward of the flow-guided feature warp (K4) for sm_90a.
 //
 // Serves mfn_deformable_conv_backward and mfn_warp_mask_backward: the gradients that the reference obtains from
 // autograd through  F.contrib.DeformableConvolution (network/layer.py:117-124), the `repeat` that builds its offsets

@@ -1,5 +1,5 @@
 // warp_fwd.cu -- flow-guided feature warp forward kernels (K3), Upsample, GridGenerator/BilinearSampler and the
-// fused cascade-input builder (K5) for sm_100a.
+// fused cascade-input builder (K5) for sm_90a.
 //
 // K3 serves two entry points with one kernel template:
 //   mfn_deformable_conv_forward  F.contrib.DeformableConvolution(x, offset, weight[, bias])   network/layer.py:117-124
@@ -474,7 +474,7 @@ extern "C" int mfn_warp_mask_forward(const float* x, const float* flow_coarse, c
 // `repeat`-ed over the taps, network/MaskFlownet.py:228-232), and bilinear sampling is linear in the image, hence
 //     sum_tap W_tap . S(p + tap + f(p))  =  bilinear sample at p + f(p) of  Y = conv3x3(x, W)   (zero padding)
 // wherever the nine samples fall strictly inside the image.  The fused warp is therefore
-//   (1) Y = plain 3x3 convolution on the tensor cores (conv3x3_umma.cu),
+//   (1) Y = plain 3x3 convolution on the tensor cores (conv3x3_wgmma.cu),
 //   (2) warp_resample_kernel: per pixel up-sample flow / mask, sample Y, + bias, x sigmoid(mask), + trade-off, LeakyReLU,
 //   (3) deform_fwd_kernel over a pixel list: the frame of pixels whose warped centre is within two pixels of the image
 //       border, where the operator's border rules (MFN_BORDER_*) are not linear, computed tap by tap as before (the list is
@@ -592,7 +592,7 @@ extern "C" int mfn_warp_mask_forward_resample(const float* x, const float* flow_
   // (2) interior (and far-outside) pixels; builds the border list
   const long long total = (long long)N * H * W;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > (long long)kNumSMs * 16) blocks = (long long)kNumSMs * 16;
   warp_resample_kernel<<<(unsigned)blocks, 256, 0, st>>>(conv_ws, flow_coarse, mask_coarse, bias, tradeoff, out, flow_up_out,
                                                         mask_up_out, pix_list, pix_count, N, H, W, F, upsample_factor,
                                                         flow_scale, level_stride, leaky_slope);

@@ -12,7 +12,7 @@
 //                                                            a_D(h) = 0 elsewhere.
 // Summing over the taps with the weights W_ij:
 //   Z x Z : bilinear sample at (y + dy, x + dx) of Yext = conv3x3(x, W) evaluated on the grid extended by one pixel per side
-//           (tcgen05 kernel, conv3x3_umma.cu with ext = 1) -- all of the operator in zero-corner mode;
+//           (wgmma kernel, conv3x3_wgmma.cu with ext = 1) -- all of the operator in zero-corner mode;
 //   D x Z : sum_i alpha_i * lerp_w( Rrow[B_i][i] )   with Rrow[B][i] = conv1d(x[row B], W[i, :]) on the extended row,
 //   Z x D : sum_j beta_j  * lerp_h( Rcol[B_j][j] )   with Rcol[B][j] = conv1d(x[:, col B], W[:, j]),
 //   D x D : sum_ij alpha_i beta_j T[B_i][B_j][i][j]  with T = W_ij . x[:, row B_i, col B_j]
@@ -52,7 +52,7 @@ __device__ __forceinline__ Band bands(int p, float d, int n) {
   return b;
 }
 
-// Yall = conv3x3_umma(ext = 2): (N, F, H + 8, W + 8); entry (r, v) <-> position (r - 1, v - 1) of the virtual image
+// Yall = conv3x3_wgmma(ext = 2): (N, F, H + 8, W + 8); entry (r, v) <-> position (r - 1, v - 1) of the virtual image
 //   rows 0 .. H+1, cols 0 .. W+1   Yext (the extended convolution)
 //   rows H+4-i / H+7-i             the 1-D convolution of the first / last image row with weight row i   (Rrow)
 //   cols W+4-j / W+7-j             ... of the first / last image column with weight column j               (Rcol)
@@ -156,8 +156,8 @@ __global__ void __launch_bounds__(256)
     }
     const bool warp_bands = BORDER == MFN_BORDER_MXNET15 && __any_sync(__activemask(), bh.any || bw.any);
     // branch-free channel loop: the corner offsets are clamped into the array and the weights of out-of-range corners are
-    // zero, so every load is legal and the loads of eight channels are issued before the first use (the first version, with
-    // per-channel band tests, executed 534 instructions per channel and warp: profiles/r02_ncu_warp_lin_L3_summary.txt)
+    // zero, so every load is legal and the loads of eight channels are issued before the first use (per-channel band tests
+    // multiplied the instructions per channel)
     const int nf = f1 - f0;
 #pragma unroll 1
     for (int fb = 0; fb < nf; fb += 8) {
@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(256)
 
 long long warp_lin_workspace_bytes(int N, int F, int H, int W) { return (long long)N * F * (H + 8) * (W + 8) * 4 + 64; }
 
-// returns -1 when the extended tcgen05 convolution does not fit the shape (caller uses the list-based path)
+// returns -1 when the extended wgmma convolution does not fit the shape (caller uses the list-based path)
 int launch_warp_lin(const float* x, const float* flow_c, const float* mask_c, const float* weight, const void* packed_weight,
                     const float* bias, const float* tradeoff, void* workspace, float* out, float* fup, float* mup, int N,
                     int C, int H, int W, int F, int up, float fs, float ls, float slope, int border_mode, cudaStream_t st) {
@@ -204,16 +204,16 @@ int launch_warp_lin(const float* x, const float* flow_c, const float* mask_c, co
   const unsigned char* wp = static_cast<const unsigned char*>(packed_weight);
   // zero-corner rule: the extended convolution alone (grid + 1 pixel per side); MXNet-1.5 rule: + the band rows / columns
   const int ext = border_mode == MFN_BORDER_MXNET15 ? 2 : 1, grow = ext == 2 ? 8 : 2;
-  int rc = conv3x3_umma_launch(x, (long long)C * H * W, wp + conv3x3_sync_packed_bytes(C, F), nullptr, Yall,
+  int rc = conv3x3_wgmma_launch(x, (long long)C * H * W, wp + conv3x3_sync_packed_bytes(C, F), nullptr, Yall,
                                (long long)F * (H + grow) * (W + grow), N, C, H, W, F, 1, 1, MFN_CONV_OUT_NCHW, 1.0f, st, ext);
   if (rc) return rc;
   const long long total = (long long)N * H * W;
   if (total >= (1LL << 31)) return -1;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 8) blocks = 148LL * 8;
-  // channels per thread: doubled while at least one resident wave of threads (148 SMs x 512) remains
+  if (blocks > (long long)kNumSMs * 8) blocks = (long long)kNumSMs * 8;
+  // channels per thread: doubled while at least one resident wave of threads (one per SM x 512) remains
   int fch = FCH;
-  while (fch < 64 && fch < F && total * ((F + 2 * fch - 1) / (2 * fch)) >= 148LL * 512) fch *= 2;
+  while (fch < 64 && fch < F && total * ((F + 2 * fch - 1) / (2 * fch)) >= (long long)kNumSMs * 512) fch *= 2;
   if (tuning().warp_lin_fch > 0) fch = tuning().warp_lin_fch;
   const dim3 grid((unsigned)blocks, (unsigned)((F + fch - 1) / fch));
   if (border_mode == MFN_BORDER_MXNET15)

@@ -4,7 +4,7 @@ forward (replicas), and ONE flattened fp32 gradient all-reduce per training step
 Mirrors what the reference does implicitly with gluon: `split_and_load` over ctx (network/pipeline.py:95,173,206) and
 `trainer.step(batch_size)` (:114), whose kvstore('device') sums each parameter's gradient across GPUs and rescales by
 1/batch_size.  Here: torch.distributed (NCCL over NVLink on the GPU box, gloo in CPU tests) on a single bucket
-(MaskFlownet-S: 10,514,256 floats = 42 MB), which a ring/NVLS all-reduce on 8 B200s moves in about 0.1 ms -- so it is
+(MaskFlownet-S: 10,514,256 floats = 42 MB), small enough for one all-reduce per step -- so it is
 neither fused into a kernel nor split into per-layer buckets (SURVEY.md section 5).
 """
 from __future__ import annotations

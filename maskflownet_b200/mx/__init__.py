@@ -11,7 +11,7 @@ tensors so that `network/MaskFlownet.py` and `network/layer.py` import and run U
     preds, masks, srcs = net(mx.nd.array(img1), mx.nd.array(img2))
 
 The four hot operators -- F.Correlation, F.contrib.DeformableConvolution, F.GridGenerator, F.BilinearSampler -- dispatch
-to the hand-written sm_100a kernels through maskflownet_b200.ops (no fallback: they raise without a CUDA device).  The
+to the hand-written sm_90a kernels through maskflownet_b200.ops (no fallback: they raise without a CUDA device).  The
 remaining generic tensor helpers (concat, reshape codes, pad, Convolution/Deconvolution used by the reference's own
 Upsample block, ...) map onto torch, which is the allocator/plumbing layer here.
 """

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's model graphs, calling the fused B200 operators.
+"""Host-side mirror of the reference's model graphs, calling the fused CUDA operators.
 
 `MaskFlownetS` computes what `MaskFlownet_S.hybrid_forward` computes (network/MaskFlownet.py:197-315) and
 `MaskFlownet` what the cascade computes (:443-545), but is organised around the hot path instead of transcribing the
@@ -11,8 +11,8 @@ unrolled reference code: one loop over pyramid levels in which
     Upsample(4) + GridGenerator + BilinearSampler + sigmoid-0.5 + concat (:308-313)
                                                                     -> one launch of ops.image_warp_concat (K5)
 
-The dense 3x3 / transposed convolutions (about 98 % of the FLOPs, SURVEY.md section 0.4; row N2) run on the tcgen05 / TMEM
-kernel of csrc/conv3x3_umma.cu: f32 in / out, bf16 hi+lo split operands, fp32 accumulation.  At inference (`_fast`) with
+The dense 3x3 / transposed convolutions (about 98 % of the FLOPs, SURVEY.md section 0.4; row N2) run on the wgmma
+kernel of csrc/conv3x3_wgmma.cu: f32 in / out, bf16 hi+lo split operands, fp32 accumulation.  At inference (`_fast`) with
 in-place concat buffers and fused heads; with gradients enabled (`train_tc_forward`, default) every 3x3 convolution still
 runs its FORWARD on that kernel and its backward through aten.convolution_backward (ops.conv3x3_train), the transposed
 convolutions and the concats through torch autograd.  Sub-module names equal the reference's gluon prefixes (conv1a ... deform5, conv5f,
@@ -88,9 +88,9 @@ class _FlowNetBase(nn.Module):
     fuse_heads = True   # inference: pred_flow / pred_mask over the block input ride on conv{L}_4's input pass
     use_resample_warp = True   # inference: K3 through linearity (ops.warp_mask(resample=True)) at every level
     use_tc_conv = True   # inference: decoder / context 3x3 convolutions on the fp32-accurate tensor-core kernel (row N2)
-    # training (grad enabled): the 3x3 convolutions still run their FORWARD on the tcgen05 kernel (ops.conv3x3_train: bias +
+    # training (grad enabled): the 3x3 convolutions still run their FORWARD on the wgmma kernel (ops.conv3x3_train: bias +
     # LeakyReLU fused, the output doubles as the activation mask), the BACKWARD is aten.convolution_backward (cuDNN fp32).
-    # Measured on BASELINE configs[2] (batch 8, 512x384, fwd + bwd): 66.4 -> 52.7 ms per step.  False: cuDNN both ways.
+    # False: cuDNN both ways.
     train_tc_forward = True
 
     def _packed(self, name):
@@ -191,7 +191,7 @@ class _FlowNetBase(nn.Module):
 
     def _pyramid(self, x, names):
         """Six levels of (3x3 stride-2, 3x3, 3x3) convolutions + LeakyReLU (network/MaskFlownet.py:200-202).  Inference:
-        all eighteen run on the tcgen05 convolution kernel (bias + activation fused)."""
+        all eighteen run on the wgmma convolution kernel (bias + activation fused)."""
         feats = []
         fast = self._fast(x)
         for lvl in range(1, 7):
@@ -365,7 +365,7 @@ class MaskFlownetS(_FlowNetBase):
             warp, flow_up, _ = ops.warp_mask(c2[lvl - 1], flow, mask, dp.weight, dp.bias, trade, self.scale,
                                              float(STRIDES[lvl]), 2, SLOPE, self.border_mode,
                                              # inference: every level is evaluated exactly through linearity (extended 3x3
-                                             # convolution on tcgen05 + bilinear re-sampling + border-band tables, warp_lin.cu)
+                                             # convolution on wgmma + bilinear re-sampling + border-band tables, warp_lin.cu)
                                              packed_weight=self._packed(f"deform{lvl}") if self._fast(flow) else None,
                                              resample=self.use_resample_warp)
             if self.event_hook is not None:
@@ -531,7 +531,7 @@ class PipelinedFlowPredictor:
         pinned uint8 images --H2D (copy stream)--> staging --D2D--> graph inputs --graph replay--> flow --D2D--> staging
         --D2H (copy stream)--> pinned fp32 flow
     with `depth` staging slots, so the H2D copy of request i+1 and the D2H copy of result i-1 run under the forward of
-    request i (PCIe is full duplex; 22 MB in / 29 MB out per batch of 8 at 1024x448 take ~0.4 / ~0.5 ms of a ~9 ms forward).
+    request i (PCIe is full duplex; 22 MB in / 29 MB out per batch of 8 at 1024x448).
     Results are complete after synchronize() (or after waiting on the event infer() returns)."""
 
     def __init__(self, net: nn.Module, depth: int = 2):

@@ -1,4 +1,4 @@
-"""Tensor-level operators of the MaskFlownet hot path, backed by libmaskflow_b200.so (hand-written sm_100a CUDA).
+"""Tensor-level operators of the MaskFlownet hot path, backed by libmaskflow_b200.so (hand-written sm_90a CUDA).
 
 Every function takes / returns torch CUDA float32 NCHW tensors and mirrors one MXNet operator (or one fused group of
 them) used by the reference; keyword names follow the MXNet operators so that the `F` shim in maskflownet_b200.mx can
@@ -250,7 +250,7 @@ def warp_mask(x, flow_coarse, mask_coarse, weight, bias=None, tradeoff=None, sca
     """Fused Upsample(up)(flow, mask) -> deformable conv (all taps offset by flow*scale/stride) -> *sigmoid(mask)
     -> + tradeoff -> LeakyReLU.   Returns (warp, flow_up, mask_up or None).
     packed_weight (ops.conv3x3_pack(weight)) selects a tensor-core path when no gradient is required: with resample=True
-    the operator is evaluated through linearity (plain 3x3 convolution on tcgen05 + bilinear re-sampling of its output +
+    the operator is evaluated through linearity (plain 3x3 convolution on wgmma + bilinear re-sampling of its output +
     tap-by-tap border frame, mfn_warp_mask_forward_resample), else the gather-then-mma.sync kernel (F <= 128)."""
     x = _chk(x, "warp_mask.x")
     fc = _chk(flow_coarse, "warp_mask.flow_coarse")
@@ -468,9 +468,9 @@ def conv3x3(x: torch.Tensor, packed: torch.Tensor, bias: Optional[torch.Tensor],
 
 
 class _Conv3x3TrainFn(torch.autograd.Function):
-    """Training-mode 3x3 convolution (+ bias + LeakyReLU): FORWARD on the tcgen05 kernel (the same launch inference uses),
+    """Training-mode 3x3 convolution (+ bias + LeakyReLU): FORWARD on the wgmma kernel (the same launch inference uses),
     BACKWARD through aten.convolution_backward (cuDNN dgrad / wgrad -- this library has no convolution backward kernels,
-    DESIGN.md section 7).  The activation's backward uses the saved OUTPUT (y > 0  <=>  pre-activation > 0 for slope > 0)."""
+    cuDNN's backward).  The activation's backward uses the saved OUTPUT (y > 0  <=>  pre-activation > 0 for slope > 0)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, packed, slope, dilation, stride):

@@ -72,19 +72,21 @@ def test_argument_errors_need_no_gpu():
 
 
 def test_conv_split_plan_is_host_arithmetic():
-    """mfn_conv3x3_workspace_bytes is pure host arithmetic (no GPU): the split-K plan of the tcgen05 convolution for the
-    shapes of BASELINE configs[1] (csrc/conv3x3_umma.cu: plan_split)."""
+    """mfn_conv3x3_workspace_bytes is pure host arithmetic (no GPU): the split-K plan of the wgmma convolution for the
+    shapes of BASELINE configs[1] (csrc/conv3x3_wgmma.cu: plan_split)."""
     L = _lib.lib()
     wb = L.mfn_conv3x3_workspace_bytes
-    # level 6 (7x16, N=8: 32 tiles): every tile split into min(148 // 32, 34 // 3, 8) = 4 parts over the whole tensor
+    # level 6 (7x16, N=8: 32 tiles): every tile split into min(132 // 32, 34 // 3, 8) = 4 parts over the whole tensor
     assert wb(8, 529, 7, 16, 64, 1, 1) == 4 * 8 * 64 * 7 * 16 * 4
     # level 5 (14x32, N=8: 56 tiles): 2 parts
     assert wb(8, 675, 14, 32, 64, 1, 1) == 2 * 8 * 64 * 14 * 32 * 4
-    # level 2, long tensor-bound layer: 896 tiles = 6 x 148 + 8 -> the last 8 tiles (8 rows of the last sample) in 18 parts
-    assert wb(8, 579, 112, 256, 128, 1, 1) == 18 * 1 * 128 * 8 * 256 * 4
+    # level 2, long tensor-bound layer at batch 6: 672 tiles = 5 x 132 + 12 -> the last 12 tiles (12 rows of the last
+    # sample) in min(132 // 12, 37 // 2) = 11 parts; at batch 8 (896 = 6 x 132 + 104) the last round is nearly full: no split
+    assert wb(6, 579, 112, 256, 128, 1, 1) == 11 * 1 * 128 * 12 * 256 * 4
+    assert wb(8, 579, 112, 256, 128, 1, 1) == 0
     # same geometry but few chunks / narrow output: not worth a second launch
-    assert wb(8, 128, 112, 256, 128, 1, 1) == 0
-    assert wb(8, 547, 112, 256, 34, 1, 1) == 0
+    assert wb(6, 128, 112, 256, 128, 1, 1) == 0
+    assert wb(6, 547, 112, 256, 34, 1, 1) == 0
     # levels 3 and 4 (224 / 112 tiles), the pyramid (thousands of tiles) and nonsense arguments: never split
     assert wb(8, 419, 56, 128, 96, 1, 1) == 0 and wb(8, 451, 28, 64, 96, 1, 1) == 0
     assert wb(16, 16, 224, 512, 16, 1, 1) == 0 and wb(16, 3, 448, 1024, 16, 2, 1) == 0

@@ -407,13 +407,13 @@ def test_conv3x3_dilated(dil):
     assert np.abs(got - ref).max() <= 1e-4 * max(1.0, float(np.abs(ref).max()))
 
 
-@pytest.mark.parametrize("umma", [1, 0])
+@pytest.mark.parametrize("wg", [1, 0])
 @pytest.mark.parametrize("N,Cin,Cout,H,W,dil", [(1, 16, 32, 4, 128, 1), (1, 32, 64, 5, 130, 1), (1, 64, 96, 9, 256, 1),
                                                 (2, 131, 128, 12, 40, 1), (1, 40, 96, 21, 45, 2), (1, 40, 64, 21, 45, 16),
                                                 (1, 128, 128, 30, 200, 8), (1, 20, 2, 9, 140, 1), (1, 33, 16, 6, 70, 1),
                                                 (1, 300, 128, 9, 140, 1), (2, 260, 96, 7, 40, 2)])
-def test_conv3x3_tcgen05_and_mma_sync_agree_with_fp64(N, Cin, Cout, H, W, dil, umma):
-    """Both kernels behind mfn_conv3x3_forward (tcgen05/TMEM and mma.sync) against a float64 convolution, incl. tiles that
+def test_conv3x3_tcgen05_and_mma_sync_agree_with_fp64(N, Cin, Cout, H, W, dil, wg):
+    """Both kernels behind mfn_conv3x3_forward (wgmma and mma.sync) against a float64 convolution, incl. tiles that
     straddle the 128-pixel M tile, the image border, channel-chunk padding and N padding."""
     rng = np.random.default_rng(41)
     x = feat(rng, (N, Cin, H, W))
@@ -422,13 +422,13 @@ def test_conv3x3_tcgen05_and_mma_sync_agree_with_fp64(N, Cin, Cout, H, W, dil, u
     ref = torch.nn.functional.conv2d(torch.from_numpy(x).double(), torch.from_numpy(w).double(),
                                      torch.from_numpy(b).double(), padding=dil, dilation=dil)
     ref = torch.nn.functional.leaky_relu(ref, 0.1).float().numpy()
-    _lib.set_tuning("conv_umma", umma)
+    _lib.set_tuning("conv_wgmma", wg)
     try:
         got = ops.conv3x3(cu(x), ops.conv3x3_pack(cu(w)), cu(b), Cout, 0.1, dilation=dil).cpu().numpy()
         kern = _lib.last_kernel()
     finally:
-        _lib.set_tuning("conv_umma", 1)
-    assert ("umma" in kern) == bool(umma), kern
+        _lib.set_tuning("conv_wgmma", 1)
+    assert ("wgmma" in kern) == bool(wg), kern
     assert np.abs(got - ref).max() <= 1e-4 * max(1.0, float(np.abs(ref).max())), kern
 
 
@@ -436,7 +436,7 @@ def test_conv3x3_tcgen05_and_mma_sync_agree_with_fp64(N, Cin, Cout, H, W, dil, u
                                             (1, 128, 196, 6, 12), (1, 4, 16, 5, 7)])
 def test_conv3x3_stride2_pyramid(N, Cin, Cout, H, W):
     """conv{L}a / conv{L}x of the feature pyramid: 3x3, stride 2, pad 1 (network/MaskFlownet.py:147-165), odd and even
-    extents, and the 196-channel level-6 layer (wider than one mma.sync CTA covers: tcgen05 image only)."""
+    extents, and the 196-channel level-6 layer (wider than one mma.sync CTA covers: wgmma image only)."""
     rng = np.random.default_rng(43)
     x = feat(rng, (N, Cin, H, W))
     w = (rng.standard_normal((Cout, Cin, 3, 3)) * np.sqrt(2.0 / (9 * Cin))).astype(np.float32)
@@ -447,7 +447,7 @@ def test_conv3x3_stride2_pyramid(N, Cin, Cout, H, W):
     got = ops.conv3x3(cu(x), ops.conv3x3_pack(cu(w)), cu(b), Cout, 0.1, stride=2).cpu().numpy()
     assert got.shape == ref.shape
     assert np.abs(got - ref).max() <= 1e-4 * max(1.0, float(np.abs(ref).max())), _lib.last_kernel()
-    # the same layer at stride 1 (196 outputs exist only in the tcgen05 weight image)
+    # the same layer at stride 1 (196 outputs exist only in the wgmma weight image)
     ref1 = torch.nn.functional.leaky_relu(torch.nn.functional.conv2d(
         torch.from_numpy(x).double(), torch.from_numpy(w).double(), torch.from_numpy(b).double(), padding=1), 0.1).float().numpy()
     got1 = ops.conv3x3(cu(x), ops.conv3x3_pack(cu(w)), cu(b), Cout, 0.1).cpu().numpy()
@@ -516,12 +516,12 @@ def test_conv3x3_split_k_small_levels(N, Cin, Cout, H, W, mode):
 
 
 @pytest.mark.parametrize("mode", ["nchw", "lin3", "d2s"])
-@pytest.mark.parametrize("N,Cin,Cout,H,W,cap", [(2, 250, 96, 14, 130, 12), (3, 260, 68, 9, 300, 20), (3, 259, 96, 112, 256, 0)])
+@pytest.mark.parametrize("N,Cin,Cout,H,W,cap", [(2, 250, 96, 14, 130, 12), (3, 260, 68, 9, 300, 20), (1, 259, 96, 272, 256, 0)])
 def test_conv3x3_split_k_last_round(N, Cin, Cout, H, W, cap, mode):
-    """Tiles are indivisible units of a persistent grid: when the last round is short (level 2: 896 tiles = 6 x 148 + 8) only
-    the left-over tiles are split over the channel chunks, the others run whole in the same launch; a second launch reduces
+    """Tiles are indivisible units of a persistent grid: when the last round is short (level 2 at batch 6 on 132 SMs: 672
+    tiles = 5 x 132 + 12) only the left-over tiles are split over the channel chunks, the others run whole in the same launch; a second launch reduces
     the tail's row range (long layers only: >= 16 chunks, Cout > 64).  Small grids (conv_grid_cap) reproduce the situation
-    cheaply; the last case is the level-2 geometry at batch 3 (336 tiles = 2 x 148 + 40).  Against float64 and against the unsplit kernel, for the three epilogues."""
+    cheaply; the last case fills a whole 132-SM grid (272 tiles = 2 x 132 + 8).  Against float64 and against the unsplit kernel, for the three epilogues."""
     rng = np.random.default_rng(59)
     x = feat(rng, (N, Cin, H, W))
     w = (rng.standard_normal((Cout, Cin, 3, 3)) * np.sqrt(2.0 / (9 * Cin))).astype(np.float32)
@@ -562,8 +562,8 @@ def test_conv3x3_split_k_last_round(N, Cin, Cout, H, W, cap, mode):
 
 @pytest.mark.parametrize("cap", [1, 3])
 def test_conv3x3_persistent_tile_loop(cap):
-    """The tcgen05 kernel is persistent: with the grid capped every CTA walks many tiles (stage rings wrap, barrier
-    parities flip, TMEM accumulators alternate); results must not depend on the grid size."""
+    """The wgmma kernel is persistent: with the grid capped every CTA walks many tiles (stage rings wrap, barrier
+    parities flip); results must not depend on the grid size."""
     rng = np.random.default_rng(49)
     N, Cin, Cout, H, W = 2, 50, 64, 13, 150
     x = feat(rng, (N, Cin, H, W))
@@ -585,7 +585,7 @@ def test_conv3x3_persistent_tile_loop(cap):
                                               (2, 128, 14, 32, 0.6), (1, 96, 28, 64, 2.5), (1, 8, 4, 6, 0.8)])
 def test_warp_mask_through_linearity_matches_tap_by_tap(N, C, H, W, flow_mag, border, lin):
     """mfn_warp_mask_forward_resample == the oracle's deformable convolution, both border rules, flows from sub-pixel to far
-    outside the image.  lin=1: every pixel through linearity (extended tcgen05 convolution + band tables, warp_lin.cu);
+    outside the image.  lin=1: every pixel through linearity (extended wgmma convolution + band tables, warp_lin.cu);
     lin=0: the round-1 path (plain convolution + re-sampling + tap-by-tap border list)."""
     rng = np.random.default_rng(53)
     x = feat(rng, (N, C, H, W))

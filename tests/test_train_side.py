@@ -1,4 +1,4 @@
-"""The training-side rows of SURVEY.md 8f: N4, GPU-side augmentation (/root/reference/augmentation.py:168-339), and the fused
+"""The training-side rows of SURVEY.md 8f: N4, GPU-side augmentation (the reference's augmentation.py:168-339), and the fused
 MultiscaleEpe of row N2 (network/MaskFlownet.py:563-611).
 
 CPU part (`-m "not gpu"`): the numpy restatement (oracle/augment_ref.py) against the fixture produced by the reference's own
@@ -463,7 +463,7 @@ def test_conv3x3_train_matches_cudnn_autograd():
         assert err < 1e-4 * max(1.0, ref.abs().max().item()), (Cin, Cout, dil, stride, err, ref.abs().max().item())
         # backward: the same activation mask on both sides (ours comes from the saved output; a pre-activation within the
         # forward's 1e-5 of zero may legitimately fall on the other side of the LeakyReLU kink in the cuDNN forward, which
-        # moves single weight-gradient entries by O(|g x|) -- seen on the B200: 1 of 98 k outputs flipped), so the
+        # moves single weight-gradient entries by O(|g x|) -- seen on the GPU: 1 of 98 k outputs flipped), so the
         # reference is the LINEAR convolution's autograd fed with the masked gradient
         g = torch.randn_like(ref)
         wrt = [w, b] + ([x] if x.requires_grad else [])
@@ -576,12 +576,14 @@ def test_pipeline_host_plumbing_on_cpu(monkeypatch):
         pipe.fix_head()                      # only the cascade has a head to freeze
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/weights/dbbSep30-1206_1000000.params"), reason="shipped checkpoints not on this box")
-def test_pipeline_load_head_and_fix_head_on_cpu():
-    """main.py:133-139: a MaskFlownet-S checkpoint goes into the cascade's head (load_head), which is then frozen (fix_head);
-    the trainer only keeps the cascade's own parameters."""
+def test_pipeline_load_head_and_fix_head_on_cpu(tmp_path):
+    """main.py:133-139: a MaskFlownet-S checkpoint (the layout of the shipped dbbSep30-1206_1000000, rebuilt from
+    tests/golden/checkpoints.npz) goes into the cascade's head (load_head), which is then frozen (fix_head); the trainer
+    only keeps the cascade's own parameters."""
+    from golden.ckpt import write_checkpoint
     from maskflownet_b200 import params as mparams, pipeline
-    ck = "/root/reference/weights/dbbSep30-1206_1000000.params"
+    ck = str(tmp_path / "s.params")
+    write_checkpoint(ck, "s")
     pipe = pipeline.PipelineFlownet(device="cpu", network_class="MaskFlownet")
     pipe.load_head(ck)
     raw = mparams.read_params(ck)
