@@ -198,6 +198,21 @@ MFN_API int mfn_grid_generator_warp_forward(const float* flow_xy, float* grid, i
 MFN_API int mfn_bilinear_sampler_forward(const float* data, const float* grid, float* out, int N, int C,
                                  int H, int W, int OH, int OW, void* stream);
 
+/* GridGenerator('warp') backward: grad_flow (N,2,H,W) overwritten,
+ * channel 0 = grad_grid[:,0] * 2/(W-1), channel 1 = grad_grid[:,1] * 2/(H-1). */
+MFN_API int mfn_grid_generator_warp_backward(const float* grad_grid, float* grad_flow, int N, int H, int W,
+                                             void* stream);
+
+/* BilinearSampler backward (MXNet BilinearSamplerBackward; equal to torch grid_sample(bilinear, zeros,
+ * align_corners=True) backward).  grad_out (N,C,OH,OW); data, grid as in the forward.
+ *   grad_data (N,C,H,W) ACCUMULATED (caller zero-fills, atomics) or NULL;
+ *   grad_grid (N,2,OH,OW) overwritten (no atomics, bit-reproducible) or NULL.
+ * A corner outside the image reads 0 and receives no data gradient; at integer sample positions the position
+ * derivative is the one from the floor side. */
+MFN_API int mfn_bilinear_sampler_backward(const float* grad_out, const float* data, const float* grid,
+                                          float* grad_data, float* grad_grid, int N, int C, int H, int W, int OH,
+                                          int OW, void* stream);
+
 /* Fused cascade-input builder.  replaces: network/MaskFlownet.py:308-313
  *     mask0 = sigmoid(Upsample(4)(mask2)) - 0.5
  *     c40   = concat( warp(im2, Upsample(4)(flow2)*scale), mask0 )       [layer.py:8-18]
@@ -207,6 +222,18 @@ MFN_API int mfn_bilinear_sampler_forward(const float* data, const float* grid, f
 MFN_API int mfn_image_warp_concat_forward(const float* im1, const float* im2, const float* flow_q,
                                   const float* mask_q, float* c30, float* c40, int N, int Ci, int H,
                                   int W, float flow_scale, void* stream);
+
+/* Backward of mfn_image_warp_concat_forward with respect to c40 (grad_c40 (N,Ci+1,H,W); the gradient of c30 with
+ * respect to im1 is its first Ci channels).
+ *   grad_flow_up (N,2,H,W) (y,x), overwritten or NULL: gradient w.r.t. Upsample(4)(flow_q), flow_scale included;
+ *   grad_mask_up (N,1,H,W), overwritten or NULL: grad_c40[:,Ci] * sigmoid'(Upsample(4)(mask_q));
+ *   grad_im2 (N,Ci,H,W) ACCUMULATED (caller zero-fills, atomics) or NULL.
+ * grad_flow_up and grad_mask_up use no atomics (bit-reproducible).  The transposed Upsample(4) to (N,2|1,H/4,W/4) is
+ * mfn_upsample_backward, as for mfn_warp_mask_backward. */
+MFN_API int mfn_image_warp_concat_backward(const float* grad_c40, const float* im2, const float* flow_q,
+                                           const float* mask_q, float* grad_im2, float* grad_flow_up,
+                                           float* grad_mask_up, int N, int Ci, int H, int W, float flow_scale,
+                                           void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Decoder dense-block convolution (SURVEY.md section 8f, row N2).

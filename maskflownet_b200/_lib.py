@@ -33,6 +33,9 @@ SIGNATURES = {
     "mfn_grid_generator_warp_forward": [_f, _f, _i, _i, _i, _f],
     "mfn_bilinear_sampler_forward": [_f, _f, _f, _i, _i, _i, _i, _i, _i, _f],
     "mfn_image_warp_concat_forward": [_f] * 6 + [_i] * 4 + [_fl, _f],
+    "mfn_grid_generator_warp_backward": [_f, _f, _i, _i, _i, _f],
+    "mfn_bilinear_sampler_backward": [_f] * 5 + [_i] * 6 + [_f],
+    "mfn_image_warp_concat_backward": [_f] * 7 + [_i] * 4 + [_fl, _f],
     "mfn_preprocess_forward": [_f, _f, _i, _f, _f, _f, _i, _i, _i, _i, _i, _i, _f],
     "mfn_postprocess_forward": [_f, _f, _i, _i, _i, _i, _i, _i, _i, _i, _f],
     "mfn_geometry_augment_forward": [_f, _f, _i, _f, _f, _i, _f, _f, _f, _f, _f, _i, _i, _i, _i, _i, _f],

@@ -5,6 +5,7 @@
 
 #include "../../include/maskflow_b200.h"
 #include "device_caps.h"
+#include "sampling.cuh"
 
 namespace mfn {
 
@@ -43,6 +44,13 @@ static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStre
 
 static inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
 
+// blocks of a grid-stride element-wise launch: enough for `total` items, at most 16 per SM
+static inline unsigned grid_for(long long total, int threads) {
+  long long b = (total + threads - 1) / threads;
+  const long long cap = (long long)kNumSMs * 16;
+  return (unsigned)(b < cap ? (b > 0 ? b : 1) : cap);
+}
+
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per function AND per device (a process may drive several GPUs: ops._call
 // switches the device per tensor): remember the largest opt-in per device, re-issue it when a launch needs more.
@@ -76,28 +84,7 @@ int launch_corr_tma(int md, const float* d1, const float* d2, float* out, int N,
 // ---- device helpers ---------------------------------------------------------------------------------
 __device__ __forceinline__ float leaky(float v, float slope) { return v > 0.f ? v : v * slope; }
 
-__device__ __forceinline__ float sigmoidf_(float v) { return 1.f / (1.f + __expf(-v)); }
-
-// Upsample(f) taps along one axis (network/MaskFlownet.py:35-62): output index o = f*i + r reads
-// in[i]*(1-r/f) + in[min(i+1, n-1)]*(r/f).
-__device__ __forceinline__ void upsample_taps(int o, int f, int n, int& i0, int& i1, float& w1) {
-  i0 = o / f;
-  const int r = o - i0 * f;
-  i1 = min(i0 + 1, n - 1);
-  w1 = (float)r / (float)f;
-}
-
-__device__ __forceinline__ float upsample_at(const float* __restrict__ plane, int Hc, int Wc, int f,
-                                             int y, int x) {
-  int y0, y1, x0, x1;
-  float wy, wx;
-  upsample_taps(y, f, Hc, y0, y1, wy);
-  upsample_taps(x, f, Wc, x0, x1, wx);
-  const float a = __ldg(plane + (size_t)y0 * Wc + x0), b = __ldg(plane + (size_t)y0 * Wc + x1);
-  const float c = __ldg(plane + (size_t)y1 * Wc + x0), d = __ldg(plane + (size_t)y1 * Wc + x1);
-  const float top = a + (b - a) * wx, bot = c + (d - c) * wx;
-  return top + (bot - top) * wy;
-}
+// sigmoidf_, upsample_taps / upsample_at and the BilinearSampler taps: sampling.cuh (shared with the host emulation)
 
 // Bilinear tap of the deformable convolution: weights + indices for one real position (h, w).
 // valid == false means the tap contributes zero (see MFN_BORDER_* in maskflow_b200.h).

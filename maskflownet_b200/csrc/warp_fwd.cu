@@ -1,5 +1,5 @@
 // warp_fwd.cu -- flow-guided feature warp forward kernels (K3), Upsample, GridGenerator/BilinearSampler and the
-// fused cascade-input builder (K5) for sm_90a.
+// fused cascade-input builder (K5) for sm_90a.  The image warp's backward kernels are in image_warp_bwd.cu.
 //
 // K3 serves two entry points with one kernel template:
 //   mfn_deformable_conv_forward  F.contrib.DeformableConvolution(x, offset, weight[, bias])   network/layer.py:117-124
@@ -293,24 +293,7 @@ __global__ void gridgen_warp_kernel(const float* __restrict__ flow, float* __res
   }
 }
 
-__device__ __forceinline__ void sampler_taps(float xr, float yr, int H, int W, int (&off)[4], float (&wt)[4]) {
-  const int x0 = (int)floorf(xr), y0 = (int)floorf(yr);
-  const float wx0 = 1.f - (xr - (float)x0), wy0 = 1.f - (yr - (float)y0);
-  const float wx1 = 1.f - wx0, wy1 = 1.f - wy0;
-  const bool xin0 = x0 >= 0 && x0 <= W - 1, xin1 = x0 + 1 >= 0 && x0 + 1 <= W - 1;
-  const bool yin0 = y0 >= 0 && y0 <= H - 1, yin1 = y0 + 1 >= 0 && y0 + 1 <= H - 1;
-  const int xc0 = max(min(x0, W - 1), 0), xc1 = max(min(x0 + 1, W - 1), 0);
-  const int yc0 = max(min(y0, H - 1), 0), yc1 = max(min(y0 + 1, H - 1), 0);
-  off[0] = yc0 * W + xc0;
-  off[1] = yc0 * W + xc1;
-  off[2] = yc1 * W + xc0;
-  off[3] = yc1 * W + xc1;
-  wt[0] = (xin0 && yin0) ? wy0 * wx0 : 0.f;
-  wt[1] = (xin1 && yin0) ? wy0 * wx1 : 0.f;
-  wt[2] = (xin0 && yin1) ? wy1 * wx0 : 0.f;
-  wt[3] = (xin1 && yin1) ? wy1 * wx1 : 0.f;
-}
-
+// sampler_taps (the four corners and their weights): sampling.cuh, shared with the backward kernels (image_warp_bwd.cu)
 __global__ void bilinear_sampler_kernel(const float* __restrict__ data, const float* __restrict__ grid,
                                         float* __restrict__ out, int N, int C, int H, int W, int OH, int OW) {
   const long long total = (long long)N * OH * OW;
@@ -337,7 +320,9 @@ __global__ void bilinear_sampler_kernel(const float* __restrict__ data, const fl
 
 // K5: c40 = [ sample(im2, pix + Upsample(4)(flow_q)*scale) ; sigmoid(Upsample(4)(mask_q)) - 0.5 ], c30 = [im1 ; 0]
 // (network/MaskFlownet.py:308-313).  The grid normalisation of GridGenerator cancels against the sampler's
-// de-normalisation, so the source position is pix + displacement directly.
+// de-normalisation, so the source position is pix + displacement directly.  Differentiable: the backward with respect to
+// im2, Upsample(4)(flow_q) and Upsample(4)(mask_q) is image_warp_concat_bwd_kernel (image_warp_bwd.cu), and the gradient of
+// c30 with respect to im1 is the identity on its first Ci channels.
 __global__ void image_warp_concat_kernel(const float* __restrict__ im1, const float* __restrict__ im2,
                                          const float* __restrict__ flow_q, const float* __restrict__ mask_q,
                                          float* __restrict__ c30, float* __restrict__ c40, int N, int Ci, int H, int W,
@@ -374,12 +359,6 @@ __global__ void image_warp_concat_kernel(const float* __restrict__ im1, const fl
 // ---------------------------------------------------------------------------------------------------------
 // Host dispatch
 // ---------------------------------------------------------------------------------------------------------
-static inline unsigned grid_for(long long total, int threads) {
-  long long b = (total + threads - 1) / threads;
-  const long long cap = (long long)kNumSMs * 16;
-  return (unsigned)(b < cap ? (b > 0 ? b : 1) : cap);
-}
-
 template <int NT, int FT, int BORDER, bool SHARED>
 static void launch_deform_cfg(const float* x, const float* offset, const float* flow_c, const float* mask_c,
                               const float* weight, const float* bias, const float* tradeoff, float* out, float* fup,

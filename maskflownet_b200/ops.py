@@ -39,10 +39,14 @@ def _chk(t: Optional[torch.Tensor], name: str, optional: bool = False) -> Option
     return t.contiguous()
 
 
+def _needs_grad(*tensors) -> bool:
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
 def _no_grad_path(name: str, *tensors) -> None:
     """Forward-only kernels: refuse to silently cut the autograd graph (ADVICE r1): raise when grad mode is on and any
     operand requires grad."""
-    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
+    if _needs_grad(*tensors):
         raise MaskflowError(f"{name} is forward-only (no backward kernel): call it under torch.no_grad() or detach the "
                             f"operands -- an operand requires grad")
 
@@ -335,29 +339,73 @@ def upsample(x, factor: int, scale: float = 1.0):
 # ----------------------------------------------------------------------------------------------------------
 # Image warp
 # ----------------------------------------------------------------------------------------------------------
-def grid_generator_warp(flow_xy):
-    """MXNet F.GridGenerator(data=flow, transform_type='warp'); flow channels are (x, y)."""
-    f = _chk(flow_xy, "grid_generator_warp.flow")
-    _no_grad_path("grid_generator_warp", f)
-    N, two, H, W = f.shape
-    if two != 2:
-        raise MaskflowError("grid_generator_warp: flow must have 2 channels")
+def _grid_generator_warp_forward(f):
+    N, _, H, W = f.shape
     grid = torch.empty_like(f)
     _call("mfn_grid_generator_warp_forward", f.device, _p(f), _p(grid), N, H, W)
     return grid
 
 
-def bilinear_sampler(data, grid):
-    """MXNet F.BilinearSampler(data, grid) (forward only)."""
-    d, g = _chk(data, "bilinear_sampler.data"), _chk(grid, "bilinear_sampler.grid")
-    _no_grad_path("bilinear_sampler", d, g)
+class _GridGeneratorWarpFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, f):
+        return _grid_generator_warp_forward(f)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gg):
+        gg = gg.contiguous()
+        N, _, H, W = gg.shape
+        gf = torch.empty_like(gg)
+        _call("mfn_grid_generator_warp_backward", gg.device, _p(gg), _p(gf), N, H, W)
+        return gf
+
+
+def grid_generator_warp(flow_xy):
+    """MXNet F.GridGenerator(data=flow, transform_type='warp'); flow channels are (x, y).  Differentiable."""
+    f = _chk(flow_xy, "grid_generator_warp.flow")
+    if f.dim() != 4 or f.shape[1] != 2:
+        raise MaskflowError("grid_generator_warp: flow must have 2 channels")
+    if _needs_grad(f):
+        return _GridGeneratorWarpFn.apply(f)
+    return _grid_generator_warp_forward(f)
+
+
+def _bilinear_sampler_forward(d, g):
     N, C, H, W = d.shape
-    if g.shape[0] != N or g.shape[1] != 2:
-        raise MaskflowError("bilinear_sampler: grid must be (N,2,OH,OW)")
     OH, OW = g.shape[2:]
     out = torch.empty((N, C, OH, OW), device=d.device, dtype=torch.float32)
     _call("mfn_bilinear_sampler_forward", d.device, _p(d), _p(g), _p(out), N, C, H, W, OH, OW)
     return out
+
+
+class _BilinearSamplerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, d, g):
+        ctx.save_for_backward(d, g)
+        return _bilinear_sampler_forward(d, g)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, go):
+        d, g = ctx.saved_tensors
+        N, C, H, W = d.shape
+        OH, OW = g.shape[2:]
+        go = go.contiguous()
+        gd = torch.zeros_like(d) if ctx.needs_input_grad[0] else None      # accumulated by the kernel
+        gg = torch.empty_like(g) if ctx.needs_input_grad[1] else None
+        _call("mfn_bilinear_sampler_backward", d.device, _p(go), _p(d), _p(g), _p(gd), _p(gg), N, C, H, W, OH, OW)
+        return gd, gg
+
+
+def bilinear_sampler(data, grid):
+    """MXNet F.BilinearSampler(data, grid).  Differentiable with respect to data and grid."""
+    d, g = _chk(data, "bilinear_sampler.data"), _chk(grid, "bilinear_sampler.grid")
+    if d.dim() != 4 or g.dim() != 4 or g.shape[0] != d.shape[0] or g.shape[1] != 2:
+        raise MaskflowError("bilinear_sampler: grid must be (N,2,OH,OW)")
+    if _needs_grad(d, g):
+        return _BilinearSamplerFn.apply(d, g)
+    return _bilinear_sampler_forward(d, g)
 
 
 def reconstruction2d(x, flow_yx):
@@ -365,20 +413,60 @@ def reconstruction2d(x, flow_yx):
     return bilinear_sampler(x, grid_generator_warp(flow_yx.flip(1)))
 
 
-def image_warp_concat(im1, im2, flow_q, mask_q, scale=20.0, want_c30=True):
-    """Fused cascade-input builder (network/MaskFlownet.py:308-313).  Returns (c30 or None, c40)."""
-    i2 = _chk(im2, "image_warp_concat.im2")
-    i1 = _chk(im1, "image_warp_concat.im1", optional=not want_c30)
-    fq, mq = _chk(flow_q, "image_warp_concat.flow_q"), _chk(mask_q, "image_warp_concat.mask_q")
-    _no_grad_path("image_warp_concat", i1, i2, fq, mq)
+def _image_warp_concat_forward(i1, i2, fq, mq, scale, want_c30):
     N, Ci, H, W = i2.shape
-    if fq.shape != (N, 2, H // 4, W // 4) or mq.shape != (N, 1, H // 4, W // 4) or H % 4 or W % 4:
-        raise MaskflowError("image_warp_concat: flow_q/mask_q must be (N,2|1,H/4,W/4)")
     c40 = torch.empty((N, Ci + 1, H, W), device=i2.device, dtype=torch.float32)
     c30 = torch.empty_like(c40) if want_c30 else None
     _call("mfn_image_warp_concat_forward", i2.device, _p(i1) if want_c30 else None, _p(i2), _p(fq), _p(mq), _p(c30),
           _p(c40), N, Ci, H, W, float(scale))
     return c30, c40
+
+
+class _ImageWarpConcatFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, i1, i2, fq, mq, scale, want_c30):
+        c30, c40 = _image_warp_concat_forward(i1, i2, fq, mq, scale, want_c30)
+        ctx.scale = scale
+        ctx.save_for_backward(i2, fq, mq)
+        if c30 is None:
+            c30 = torch.empty(0, device=i2.device)
+        return c30, c40
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g30, g40):
+        i2, fq, mq = ctx.saved_tensors
+        N, Ci, H, W = i2.shape
+        need = ctx.needs_input_grad  # im1, im2, flow_q, mask_q
+        # c30 = [im1 ; 0]: im1's gradient is the first Ci channels of c30's
+        gi1 = g30[:, :Ci] if (need[0] and g30 is not None and g30.numel()) else None
+        gi2 = gfq = gmq = None
+        if g40 is not None and (need[1] or need[2] or need[3]):
+            g40 = g40.contiguous()
+            gi2 = torch.zeros_like(i2) if need[1] else None                    # accumulated by the kernel
+            gfu = torch.empty((N, 2, H, W), device=i2.device, dtype=torch.float32) if need[2] else None
+            gmu = torch.empty((N, 1, H, W), device=i2.device, dtype=torch.float32) if need[3] else None
+            _call("mfn_image_warp_concat_backward", i2.device, _p(g40), _p(i2), _p(fq), _p(mq), _p(gi2), _p(gfu), _p(gmu),
+                  N, Ci, H, W, float(ctx.scale))
+            # the transposed Upsample(4) brings the up-sampled gradients to the quarter-resolution grid
+            gfq = _upsample_backward(gfu, 4, 1.0) if need[2] else None
+            gmq = _upsample_backward(gmu, 4, 1.0) if need[3] else None
+        return gi1, gi2, gfq, gmq, None, None
+
+
+def image_warp_concat(im1, im2, flow_q, mask_q, scale=20.0, want_c30=True):
+    """Fused cascade-input builder (network/MaskFlownet.py:308-313).  Returns (c30 or None, c40).  Differentiable with
+    respect to im1 (through c30), im2, flow_q and mask_q; without a gradient to compute it is the single forward launch."""
+    i2 = _chk(im2, "image_warp_concat.im2")
+    i1 = _chk(im1, "image_warp_concat.im1", optional=not want_c30)
+    fq, mq = _chk(flow_q, "image_warp_concat.flow_q"), _chk(mask_q, "image_warp_concat.mask_q")
+    N, Ci, H, W = i2.shape
+    if fq.shape != (N, 2, H // 4, W // 4) or mq.shape != (N, 1, H // 4, W // 4) or H % 4 or W % 4:
+        raise MaskflowError("image_warp_concat: flow_q/mask_q must be (N,2|1,H/4,W/4)")
+    if _needs_grad(i1 if want_c30 else None, i2, fq, mq):
+        c30, c40 = _ImageWarpConcatFn.apply(i1 if want_c30 else None, i2, fq, mq, float(scale), bool(want_c30))
+        return (c30 if want_c30 else None), c40
+    return _image_warp_concat_forward(i1, i2, fq, mq, scale, want_c30)
 
 
 # ----------------------------------------------------------------------------------------------------------

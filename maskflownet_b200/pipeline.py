@@ -83,7 +83,8 @@ class PipelineFlownet:
             head.load_state_dict(torch.load(checkpoint, map_location=self.device))
 
     def fix_head(self) -> None:
-        """Freeze the MaskFlownet-S head of the cascade (MaskFlownet.fix_head, network/MaskFlownet.py:412-414)."""
+        """Freeze the MaskFlownet-S head of the cascade (MaskFlownet.fix_head, network/MaskFlownet.py:412-414) and rebuild Adam
+        over the cascade's own parameters.  Optional: without it train_batch trains the cascade end to end, head included."""
         head = getattr(self.network, "MaskFlownet_S", None)
         if head is None:
             raise MaskflowError("fix_head: the network has no MaskFlownet_S head (only the cascade does)")

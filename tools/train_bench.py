@@ -3,6 +3,10 @@
 
     python tools/train_bench.py --hw 384x512 --batch 8 --steps 5
     torchrun --nproc-per-node 2 tools/train_bench.py --hw 576x960 --batch 8 --steps 5     (global batch = 8 * world)
+    python tools/train_bench.py --network MaskFlownet --hw 320x768 --batch 4 --steps 10 [--fix-head]
+
+--network MaskFlownet trains the cascade (the reference's cascade training shape is 320x768, batch 4); --fix-head freezes
+its MaskFlownet-S head and gives Adam only the trainable parameters, as PipelineFlownet.fix_head does.
 
 Prints one JSON line: ms/step, pairs/s, time of the hand-written backward kernels (CUDA events) and of the all-reduce.
 """
@@ -18,7 +22,11 @@ def main():
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--network", choices=("MaskFlownet_S", "MaskFlownet"), default="MaskFlownet_S")
+    ap.add_argument("--fix-head", action="store_true", help="freeze the cascade's MaskFlownet-S head (MaskFlownet only)")
     a = ap.parse_args()
+    if a.fix_head and a.network != "MaskFlownet":
+        ap.error("--fix-head needs --network MaskFlownet (only the cascade has a head)")
     H, W = map(int, a.hw.split("x"))
     rank, local, world = mdist.init_from_env("nccl")
     torch.cuda.set_device(local)
@@ -27,9 +35,12 @@ def main():
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.benchmark = True
     torch.manual_seed(0)
-    model = network.MaskFlownetS().to(dev).train()
-    bucket = mdist.GradBucket(model.parameters())
-    opt = torch.optim.Adam(model.parameters(), lr=1e-4)     # network/pipeline.py:27
+    model = (network.MaskFlownet() if a.network == "MaskFlownet" else network.MaskFlownetS()).to(dev).train()
+    if a.fix_head:                                          # PipelineFlownet.fix_head (network/MaskFlownet.py:412-414)
+        for p in model.MaskFlownet_S.parameters():
+            p.requires_grad_(False)
+    bucket = mdist.GradBucket(model.parameters())           # skips frozen parameters
+    opt = torch.optim.Adam([p for p in model.parameters() if p.requires_grad], lr=1e-4)     # network/pipeline.py:27
     g = torch.Generator(device=dev).manual_seed(1 + rank)
     im1 = torch.rand(a.batch, 3, H, W, device=dev, generator=g) - 0.5
     im2 = torch.rand(a.batch, 3, H, W, device=dev, generator=g) - 0.5
@@ -66,7 +77,7 @@ def main():
     ms = mdist.max_over_ranks(s0.elapsed_time(s1), dev) / a.steps
     ar = sum(x.elapsed_time(y) for x, y in t_ar) / len(t_ar)
     if rank == 0:
-        print(json.dumps({"bench": "train_step", "hw": a.hw, "batch_per_gpu": a.batch, "n_gpus": world,
+        print(json.dumps({"bench": "train_step", "network": a.network, "fix_head": a.fix_head, "hw": a.hw, "batch_per_gpu": a.batch, "n_gpus": world,
                           "ms_per_step": round(ms, 3), "pairs_per_s": round(a.batch * world / ms * 1e3, 2),
                           "native_launches_per_step": (_lib.launch_count() - n0) // a.steps,
                           "grad_allreduce_ms": round(ar, 4), "grad_bucket_mb": round(bucket.numel * 4 / 1e6, 1),
