@@ -300,6 +300,21 @@ MFN_API int mfn_postprocess_forward(const float* pred, float* out, int N, int ch
                                     int flip_channels, int is_flow, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Middlebury colour coding of a flow (Baker et al.; flow_vis.flow_to_color, which predict_new_data.py writes).
+ *   flow_xy (N,H,W,2) float32, (x,y) = (u,v) in pixels: the layout mfn_postprocess_forward writes; 8-byte aligned.
+ *   rgb (N,H,W,3) uint8 out, channels R,G,B (B,G,R when bgr).
+ *   max_radius <= 0: each sample is divided by (r + 1e-5), r = its largest sqrt(u^2+v^2) (the reference's behaviour);
+ *   max_radius > 0: every sample is divided by max_radius (colours comparable across the frames of a video).
+ *   rad_max (N) float32 out: the radius each sample was normalised by (r, or max_radius).
+ * Per pixel: rad = |(u,v)|, angle atan2(-v,-u)/pi -> blend of two neighbouring entries of a 55-entry colour wheel;
+ * rad <= 1 whitens towards the centre (1 - rad (1 - col)), rad > 1 darkens (0.75 col); out = floor(255 col).
+ * Any input, NaN and inf included, stays inside the wheel (such pixels get unspecified colours).  Capture-safe, no
+ * allocation: a cudaMemsetAsync and a max pass (per-sample mode only), then one colouring pass.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API int mfn_flow_to_color(const float* flow_xy, unsigned char* rgb, float* rad_max, int N, int H, int W,
+                              float max_radius, int bgr, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * GPU-side training augmentation (SURVEY.md section 8f, row N4): /root/reference/augmentation.py:168-339, constructed in
  * main.py:386-419, applied in network/pipeline.py:100-102 (`/ 255`, geo_aug, color_aug).  The random draws and the small
  * per-sample matrices derived from them are host logic (maskflownet_b200/augment.py); the kernels take the result as a

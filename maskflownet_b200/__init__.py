@@ -8,6 +8,7 @@ the local correlation cost volume and the flow-guided deformable feature warp x 
   maskflownet_b200.losses   MultiscaleEpe on the fused kernels (network/MaskFlownet.py:563-611)
   maskflownet_b200.augment  GeometryAugmentation / ColorAugmentation with the reference's constructor arguments (augmentation.py)
   maskflownet_b200.pipeline PipelineFlownet: train_batch / do_batch / validate / predict (network/pipeline.py:19-223)
+  maskflownet_b200.video    VideoFlowPredictor: a video -> one colour-coded flow per frame pair, one CUDA graph per size
   maskflownet_b200.dist     batch sharding + the one gradient all-reduce;  .params  reader of the reference's checkpoints
 """
 from . import _lib  # noqa: F401

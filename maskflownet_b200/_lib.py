@@ -38,6 +38,7 @@ SIGNATURES = {
     "mfn_image_warp_concat_backward": [_f] * 7 + [_i] * 4 + [_fl, _f],
     "mfn_preprocess_forward": [_f, _f, _i, _f, _f, _f, _i, _i, _i, _i, _i, _i, _f],
     "mfn_postprocess_forward": [_f, _f, _i, _i, _i, _i, _i, _i, _i, _i, _f],
+    "mfn_flow_to_color": [_f, _f, _f, _i, _i, _i, _fl, _i, _f],
     "mfn_geometry_augment_forward": [_f, _f, _i, _f, _f, _i, _f, _f, _f, _f, _f, _i, _i, _i, _i, _i, _f],
     "mfn_color_augment_forward": [_f, _f, _f, _f, _f, _fl, _ll, _f, _f, _f, _ll, _i, _i, _i, _i, _f],
     "mfn_multiscale_epe_forward": [_f, _f, _f, _f, _f, _i, _fl, _fl, _f, _f, _f, _ll, _i, _i, _i, _f],

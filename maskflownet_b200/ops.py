@@ -631,3 +631,24 @@ def postprocess(pred: torch.Tensor, H: int, W: int, flip_channels: bool = True, 
     _call("mfn_postprocess_forward", p.device, _p(p), _p(out), N, CH, Hq, Wq, int(H), int(W), 1 if flip_channels else 0,
           1 if is_flow else 0)
     return out
+
+
+def flow_to_color(flow_xy: torch.Tensor, max_radius: Optional[float] = None, bgr: bool = False):
+    """Middlebury colour coding (flow_vis.flow_to_color, what predict_new_data.py writes) of an (x,y) flow in pixels, the
+    layout postprocess returns: (N,H,W,2) -> (rgb uint8 (N,H,W,3), rad_max (N,)); an (H,W,2) flow gives (H,W,3) and a
+    0-d rad_max.  max_radius None: each sample is normalised by its own largest radius (the reference); a positive
+    value fixes the scale, so that colours stay comparable across the frames of a video.  rad_max is the radius used.
+    Channels R,G,B, or B,G,R with bgr (for cv2).  Forward only."""
+    f = _chk(flow_xy, "flow_to_color.flow_xy")
+    if f.dim() not in (3, 4) or f.shape[-1] != 2:
+        raise MaskflowError(f"flow_to_color: expected an (N,H,W,2) or (H,W,2) flow, got {tuple(f.shape)}")
+    if max_radius is not None and not (0.0 < float(max_radius) < float("inf")):
+        raise MaskflowError(f"flow_to_color: max_radius must be positive and finite, got {max_radius}")
+    _no_grad_path("flow_to_color", f)
+    f4 = f if f.dim() == 4 else f.unsqueeze(0)
+    N, H, W, _ = f4.shape
+    rgb = torch.empty((N, H, W, 3), device=f.device, dtype=torch.uint8)
+    rad_max = torch.empty((N,), device=f.device, dtype=torch.float32)
+    _call("mfn_flow_to_color", f.device, _p(f4), _p(rgb), _p(rad_max), N, H, W,
+          float(max_radius) if max_radius is not None else 0.0, 1 if bgr else 0)
+    return (rgb, rad_max) if f.dim() == 4 else (rgb[0], rad_max[0])

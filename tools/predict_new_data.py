@@ -1,0 +1,126 @@
+"""Flow of a user's own data, written as the Middlebury colour coding: the reference's predict_new_data.py on this library.
+
+    python tools/predict_new_data.py out.png --image_1 a.png --image_2 b.png -c weights.params [-n MaskFlownet_S]
+    python tools/predict_new_data.py out.avi --video_filepath in.mp4 -c weights.params [--batch 8] [--resize 448,1024]
+                                     [--max_radius 20]
+
+An image pair gives one PNG.  A video gives a video of the input's frame rate with one colour frame per consecutive frame
+pair (so one frame fewer than the input), streamed through network.VideoFlowPredictor: each frame is uploaded once and
+coloured on the GPU.  Frames go to the network in the channel order cv2 reads them (B,G,R), as in the reference.
+
+-c takes a shipped .params checkpoint (maskflownet_b200.params.load_checkpoint) or a .pt state_dict of the model class
+-n names.  Departures from the reference, on purpose:
+  * the PNG has standard colours.  The reference hands an RGB image to cv2.imwrite, which expects B,G,R, so its PNGs have
+    red and blue swapped; here the colour kernel writes B,G,R for cv2.
+  * --resize is honoured.  The reference parses it but passes it to neither the image nor the video path.
+  * videos are written with cv2.VideoWriter (MJPG for .avi, mp4v otherwise) instead of moviepy; there is no audio.
+  * --max_radius (new) fixes the colour scale across frames; by default every frame is normalised by its own largest
+    flow, as flow_vis does.
+"""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from maskflownet_b200 import network, ops, params  # noqa: E402
+from maskflownet_b200.video import VideoFlowPredictor  # noqa: E402
+
+NETWORKS = {"MaskFlownet": network.MaskFlownet, "MaskFlownet_S": network.MaskFlownetS}
+
+
+def load_model(name: str, checkpoint: str, device="cuda") -> torch.nn.Module:
+    model = NETWORKS[name]()
+    if checkpoint.endswith(".params"):
+        params.load_checkpoint(model, checkpoint)
+    else:
+        model.load_state_dict(torch.load(checkpoint, map_location="cpu"))
+    return model.to(device).eval()
+
+
+def _imread(cv2, path):
+    img = cv2.imread(path)
+    if img is None:
+        raise FileNotFoundError(f"cannot read image {path}")
+    return img
+
+
+@torch.no_grad()
+def predict_files(model: torch.nn.Module, flow_filepath: str, image_1=None, image_2=None, video_filepath=None, batch=8,
+                  resize=None, max_radius=None) -> int:
+    """Writes the colour-coded flow of an image pair (one image) or of a video (one frame per consecutive pair) to
+    flow_filepath; returns the number of images written."""
+    import cv2
+
+    if video_filepath is None:
+        if image_1 is None or image_2 is None:
+            raise ValueError("give --image_1 and --image_2, or --video_filepath")
+        a, b = _imread(cv2, image_1), _imread(cv2, image_2)
+        if a.shape != b.shape:
+            raise ValueError(f"the images differ in size: {a.shape} vs {b.shape}")
+        dev = next(model.parameters()).device
+        to_dev = lambda im: torch.from_numpy(im).permute(2, 0, 1)[None].contiguous().to(dev)  # noqa: E731
+        flow, _ = network.predict(model, to_dev(a), to_dev(b), resize)
+        rgb, _ = ops.flow_to_color(flow[0], max_radius, bgr=True)
+        if not cv2.imwrite(flow_filepath, rgb.cpu().numpy()):
+            raise OSError(f"cannot write {flow_filepath}")
+        return 1
+
+    cap = cv2.VideoCapture(video_filepath)
+    if not cap.isOpened():
+        raise FileNotFoundError(f"cannot open video {video_filepath}")
+    fps = cap.get(cv2.CAP_PROP_FPS)
+
+    def frames():
+        try:
+            while True:
+                ok, frame = cap.read()
+                if not ok:
+                    return
+                yield frame
+        finally:
+            cap.release()
+
+    pred = VideoFlowPredictor(model, batch=batch, resize=resize, max_radius=max_radius, bgr=True)
+    fourcc = cv2.VideoWriter_fourcc(*("MJPG" if flow_filepath.lower().endswith(".avi") else "mp4v"))
+    writer, n = None, 0
+    try:
+        for rgb in pred.run(frames()):
+            if writer is None:
+                writer = cv2.VideoWriter(flow_filepath, fourcc, fps if fps > 0 else 25.0, (rgb.shape[1], rgb.shape[0]))
+                if not writer.isOpened():
+                    raise OSError(f"cannot write {flow_filepath}")
+            writer.write(rgb)
+            n += 1
+    finally:
+        if writer is not None:
+            writer.release()
+    return n
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("flow_filepath", help="destination of the flow image / video")
+    ap.add_argument("--image_1", help="first image")
+    ap.add_argument("--image_2", help="second image")
+    ap.add_argument("--video_filepath", help="input video")
+    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
+    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
+    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay (video)")
+    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
+    ap.add_argument("--max_radius", type=float, default=None,
+                    help="fixed flow magnitude (pixels) of the colour wheel's rim; default: each frame's largest flow")
+    a = ap.parse_args(argv)
+    if a.video_filepath is None and (a.image_1 is None or a.image_2 is None):
+        ap.error("give --image_1 and --image_2, or --video_filepath")
+    resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
+    model = load_model(a.network, a.checkpoint)
+    n = predict_files(model, a.flow_filepath, a.image_1, a.image_2, a.video_filepath, a.batch, resize, a.max_radius)
+    print(f"wrote {n} image(s) to {a.flow_filepath}")
+
+
+if __name__ == "__main__":
+    main()
