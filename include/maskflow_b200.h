@@ -315,6 +315,48 @@ MFN_API int mfn_flow_to_color(const float* flow_xy, unsigned char* rgb, float* r
                               float max_radius, int bgr, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Deterministic mode: bit-reproducible variants of the entry points whose default kernels accumulate with fp32 atomics
+ * (the scatter of a bilinear sample's gradient to its four corners, per-CTA weight partials, per-slice plane sums).  Same
+ * arguments and results as the counterpart named without _det, plus a caller-owned workspace `det_ws` of `det_ws_bytes`
+ * bytes (16-byte aligned; contents need not be initialised); a null or too small workspace returns MFN_ERR_INVALID_ARG.
+ * Two calls with the same inputs give bit-identical outputs, whatever the GPU and the thread schedule.
+ *   - Scatters (grad_x, grad_data, grad_im2) accumulate in 64-bit fixed point with integer atomics; the scale
+ *     2^s is chosen on the device from a bound on the largest contribution and the largest fan-in, so no sum can overflow.
+ *     Each element differs from the exact sum of its fp32 contributions by at most n * 2^-(s+1) (n = contributions to it)
+ *     plus the final fp32 rounding: far below fp32 atomics' reordering noise.  NaN / inf in the bound give NaN in the output.
+ *   - grad_weight of the K4 entries: per-CTA partials (128 pixels per CTA) reduced in CTA order.
+ *   - mfn_preprocess_forward_det: 64 slices per plane whatever the GPU, partial sums added in slice order.
+ * Workspace bytes (the formulas of maskflownet_b200/ops.py, det_workspace_bytes):
+ *   mfn_warp_mask_backward_det, mfn_deformable_conv_backward_det:
+ *       256 + 8*N*C*H*W + 4*F*C*9*ceil(N*H*W / 128)
+ *   mfn_bilinear_sampler_backward_det:   256 + 8*N*C*H*W      (data extents)
+ *   mfn_image_warp_concat_backward_det:  256 + 8*N*Ci*H*W
+ *   mfn_preprocess_forward_det:          256 + 4*N*C*64
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API int mfn_warp_mask_backward_det(const float* grad_out, const float* out, const float* conv_out,
+                                       const float* x, const float* flow_up, const float* mask_up,
+                                       const float* weight, float* grad_x, float* grad_flow_up,
+                                       float* grad_mask_up, float* grad_weight, float* grad_bias,
+                                       float* grad_tradeoff, float* grad_conv_ws, int N, int C, int H, int W,
+                                       int F, float flow_scale, float level_stride, float leaky_slope,
+                                       int border_mode, void* det_ws, long long det_ws_bytes, void* stream);
+MFN_API int mfn_deformable_conv_backward_det(const float* grad_out, const float* data, const float* offset,
+                                             const float* weight, float* grad_data, float* grad_offset,
+                                             float* grad_weight, float* grad_bias, int N, int C, int H, int W,
+                                             int F, int border_mode, void* det_ws, long long det_ws_bytes,
+                                             void* stream);
+MFN_API int mfn_bilinear_sampler_backward_det(const float* grad_out, const float* data, const float* grid,
+                                              float* grad_data, float* grad_grid, int N, int C, int H, int W,
+                                              int OH, int OW, void* det_ws, long long det_ws_bytes, void* stream);
+MFN_API int mfn_image_warp_concat_backward_det(const float* grad_c40, const float* im2, const float* flow_q,
+                                               const float* mask_q, float* grad_im2, float* grad_flow_up,
+                                               float* grad_mask_up, int N, int Ci, int H, int W, float flow_scale,
+                                               void* det_ws, long long det_ws_bytes, void* stream);
+MFN_API int mfn_preprocess_forward_det(const void* img1, const void* img2, int is_uint8, float* out1, float* out2,
+                                       float* rgb_mean, int N, int C, int H, int W, int OH, int OW, void* det_ws,
+                                       long long det_ws_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * GPU-side training augmentation (SURVEY.md section 8f, row N4): /root/reference/augmentation.py:168-339, constructed in
  * main.py:386-419, applied in network/pipeline.py:100-102 (`/ 255`, geo_aug, color_aug).  The random draws and the small
  * per-sample matrices derived from them are host logic (maskflownet_b200/augment.py); the kernels take the result as a

@@ -39,6 +39,11 @@ SIGNATURES = {
     "mfn_preprocess_forward": [_f, _f, _i, _f, _f, _f, _i, _i, _i, _i, _i, _i, _f],
     "mfn_postprocess_forward": [_f, _f, _i, _i, _i, _i, _i, _i, _i, _i, _f],
     "mfn_flow_to_color": [_f, _f, _f, _i, _i, _i, _fl, _i, _f],
+    "mfn_warp_mask_backward_det": [_f] * 14 + [_i] * 5 + [_fl, _fl, _fl, _i, _f, _ll, _f],
+    "mfn_deformable_conv_backward_det": [_f] * 8 + [_i] * 6 + [_f, _ll, _f],
+    "mfn_bilinear_sampler_backward_det": [_f] * 5 + [_i] * 6 + [_f, _ll, _f],
+    "mfn_image_warp_concat_backward_det": [_f] * 7 + [_i] * 4 + [_fl, _f, _ll, _f],
+    "mfn_preprocess_forward_det": [_f, _f, _i, _f, _f, _f, _i, _i, _i, _i, _i, _i, _f, _ll, _f],
     "mfn_geometry_augment_forward": [_f, _f, _i, _f, _f, _i, _f, _f, _f, _f, _f, _i, _i, _i, _i, _i, _f],
     "mfn_color_augment_forward": [_f, _f, _f, _f, _f, _fl, _ll, _f, _f, _f, _ll, _i, _i, _i, _i, _f],
     "mfn_multiscale_epe_forward": [_f, _f, _f, _f, _f, _i, _fl, _fl, _f, _f, _f, _ll, _i, _i, _i, _f],

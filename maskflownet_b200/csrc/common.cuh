@@ -81,6 +81,15 @@ int launch_corr_rb(int md, const float* d1, const float* d2, float* out, int N, 
 int launch_corr_tma(int md, const float* d1, const float* d2, float* out, int N, int C, int H, int W, long long obs,
                     float slope, cudaStream_t st);
 
+// det_bwd.cu: the shared passes of the deterministic backward mode (arithmetic in det.cuh)
+int det_launch_abs_max(const float* v, long long n, unsigned* bound, cudaStream_t st);
+int det_launch_pixel_abs_sum_max(const float* g, int N, int F, long long HW, unsigned* bound, cudaStream_t st);
+int det_launch_fixed_to_float(const unsigned long long* acc, float* out, long long n, const unsigned* bound, int nb,
+                              int fanin_bits, cudaStream_t st);
+int det_launch_ordered_sum(const float* part, int nparts, long long part_stride, long long elem_stride, float* out,
+                           long long n, int accumulate, cudaStream_t st);
+int det_check_workspace(const char* fn, const void* ws, long long bytes, long long need);
+
 // ---- device helpers ---------------------------------------------------------------------------------
 __device__ __forceinline__ float leaky(float v, float slope) { return v > 0.f ? v : v * slope; }
 

@@ -10,6 +10,7 @@
 // BilinearResize2D is MXNet's contrib operator [MXNet-recalled, bilinear_resize-inl.h]: "align corners" mapping
 //   src = dst * (in - 1) / (out - 1),  i0 = (int)src,  i1 = i0 + (i0 < in - 1),  l = src - i0.
 #include "common.cuh"
+#include "det.cuh"
 
 namespace mfn {
 
@@ -27,7 +28,8 @@ __device__ __forceinline__ Lin resize_tap(int o, int n_in, int n_out) {
   return t;
 }
 
-template <typename T>
+// DET: the partial sum of block (p, s) is stored to sums[p * slices + s] instead (det_ordered_sum_kernel adds them in order)
+template <typename T, bool DET = false>
 __global__ void __launch_bounds__(256)
     rgb_sum_kernel(const T* __restrict__ a, const T* __restrict__ b, float* __restrict__ sums, int planes, int HW, int slices) {
   // grid = planes * slices; partial sums of both images of plane p are added to sums[p]
@@ -46,7 +48,12 @@ __global__ void __launch_bounds__(256)
     float v = red[threadIdx.x];
 #pragma unroll
     for (int o = 4; o > 0; o >>= 1) v += __shfl_xor_sync(0xffu, v, o);
-    if (threadIdx.x == 0) atomicAdd(sums + p, v);
+    if (threadIdx.x == 0) {
+      if constexpr (DET)
+        sums[blockIdx.x] = v;
+      else
+        atomicAdd(sums + p, v);
+    }
   }
 }
 
@@ -121,31 +128,57 @@ static inline unsigned grid_of(long long total) {
 
 }  // namespace mfn
 
-extern "C" int mfn_preprocess_forward(const void* img1, const void* img2, int is_uint8, float* out1, float* out2,
-                                      float* rgb_mean, int N, int C, int H, int W, int OH, int OW, void* stream) {
-  using namespace mfn;
-  MFN_REQUIRE(img1 && img2 && out1 && out2 && rgb_mean, MFN_ERR_INVALID_ARG, "mfn_preprocess_forward: null pointer");
-  MFN_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && OH > 0 && OW > 0, MFN_ERR_INVALID_ARG,
-              "mfn_preprocess_forward: non-positive extent");
+namespace mfn {
+
+// det_part: null = the default path (slices sized to fill the GPU, partial sums added with atomics); else the deterministic
+// one: kDetSlices slices per plane whatever the GPU, partials stored to det_part and summed in slice order.
+static int preprocess_forward(const void* img1, const void* img2, int is_uint8, float* out1, float* out2, float* rgb_mean,
+                              int N, int C, int H, int W, int OH, int OW, void* stream, void* det_ws, long long det_ws_bytes,
+                              bool det) {
+  const char* fn = det ? "mfn_preprocess_forward_det" : "mfn_preprocess_forward";
+  MFN_REQUIRE(img1 && img2 && out1 && out2 && rgb_mean, MFN_ERR_INVALID_ARG, "%s: null pointer", fn);
+  MFN_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && OH > 0 && OW > 0, MFN_ERR_INVALID_ARG, "%s: non-positive extent", fn);
   MFN_REQUIRE((long long)N * C * OH * OW < (1LL << 40) && (long long)H * W < (1LL << 31), MFN_ERR_ALIGNMENT,
-              "mfn_preprocess_forward: extents overflow kernel indexing");
-  cudaStream_t st = as_stream(stream);
+              "%s: extents overflow kernel indexing", fn);
   const int planes = N * C;
-  cudaError_t ce = cudaMemsetAsync(rgb_mean, 0, sizeof(float) * planes, st);
-  if (ce != cudaSuccess) return fail((int)ce, "mfn_preprocess_forward: cudaMemsetAsync: %s", cudaGetErrorString(ce));
-  int slices = (kNumSMs * 4 + planes - 1) / planes;
-  if (slices < 1) slices = 1;
-  // rgb_mean first accumulates the per-plane sums (atomics over `slices` partial sums), is read as such by the resampling
-  // kernel, and is turned into the means by a last tiny launch
-  if (is_uint8)
-    rgb_sum_kernel<unsigned char><<<planes * slices, 256, 0, st>>>(static_cast<const unsigned char*>(img1),
-                                                                  static_cast<const unsigned char*>(img2), rgb_mean, planes,
-                                                                  H * W, slices);
-  else
-    rgb_sum_kernel<float><<<planes * slices, 256, 0, st>>>(static_cast<const float*>(img1), static_cast<const float*>(img2),
-                                                          rgb_mean, planes, H * W, slices);
-  int rc = check_launch("rgb_sum_kernel");
-  if (rc) return rc;
+  float* part = nullptr;
+  if (det) {
+    const int rc = det_check_workspace(fn, det_ws, det_ws_bytes, kDetHeaderBytes + 4LL * planes * kDetSlices);
+    if (rc) return rc;
+    part = reinterpret_cast<float*>(static_cast<char*>(det_ws) + kDetHeaderBytes);
+  }
+  cudaStream_t st = as_stream(stream);
+  int slices;
+  if (det) {
+    slices = kDetSlices;
+    if (is_uint8)
+      rgb_sum_kernel<unsigned char, true><<<planes * slices, 256, 0, st>>>(
+          static_cast<const unsigned char*>(img1), static_cast<const unsigned char*>(img2), part, planes, H * W, slices);
+    else
+      rgb_sum_kernel<float, true><<<planes * slices, 256, 0, st>>>(static_cast<const float*>(img1),
+                                                                  static_cast<const float*>(img2), part, planes, H * W,
+                                                                  slices);
+    int rc = check_launch("rgb_sum_kernel");
+    if (rc) return rc;
+    // rgb_mean[p] = sum_s part[p * slices + s]
+    if ((rc = det_launch_ordered_sum(part, slices, 1, slices, rgb_mean, planes, 0, st))) return rc;
+  } else {
+    cudaError_t ce = cudaMemsetAsync(rgb_mean, 0, sizeof(float) * planes, st);
+    if (ce != cudaSuccess) return fail((int)ce, "%s: cudaMemsetAsync: %s", fn, cudaGetErrorString(ce));
+    slices = (kNumSMs * 4 + planes - 1) / planes;
+    if (slices < 1) slices = 1;
+    // rgb_mean first accumulates the per-plane sums (atomics over `slices` partial sums), is read as such by the resampling
+    // kernel, and is turned into the means by a last tiny launch
+    if (is_uint8)
+      rgb_sum_kernel<unsigned char><<<planes * slices, 256, 0, st>>>(static_cast<const unsigned char*>(img1),
+                                                                    static_cast<const unsigned char*>(img2), rgb_mean, planes,
+                                                                    H * W, slices);
+    else
+      rgb_sum_kernel<float><<<planes * slices, 256, 0, st>>>(static_cast<const float*>(img1), static_cast<const float*>(img2),
+                                                            rgb_mean, planes, H * W, slices);
+    const int rc = check_launch("rgb_sum_kernel");
+    if (rc) return rc;
+  }
   const long long total = (long long)planes * OH * OW;
   const float in_scale = is_uint8 ? 1.f / 255.f : 1.f;
   if (is_uint8)
@@ -155,10 +188,24 @@ extern "C" int mfn_preprocess_forward(const void* img1, const void* img2, int is
   else
     preprocess_kernel<float><<<grid_of(total), 256, 0, st>>>(static_cast<const float*>(img1), static_cast<const float*>(img2),
                                                             rgb_mean, out1, out2, nullptr, planes, H, W, OH, OW, in_scale);
-  rc = check_launch("preprocess_kernel");
+  const int rc = check_launch("preprocess_kernel");
   if (rc) return rc;
   scale_kernel<<<(planes + 255) / 256, 256, 0, st>>>(rgb_mean, planes, in_scale / (2.f * (float)H * (float)W));
   return check_launch("preprocess_kernel");
+}
+
+}  // namespace mfn
+
+extern "C" int mfn_preprocess_forward(const void* img1, const void* img2, int is_uint8, float* out1, float* out2,
+                                      float* rgb_mean, int N, int C, int H, int W, int OH, int OW, void* stream) {
+  return mfn::preprocess_forward(img1, img2, is_uint8, out1, out2, rgb_mean, N, C, H, W, OH, OW, stream, nullptr, 0, false);
+}
+
+extern "C" int mfn_preprocess_forward_det(const void* img1, const void* img2, int is_uint8, float* out1, float* out2,
+                                          float* rgb_mean, int N, int C, int H, int W, int OH, int OW, void* det_ws,
+                                          long long det_ws_bytes, void* stream) {
+  return mfn::preprocess_forward(img1, img2, is_uint8, out1, out2, rgb_mean, N, C, H, W, OH, OW, stream, det_ws,
+                                 det_ws_bytes, true);
 }
 
 extern "C" int mfn_postprocess_forward(const float* pred, float* out, int N, int channels, int Hq, int Wq, int H, int W,

@@ -13,6 +13,7 @@
 // Three kernels: warp_bwd_pre (element-wise part), deform_bwd_input (g_S, scatter to g_x, coordinate gradients) and
 // deform_bwd_weight (g_W as a pixel-reduction GEMM through shared memory), plus a plane reduction for g_b.
 #include "common.cuh"
+#include "det.cuh"
 
 namespace mfn {
 
@@ -119,12 +120,14 @@ constexpr int KB = CB * 9;
 constexpr int FT = 32;
 }  // namespace k4
 
-template <int BORDER, bool SHARED>
+// DET: the scatter into g_x goes to the int64 fixed-point sums gx_acc (det.cuh; bound = max_p sum_f |g_conv|, max |W|)
+template <int BORDER, bool SHARED, bool DET>
 __global__ void __launch_bounds__(k4::NT)
     deform_bwd_input_kernel(const float* __restrict__ gconv, const float* __restrict__ x,
                             const float* __restrict__ offset, const float* __restrict__ flow_up,
                             const float* __restrict__ weight, float* __restrict__ gx, float* __restrict__ gcoord,
-                            int N, int C, int H, int W, int F, int Fpad, float flow_scale, float level_stride) {
+                            int N, int C, int H, int W, int F, int Fpad, float flow_scale, float level_stride,
+                            unsigned long long* __restrict__ gx_acc, const unsigned* __restrict__ bound, int fanin_bits) {
   using namespace k4;
   extern __shared__ __align__(16) float Wt[];  // [KB][Fpad]
   const int tid = threadIdx.x;
@@ -162,6 +165,9 @@ __global__ void __launch_bounds__(k4::NT)
   const float* gc = gconv + (size_t)n * F * plane + pix;
   const float* xn = x + (size_t)n * C * plane;
   float* gxn = gx ? gx + (size_t)n * C * plane : nullptr;
+  unsigned long long* gqn = DET && gx_acc ? gx_acc + (size_t)n * C * plane : nullptr;
+  FixedScale fsc{};
+  if constexpr (DET) fsc = det_scale(bound, 2, fanin_bits);
   const float* offn = SHARED ? nullptr : offset + (size_t)n * 18 * plane + pix;
 
   for (int c0 = 0; c0 < C; c0 += CB) {
@@ -221,7 +227,15 @@ __global__ void __launch_bounds__(k4::NT)
         // dS/dh = d0*(ww0 v00 + ww1 v01) + d1*(ww0 v10 + ww1 v11);  dS/dw = wh0*(dw0 v00 + dw1 v01) + wh1*(dw0 v10 + dw1 v11)
         th = fmaf(gs, hA.d0 * (wA.w0 * v00 + wA.w1 * v01) + hA.d1 * (wA.w0 * v10 + wA.w1 * v11), th);
         tw = fmaf(gs, hA.w0 * (wA.d0 * v00 + wA.d1 * v01) + hA.w1 * (wA.d0 * v10 + wA.d1 * v11), tw);
-        if (gxn) {
+        if constexpr (DET) {
+          if (gqn) {
+            unsigned long long* gq = gqn + (size_t)(c0 + cc) * plane;
+            if (w00 != 0.f) det_scatter(gq + o00, gs * w00, fsc);
+            if (w01 != 0.f) det_scatter(gq + o01, gs * w01, fsc);
+            if (w10 != 0.f) det_scatter(gq + o10, gs * w10, fsc);
+            if (w11 != 0.f) det_scatter(gq + o11, gs * w11, fsc);
+          }
+        } else if (gxn) {
           float* gp = gxn + (size_t)(c0 + cc) * plane;
           if (w00 != 0.f) atomicAdd(gp + o00, gs * w00);
           if (w01 != 0.f) atomicAdd(gp + o01, gs * w01);
@@ -252,13 +266,15 @@ __global__ void __launch_bounds__(k4::NT)
 // ---------------------------------------------------------------------------------------------------------
 // g_W[f][c][tap] += sum_p gconv[f][p] * S[p][c][tap].  CTA = 128 pixels; per (channel block, f tile): every thread
 // samples its pixel into shared memory, then the CTA contracts the 128-pixel axis and issues one atomic per element.
+// DET: CTA b instead stores its whole (F,C,3,3) partial, zeros included, at gw + b*F*C*9; det_ordered_sum_kernel adds the
+// partials in CTA order.  The partition (128 consecutive pixels per CTA) depends on the shape only.
 // ---------------------------------------------------------------------------------------------------------
 namespace k4w {
 constexpr int PX = 128;   // pixels per CTA (= threads)
 constexpr int CB = 4, KB = CB * 9, FT = 32;
 }  // namespace k4w
 
-template <int BORDER, bool SHARED>
+template <int BORDER, bool SHARED, bool DET>
 __global__ void __launch_bounds__(k4w::PX)
     deform_bwd_weight_kernel(const float* __restrict__ gconv, const float* __restrict__ x,
                              const float* __restrict__ offset, const float* __restrict__ flow_up,
@@ -338,7 +354,11 @@ __global__ void __launch_bounds__(k4w::PX)
 #pragma unroll
         for (int i = 0; i < 9; ++i) {
           const int k = kb + 4 * i, c = c0 + k / 9;
-          if (c < C && acc[i] != 0.f) atomicAdd(gw + ((size_t)(f0 + f) * C + c) * 9 + (k % 9), acc[i]);
+          if constexpr (DET) {
+            if (c < C) gw[(size_t)blockIdx.x * F * C * 9 + ((size_t)(f0 + f) * C + c) * 9 + (k % 9)] = acc[i];
+          } else {
+            if (c < C && acc[i] != 0.f) atomicAdd(gw + ((size_t)(f0 + f) * C + c) * 9 + (k % 9), acc[i]);
+          }
         }
       }
     }
@@ -348,74 +368,130 @@ __global__ void __launch_bounds__(k4w::PX)
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
+// Deterministic workspace (maskflow_b200.h, mfn_warp_mask_backward_det): the bound words, the int64 sums of g_x, the
+// per-CTA partials of g_W.
+struct DetK4 {
+  unsigned* bound;
+  unsigned long long* gx_acc;
+  float* gw_part;
+};
+
+static long long det_k4_bytes(int N, int C, int H, int W, int F) {
+  const long long pix = (long long)N * H * W, ctas = (pix + k4w::PX - 1) / k4w::PX;
+  return kDetHeaderBytes + 8 * pix * C + 4 * ctas * F * C * 9;
+}
+
+static DetK4 det_k4_layout(void* ws, int N, int C, int H, int W) {
+  char* b = static_cast<char*>(ws);
+  DetK4 d;
+  d.bound = reinterpret_cast<unsigned*>(b);
+  d.gx_acc = reinterpret_cast<unsigned long long*>(b + kDetHeaderBytes);
+  d.gw_part = reinterpret_cast<float*>(b + kDetHeaderBytes + 8LL * N * C * H * W);
+  return d;
+}
+
 template <int BORDER, bool SHARED>
 static int launch_deform_bwd(const float* gconv, const float* x, const float* offset, const float* flow_up,
                              const float* weight, float* gx, float* gcoord, float* gw, float* gb, int N, int C, int H,
-                             int W, int F, float fs, float ls, cudaStream_t st) {
+                             int W, int F, float fs, float ls, cudaStream_t st, const DetK4* det = nullptr) {
   const long long total = (long long)N * H * W;
+  const long long xsize = total * C;
+  // a g_x element receives at most one contribution per (pixel, tap, corner) of its sample
+  const int fanin_bits = det_bits(36LL * H * W);
+  int rc;
+  if (det && gx) {
+    cudaError_t ce = cudaMemsetAsync(det->bound, 0, kDetHeaderBytes + 8 * xsize, st);
+    if (ce != cudaSuccess) return fail((int)ce, "deterministic K4 backward: cudaMemsetAsync: %s", cudaGetErrorString(ce));
+    if ((rc = det_launch_pixel_abs_sum_max(gconv, N, F, (long long)H * W, det->bound, st))) return rc;
+    if ((rc = det_launch_abs_max(weight, (long long)F * C * 9, det->bound + 1, st))) return rc;
+  }
   if (gx || gcoord) {
     const int Fpad = ((F + k4::FT - 1) / k4::FT) * k4::FT;
     const int smem = (int)sizeof(float) * k4::KB * Fpad;
-    cudaFuncSetAttribute(deform_bwd_input_kernel<BORDER, SHARED>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     const unsigned grid = (unsigned)((total + k4::NT - 1) / k4::NT);
-    deform_bwd_input_kernel<BORDER, SHARED><<<grid, k4::NT, smem, st>>>(gconv, x, offset, flow_up, weight, gx, gcoord,
-                                                                        N, C, H, W, F, Fpad, fs, ls);
-    const int rc = check_launch("deform_bwd_input_kernel");
-    if (rc) return rc;
+    if (det) {
+      cudaFuncSetAttribute(deform_bwd_input_kernel<BORDER, SHARED, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           smem);
+      deform_bwd_input_kernel<BORDER, SHARED, true><<<grid, k4::NT, smem, st>>>(
+          gconv, x, offset, flow_up, weight, nullptr, gcoord, N, C, H, W, F, Fpad, fs, ls, gx ? det->gx_acc : nullptr,
+          det->bound, fanin_bits);
+    } else {
+      cudaFuncSetAttribute(deform_bwd_input_kernel<BORDER, SHARED, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           smem);
+      deform_bwd_input_kernel<BORDER, SHARED, false><<<grid, k4::NT, smem, st>>>(
+          gconv, x, offset, flow_up, weight, gx, gcoord, N, C, H, W, F, Fpad, fs, ls, nullptr, nullptr, 0);
+    }
+    if ((rc = check_launch("deform_bwd_input_kernel"))) return rc;
+    if (det && gx && (rc = det_launch_fixed_to_float(det->gx_acc, gx, xsize, det->bound, 2, fanin_bits, st))) return rc;
   }
   if (gw) {
     const unsigned grid = (unsigned)((total + k4w::PX - 1) / k4w::PX);
-    deform_bwd_weight_kernel<BORDER, SHARED><<<grid, k4w::PX, 0, st>>>(gconv, x, offset, flow_up, gw, N, C, H, W, F,
-                                                                       fs, ls);
-    const int rc = check_launch("deform_bwd_weight_kernel");
-    if (rc) return rc;
+    if (det)
+      deform_bwd_weight_kernel<BORDER, SHARED, true><<<grid, k4w::PX, 0, st>>>(gconv, x, offset, flow_up, det->gw_part, N,
+                                                                               C, H, W, F, fs, ls);
+    else
+      deform_bwd_weight_kernel<BORDER, SHARED, false><<<grid, k4w::PX, 0, st>>>(gconv, x, offset, flow_up, gw, N, C, H,
+                                                                                W, F, fs, ls);
+    if ((rc = check_launch("deform_bwd_weight_kernel"))) return rc;
+    if (det && (rc = det_launch_ordered_sum(det->gw_part, (int)grid, (long long)F * C * 9, 1, gw, (long long)F * C * 9, 1,
+                                            st)))
+      return rc;
   }
   if (gb) {
-    plane_sum_kernel<<<F, 256, 0, st>>>(gconv, gb, N, F, H * W);
+    plane_sum_kernel<<<F, 256, 0, st>>>(gconv, gb, N, F, H * W);   // one atomic per element: already order-independent
     return check_launch("plane_sum_kernel");
   }
   return MFN_OK;
 }
 
-}  // namespace mfn
-
-extern "C" int mfn_deformable_conv_backward(const float* grad_out, const float* data, const float* offset,
-                                            const float* weight, float* grad_data, float* grad_offset,
-                                            float* grad_weight, float* grad_bias, int N, int C, int H, int W, int F,
-                                            int border_mode, void* stream) {
-  using namespace mfn;
-  MFN_REQUIRE(grad_out && data && offset && weight, MFN_ERR_INVALID_ARG, "mfn_deformable_conv_backward: null pointer");
-  MFN_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && F > 0, MFN_ERR_INVALID_ARG,
-              "mfn_deformable_conv_backward: non-positive extent");
+static int deformable_conv_backward(const float* grad_out, const float* data, const float* offset, const float* weight,
+                                    float* grad_data, float* grad_offset, float* grad_weight, float* grad_bias, int N,
+                                    int C, int H, int W, int F, int border_mode, void* stream, void* det_ws,
+                                    long long det_ws_bytes, bool det) {
+  const char* fn = det ? "mfn_deformable_conv_backward_det" : "mfn_deformable_conv_backward";
+  MFN_REQUIRE(grad_out && data && offset && weight, MFN_ERR_INVALID_ARG, "%s: null pointer", fn);
+  MFN_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && F > 0, MFN_ERR_INVALID_ARG, "%s: non-positive extent", fn);
   MFN_REQUIRE(border_mode == MFN_BORDER_MXNET15 || border_mode == MFN_BORDER_ZERO_CORNER, MFN_ERR_INVALID_ARG,
-              "mfn_deformable_conv_backward: unknown border_mode %d", border_mode);
-  MFN_REQUIRE(F <= 1024, MFN_ERR_UNSUPPORTED, "mfn_deformable_conv_backward: F > 1024 not supported");
+              "%s: unknown border_mode %d", fn, border_mode);
+  MFN_REQUIRE(F <= 1024, MFN_ERR_UNSUPPORTED, "%s: F > 1024 not supported", fn);
+  DetK4 d{};
+  if (det) {
+    const int rc = det_check_workspace(fn, det_ws, det_ws_bytes, det_k4_bytes(N, C, H, W, F));
+    if (rc) return rc;
+    d = det_k4_layout(det_ws, N, C, H, W);
+  }
   cudaStream_t st = as_stream(stream);
   if (border_mode == MFN_BORDER_MXNET15)
     return launch_deform_bwd<MFN_BORDER_MXNET15, false>(grad_out, data, offset, nullptr, weight, grad_data,
                                                         grad_offset, grad_weight, grad_bias, N, C, H, W, F, 0.f, 1.f,
-                                                        st);
+                                                        st, det ? &d : nullptr);
   return launch_deform_bwd<MFN_BORDER_ZERO_CORNER, false>(grad_out, data, offset, nullptr, weight, grad_data,
                                                           grad_offset, grad_weight, grad_bias, N, C, H, W, F, 0.f, 1.f,
-                                                          st);
+                                                          st, det ? &d : nullptr);
 }
 
-extern "C" int mfn_warp_mask_backward(const float* grad_out, const float* out, const float* conv_out, const float* x,
-                                      const float* flow_up, const float* mask_up, const float* weight, float* grad_x,
-                                      float* grad_flow_up, float* grad_mask_up, float* grad_weight, float* grad_bias,
-                                      float* grad_tradeoff, float* grad_conv_ws, int N, int C, int H, int W, int F,
-                                      float flow_scale, float level_stride, float leaky_slope, int border_mode,
-                                      void* stream) {
-  using namespace mfn;
+static int warp_mask_backward(const float* grad_out, const float* out, const float* conv_out, const float* x,
+                              const float* flow_up, const float* mask_up, const float* weight, float* grad_x,
+                              float* grad_flow_up, float* grad_mask_up, float* grad_weight, float* grad_bias,
+                              float* grad_tradeoff, float* grad_conv_ws, int N, int C, int H, int W, int F,
+                              float flow_scale, float level_stride, float leaky_slope, int border_mode, void* stream,
+                              void* det_ws, long long det_ws_bytes, bool det) {
+  const char* fn = det ? "mfn_warp_mask_backward_det" : "mfn_warp_mask_backward";
   MFN_REQUIRE(grad_out && out && x && flow_up && weight && grad_conv_ws, MFN_ERR_INVALID_ARG,
-              "mfn_warp_mask_backward: null pointer (grad_conv_ws, an (N,F,H,W) workspace, is required)");
+              "%s: null pointer (grad_conv_ws, an (N,F,H,W) workspace, is required)", fn);
   MFN_REQUIRE(!grad_mask_up || (mask_up && conv_out), MFN_ERR_INVALID_ARG,
-              "mfn_warp_mask_backward: grad_mask_up needs mask_up and conv_out");
+              "%s: grad_mask_up needs mask_up and conv_out", fn);
   MFN_REQUIRE(N > 0 && C > 0 && H > 0 && W > 0 && F > 0 && level_stride > 0.f, MFN_ERR_INVALID_ARG,
-              "mfn_warp_mask_backward: bad extent");
+              "%s: bad extent", fn);
   MFN_REQUIRE(border_mode == MFN_BORDER_MXNET15 || border_mode == MFN_BORDER_ZERO_CORNER, MFN_ERR_INVALID_ARG,
-              "mfn_warp_mask_backward: unknown border_mode %d", border_mode);
-  MFN_REQUIRE(F <= 1024, MFN_ERR_UNSUPPORTED, "mfn_warp_mask_backward: F > 1024 not supported");
+              "%s: unknown border_mode %d", fn, border_mode);
+  MFN_REQUIRE(F <= 1024, MFN_ERR_UNSUPPORTED, "%s: F > 1024 not supported", fn);
+  DetK4 d{};
+  if (det) {
+    const int rc = det_check_workspace(fn, det_ws, det_ws_bytes, det_k4_bytes(N, C, H, W, F));
+    if (rc) return rc;
+    d = det_k4_layout(det_ws, N, C, H, W);
+  }
   cudaStream_t st = as_stream(stream);
   const long long total = (long long)N * H * W;
   long long blocks = (total + 255) / 256;
@@ -427,8 +503,48 @@ extern "C" int mfn_warp_mask_backward(const float* grad_out, const float* out, c
   if (border_mode == MFN_BORDER_MXNET15)
     return launch_deform_bwd<MFN_BORDER_MXNET15, true>(grad_conv_ws, x, nullptr, flow_up, weight, grad_x, grad_flow_up,
                                                        grad_weight, grad_bias, N, C, H, W, F, flow_scale, level_stride,
-                                                       st);
+                                                       st, det ? &d : nullptr);
   return launch_deform_bwd<MFN_BORDER_ZERO_CORNER, true>(grad_conv_ws, x, nullptr, flow_up, weight, grad_x,
                                                          grad_flow_up, grad_weight, grad_bias, N, C, H, W, F,
-                                                         flow_scale, level_stride, st);
+                                                         flow_scale, level_stride, st, det ? &d : nullptr);
+}
+
+}  // namespace mfn
+
+extern "C" int mfn_deformable_conv_backward(const float* grad_out, const float* data, const float* offset,
+                                            const float* weight, float* grad_data, float* grad_offset,
+                                            float* grad_weight, float* grad_bias, int N, int C, int H, int W, int F,
+                                            int border_mode, void* stream) {
+  return mfn::deformable_conv_backward(grad_out, data, offset, weight, grad_data, grad_offset, grad_weight, grad_bias, N,
+                                       C, H, W, F, border_mode, stream, nullptr, 0, false);
+}
+
+extern "C" int mfn_deformable_conv_backward_det(const float* grad_out, const float* data, const float* offset,
+                                                const float* weight, float* grad_data, float* grad_offset,
+                                                float* grad_weight, float* grad_bias, int N, int C, int H, int W, int F,
+                                                int border_mode, void* det_ws, long long det_ws_bytes, void* stream) {
+  return mfn::deformable_conv_backward(grad_out, data, offset, weight, grad_data, grad_offset, grad_weight, grad_bias, N,
+                                       C, H, W, F, border_mode, stream, det_ws, det_ws_bytes, true);
+}
+
+extern "C" int mfn_warp_mask_backward(const float* grad_out, const float* out, const float* conv_out, const float* x,
+                                      const float* flow_up, const float* mask_up, const float* weight, float* grad_x,
+                                      float* grad_flow_up, float* grad_mask_up, float* grad_weight, float* grad_bias,
+                                      float* grad_tradeoff, float* grad_conv_ws, int N, int C, int H, int W, int F,
+                                      float flow_scale, float level_stride, float leaky_slope, int border_mode,
+                                      void* stream) {
+  return mfn::warp_mask_backward(grad_out, out, conv_out, x, flow_up, mask_up, weight, grad_x, grad_flow_up, grad_mask_up,
+                                 grad_weight, grad_bias, grad_tradeoff, grad_conv_ws, N, C, H, W, F, flow_scale,
+                                 level_stride, leaky_slope, border_mode, stream, nullptr, 0, false);
+}
+
+extern "C" int mfn_warp_mask_backward_det(const float* grad_out, const float* out, const float* conv_out, const float* x,
+                                          const float* flow_up, const float* mask_up, const float* weight, float* grad_x,
+                                          float* grad_flow_up, float* grad_mask_up, float* grad_weight,
+                                          float* grad_bias, float* grad_tradeoff, float* grad_conv_ws, int N, int C,
+                                          int H, int W, int F, float flow_scale, float level_stride, float leaky_slope,
+                                          int border_mode, void* det_ws, long long det_ws_bytes, void* stream) {
+  return mfn::warp_mask_backward(grad_out, out, conv_out, x, flow_up, mask_up, weight, grad_x, grad_flow_up, grad_mask_up,
+                                 grad_weight, grad_bias, grad_tradeoff, grad_conv_ws, N, C, H, W, F, flow_scale,
+                                 level_stride, leaky_slope, border_mode, stream, det_ws, det_ws_bytes, true);
 }

@@ -12,6 +12,10 @@ Reference call sites (under /root/reference):
   upsample               network/MaskFlownet.py:35-62
   grid_generator_warp / bilinear_sampler / reconstruction2d   network/layer.py:8-18
   image_warp_concat      network/MaskFlownet.py:308-313
+
+Under torch.use_deterministic_algorithms(True) the ops whose default kernels accumulate with fp32 atomics (the backward of
+deformable_convolution, warp_mask, bilinear_sampler and image_warp_concat, and preprocess) call the *_det entry points
+instead: bit-identical results from run to run, no warning needed (see deterministic()).
 """
 from __future__ import annotations
 
@@ -62,6 +66,32 @@ def _stream():
 def _call(name, dev, *args):
     with torch.cuda.device(dev):
         _lib.call(name, *args, _stream())
+
+
+# ----------------------------------------------------------------------------------------------------------
+# Deterministic mode
+# ----------------------------------------------------------------------------------------------------------
+def deterministic() -> bool:
+    """True under torch.use_deterministic_algorithms(True) (warn_only included): the ops whose default kernels accumulate
+    with fp32 atomics then call their *_det entry points, which give bit-identical results from run to run."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def det_workspace_bytes(op: str, N: int, C: int, H: int, W: int, F: int = 0) -> int:
+    """Bytes of the det_ws workspace of the *_det entry points (include/maskflow_b200.h, "Deterministic mode").
+    op: "warp_mask" / "deformable_conv" (x (N,C,H,W), F filters), "bilinear_sampler" (data (N,C,H,W)), "image_warp_concat"
+    (im2 (N,C,H,W)), "preprocess" (images (N,C,H,W))."""
+    if op in ("warp_mask", "deformable_conv"):
+        return 256 + 8 * N * C * H * W + 4 * F * C * 9 * (-(-N * H * W // 128))
+    if op in ("bilinear_sampler", "image_warp_concat"):
+        return 256 + 8 * N * C * H * W
+    if op == "preprocess":
+        return 256 + 4 * N * C * 64
+    raise MaskflowError(f"det_workspace_bytes: unknown op {op!r}")
+
+
+def _det_ws(nbytes: int, dev):
+    return torch.empty(nbytes, dtype=torch.uint8, device=dev)
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -167,8 +197,12 @@ class _DeformConvFn(torch.autograd.Function):
         goff = torch.empty_like(offset) if need[1] else None
         gw = torch.zeros_like(weight) if need[2] else None
         gb = torch.zeros(Fo, device=x.device, dtype=torch.float32) if (ctx.has_bias and need[3]) else None
-        _call("mfn_deformable_conv_backward", x.device, _p(go), _p(x), _p(offset), _p(weight), _p(gx), _p(goff),
-              _p(gw), _p(gb), N, C, H, W, Fo, int(ctx.border_mode))
+        args = (_p(go), _p(x), _p(offset), _p(weight), _p(gx), _p(goff), _p(gw), _p(gb), N, C, H, W, Fo, int(ctx.border_mode))
+        if deterministic():
+            nb = det_workspace_bytes("deformable_conv", N, C, H, W, Fo)
+            _call("mfn_deformable_conv_backward_det", x.device, *args, _p(_det_ws(nb, x.device)), nb)
+        else:
+            _call("mfn_deformable_conv_backward", x.device, *args)
         return gx, goff, gw, gb, None
 
 
@@ -234,9 +268,14 @@ class _WarpMaskFn(torch.autograd.Function):
         gb = torch.zeros(Fo, device=dev, dtype=torch.float32) if (has_bias and need[4]) else None
         gtrade = torch.empty_like(out) if (has_trade and need[5]) else None
         ws = torch.empty_like(out)
-        _call("mfn_warp_mask_backward", dev, _p(g_out), _p(out), _p(conv_out), _p(x), _p(flow_up),
-              _p(mask_up) if has_mask else None, _p(weight), _p(gx), _p(gflow), _p(gmask), _p(gw), _p(gb), _p(gtrade),
-              _p(ws), N, C, H, W, Fo, float(scale), float(stride), float(slope), int(border_mode))
+        args = (_p(g_out), _p(out), _p(conv_out), _p(x), _p(flow_up), _p(mask_up) if has_mask else None, _p(weight), _p(gx),
+                _p(gflow), _p(gmask), _p(gw), _p(gb), _p(gtrade), _p(ws), N, C, H, W, Fo, float(scale), float(stride),
+                float(slope), int(border_mode))
+        if deterministic():
+            nb = det_workspace_bytes("warp_mask", N, C, H, W, Fo)
+            _call("mfn_warp_mask_backward_det", dev, *args, _p(_det_ws(nb, dev)), nb)
+        else:
+            _call("mfn_warp_mask_backward", dev, *args)
         # gradients arriving on the up-sampled flow / mask outputs join the ones through the warp, then the
         # transposed Upsample brings them to the coarse grid
         gflow_c = gmask_c = None
@@ -394,7 +433,12 @@ class _BilinearSamplerFn(torch.autograd.Function):
         go = go.contiguous()
         gd = torch.zeros_like(d) if ctx.needs_input_grad[0] else None      # accumulated by the kernel
         gg = torch.empty_like(g) if ctx.needs_input_grad[1] else None
-        _call("mfn_bilinear_sampler_backward", d.device, _p(go), _p(d), _p(g), _p(gd), _p(gg), N, C, H, W, OH, OW)
+        args = (_p(go), _p(d), _p(g), _p(gd), _p(gg), N, C, H, W, OH, OW)
+        if deterministic():
+            nb = det_workspace_bytes("bilinear_sampler", N, C, H, W)
+            _call("mfn_bilinear_sampler_backward_det", d.device, *args, _p(_det_ws(nb, d.device)), nb)
+        else:
+            _call("mfn_bilinear_sampler_backward", d.device, *args)
         return gd, gg
 
 
@@ -446,8 +490,12 @@ class _ImageWarpConcatFn(torch.autograd.Function):
             gi2 = torch.zeros_like(i2) if need[1] else None                    # accumulated by the kernel
             gfu = torch.empty((N, 2, H, W), device=i2.device, dtype=torch.float32) if need[2] else None
             gmu = torch.empty((N, 1, H, W), device=i2.device, dtype=torch.float32) if need[3] else None
-            _call("mfn_image_warp_concat_backward", i2.device, _p(g40), _p(i2), _p(fq), _p(mq), _p(gi2), _p(gfu), _p(gmu),
-                  N, Ci, H, W, float(ctx.scale))
+            args = (_p(g40), _p(i2), _p(fq), _p(mq), _p(gi2), _p(gfu), _p(gmu), N, Ci, H, W, float(ctx.scale))
+            if deterministic():
+                nb = det_workspace_bytes("image_warp_concat", N, Ci, H, W)
+                _call("mfn_image_warp_concat_backward_det", i2.device, *args, _p(_det_ws(nb, i2.device)), nb)
+            else:
+                _call("mfn_image_warp_concat_backward", i2.device, *args)
             # the transposed Upsample(4) brings the up-sampled gradients to the quarter-resolution grid
             gfq = _upsample_backward(gfu, 4, 1.0) if need[2] else None
             gmq = _upsample_backward(gmu, 4, 1.0) if need[3] else None
@@ -616,8 +664,12 @@ def preprocess(img1: torch.Tensor, img2: torch.Tensor, out_hw=None):
     o1 = torch.empty((N, C, OH, OW), device=img1.device, dtype=torch.float32)
     o2 = torch.empty_like(o1)
     mean = torch.empty((N, C, 1, 1), device=img1.device, dtype=torch.float32)
-    _call("mfn_preprocess_forward", img1.device, _p(img1), _p(img2), 1 if img1.dtype == torch.uint8 else 0, _p(o1), _p(o2),
-          _p(mean), N, C, H, W, OH, OW)
+    args = (_p(img1), _p(img2), 1 if img1.dtype == torch.uint8 else 0, _p(o1), _p(o2), _p(mean), N, C, H, W, OH, OW)
+    if deterministic():
+        nb = det_workspace_bytes("preprocess", N, C, H, W)
+        _call("mfn_preprocess_forward_det", img1.device, *args, _p(_det_ws(nb, img1.device)), nb)
+    else:
+        _call("mfn_preprocess_forward", img1.device, *args)
     return o1, o2, mean
 
 

@@ -16,6 +16,7 @@ Images arrive as uint8 NCHW arrays / tensors like the reference's (`img / 255.0`
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -40,10 +41,18 @@ def epe_loss_with_mask(pred: torch.Tensor, label: torch.Tensor, mask: torch.Tens
 
 
 class PipelineFlownet:
+    """deterministic=True makes train_batch, do_batch(_mx), validate and predict bit-reproducible: each call runs under
+    torch.use_deterministic_algorithms(True) (restored afterwards), so this library's ops take their *_det kernels and torch
+    picks deterministic cuDNN algorithms.  torch.backends.cudnn.benchmark must stay off (it may pick a different algorithm
+    per run; the pipeline raises if it is on), and the process must be started with CUBLAS_WORKSPACE_CONFIG=:4096:8 (or
+    :16:8) in the environment, which torch requires for deterministic cuBLAS calls."""
     _lr = None
 
     def __init__(self, device=None, network_class: str = "MaskFlownet_S", lr_schedule: Optional[Sequence[Tuple[int, float]]] = None,
-                 multiscale_weights: Sequence[float] = losses.WEIGHTS, q: Optional[float] = None, learning_rate: float = 1e-4):
+                 multiscale_weights: Sequence[float] = losses.WEIGHTS, q: Optional[float] = None, learning_rate: float = 1e-4,
+                 deterministic: bool = False):
+        self.deterministic = bool(deterministic)
+        self._check_deterministic_settings()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         cls = {"MaskFlownet_S": network.MaskFlownetS, "MaskFlownet": network.MaskFlownet}.get(network_class)
         if cls is None:
@@ -58,6 +67,26 @@ class PipelineFlownet:
         self.q = q
         self.lr_schedule = list(lr_schedule) if lr_schedule is not None else []
         self._bucket: Optional[mdist.GradBucket] = None
+
+    # ---- deterministic mode -------------------------------------------------------------------------------------
+    def _check_deterministic_settings(self) -> None:
+        if self.deterministic and torch.backends.cudnn.benchmark:
+            raise MaskflowError("PipelineFlownet(deterministic=True): torch.backends.cudnn.benchmark is on; benchmark mode "
+                                "may pick a different convolution algorithm in every run -- turn it off")
+
+    @contextlib.contextmanager
+    def _determinism(self):
+        """torch.use_deterministic_algorithms(True) for the duration of one call when the pipeline is deterministic."""
+        if not self.deterministic:
+            yield
+            return
+        self._check_deterministic_settings()
+        prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
+        torch.use_deterministic_algorithms(True)
+        try:
+            yield
+        finally:
+            torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
 
     # ---- checkpoints, schedule ---------------------------------------------------------------------------------
     def save(self, prefix: str) -> None:
@@ -122,6 +151,10 @@ class PipelineFlownet:
         order (flipped to the network's (y,x) after the augmentation, pipeline.py:106), mask (n,1,H,W) uint8 or None.
         global_batch: the batch size over ALL ranks (default: n * world size) -- what Trainer.step(batch_size) divides by.
         Returns {"epe": mean EPE of THIS rank's samples} (the reference averages over its context list in one process)."""
+        with self._determinism():
+            return self._train_batch(img1, img2, label, geo_aug, color_aug, mask, global_batch)
+
+    def _train_batch(self, img1, img2, label, geo_aug, color_aug, mask, global_batch) -> Dict[str, float]:
         dev = self.device
         n = img1.shape[0]
         if mask is None:
@@ -152,11 +185,16 @@ class PipelineFlownet:
     def do_batch_mx(self, img1, img2, resize=None):
         """img1 / img2 in [0,1] float32 (or uint8): centralize, resize to multiples of 64 (or `resize`), network."""
         H, W = img1.shape[2:]
-        a, b, _ = ops.preprocess(img1.contiguous(), img2.contiguous(), ops.padded_size(H, W, resize))
-        return self.network(a, b)
+        with self._determinism():
+            a, b, _ = ops.preprocess(img1.contiguous(), img2.contiguous(), ops.padded_size(H, W, resize))
+            return self.network(a, b)
 
     @torch.no_grad()
     def do_batch(self, img1, img2, label=None, mask=None, resize=None):
+        with self._determinism():
+            return self._do_batch(img1, img2, label, mask, resize)
+
+    def _do_batch(self, img1, img2, label, mask, resize):
         H, W = img1.shape[2:]
         self.network.eval()
         flows, occ_masks, _ = self.do_batch_mx(img1, img2, resize=resize)

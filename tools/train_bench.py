@@ -3,14 +3,18 @@
 
     python tools/train_bench.py --hw 384x512 --batch 8 --steps 5
     torchrun --nproc-per-node 2 tools/train_bench.py --hw 576x960 --batch 8 --steps 5     (global batch = 8 * world)
-    python tools/train_bench.py --network MaskFlownet --hw 320x768 --batch 4 --steps 10 [--fix-head]
+    python tools/train_bench.py --network MaskFlownet --hw 320x768 --batch 4 --steps 10 [--fix-head] [--deterministic]
 
 --network MaskFlownet trains the cascade (the reference's cascade training shape is 320x768, batch 4); --fix-head freezes
-its MaskFlownet-S head and gives Adam only the trainable parameters, as PipelineFlownet.fix_head does.
+its MaskFlownet-S head and gives Adam only the trainable parameters, as PipelineFlownet.fix_head does.  --deterministic runs
+the steps under torch.use_deterministic_algorithms(True) (PipelineFlownet(deterministic=True)): the bit-reproducible
+kernels, deterministic cuDNN algorithms, cudnn.benchmark off; CUBLAS_WORKSPACE_CONFIG defaults to :4096:8.
 
 Prints one JSON line: ms/step, pairs/s, time of the hand-written backward kernels (CUDA events) and of the all-reduce.
 """
 import argparse, json, os, sys, time
+if "--deterministic" in sys.argv:                           # must be set before CUDA initialises
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from maskflownet_b200 import _lib, dist as mdist, losses, network
@@ -24,6 +28,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--network", choices=("MaskFlownet_S", "MaskFlownet"), default="MaskFlownet_S")
     ap.add_argument("--fix-head", action="store_true", help="freeze the cascade's MaskFlownet-S head (MaskFlownet only)")
+    ap.add_argument("--deterministic", action="store_true", help="bit-reproducible steps (torch.use_deterministic_algorithms)")
     a = ap.parse_args()
     if a.fix_head and a.network != "MaskFlownet":
         ap.error("--fix-head needs --network MaskFlownet (only the cascade has a head)")
@@ -33,7 +38,9 @@ def main():
     dev = torch.device("cuda", local)
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.benchmark = True
+    torch.backends.cudnn.benchmark = not a.deterministic
+    if a.deterministic:
+        torch.use_deterministic_algorithms(True)
     torch.manual_seed(0)
     model = (network.MaskFlownet() if a.network == "MaskFlownet" else network.MaskFlownetS()).to(dev).train()
     if a.fix_head:                                          # PipelineFlownet.fix_head (network/MaskFlownet.py:412-414)
@@ -77,7 +84,8 @@ def main():
     ms = mdist.max_over_ranks(s0.elapsed_time(s1), dev) / a.steps
     ar = sum(x.elapsed_time(y) for x, y in t_ar) / len(t_ar)
     if rank == 0:
-        print(json.dumps({"bench": "train_step", "network": a.network, "fix_head": a.fix_head, "hw": a.hw, "batch_per_gpu": a.batch, "n_gpus": world,
+        print(json.dumps({"bench": "train_step", "network": a.network, "fix_head": a.fix_head,
+                          "deterministic": a.deterministic, "hw": a.hw, "batch_per_gpu": a.batch, "n_gpus": world,
                           "ms_per_step": round(ms, 3), "pairs_per_s": round(a.batch * world / ms * 1e3, 2),
                           "native_launches_per_step": (_lib.launch_count() - n0) // a.steps,
                           "grad_allreduce_ms": round(ar, 4), "grad_bucket_mb": round(bucket.numel * 4 / 1e6, 1),
