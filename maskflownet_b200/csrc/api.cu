@@ -59,6 +59,7 @@ extern "C" int mfn_set_tuning(const char* key, int value) {
   else if (!strcmp(key, "corr_ts_lo")) mfn::tuning().corr_ts_lo = value;
   else if (!strcmp(key, "corr_ts_hi")) mfn::tuning().corr_ts_hi = value;
   else if (!strcmp(key, "corr_dbg")) mfn::tuning().corr_dbg = value;
+  else if (!strcmp(key, "conv_dbg")) mfn::tuning().conv_dbg = value;
   else if (!strcmp(key, "corr_ring_th")) mfn::tuning().corr_ring_th = value;
   else if (!strcmp(key, "conv_wgmma")) mfn::tuning().conv_wgmma = value;
   else if (!strcmp(key, "conv_grid_cap")) mfn::tuning().conv_grid_cap = value;

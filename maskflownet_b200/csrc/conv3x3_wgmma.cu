@@ -15,7 +15,8 @@
 //     one thread with 1-D bulk copies (cp.async.bulk + mbarrier complete_tx) through a deep ring (up to 24 stages).
 //   * two consumer warpgroups, one per output row, each issue m64nNk16 MMAs (bf16 x bf16 -> fp32) for the two 64-pixel
 //     halves of their row; after each tap's group they wait for the previous group and release the weight / input
-//     stages it read, and at the end of a tile apply bias + LeakyReLU from registers and store NCHW -- or, for the
+//     stages it read, and at the end of a tile apply bias + LeakyReLU and store NCHW -- through shared-memory staging
+//     rows and asynchronous bulk copies when the output rows are 16-byte aligned, else from registers -- or, for the
 //     transposed convolutions, scatter 2x2 sub-pixel phases (depth-to-space).
 //   * layers wider than 128 output channels are cut into two 128-channel work items per tile (register budget).
 #include "mma_tiles.cuh"
@@ -53,10 +54,9 @@ __host__ __device__ inline int tap_xoff(int kx, int stride, int dil) {
 // first / last row and column and the four corner pixels that the MXNet-1.5 border rule needs.  Maps a virtual
 // coordinate to the real one, or -1 (zero).
 __host__ __device__ inline int band_map(int v, int n) { return v < n ? v : (v == n + 2 ? 0 : (v == n + 5 ? n - 1 : -1)); }
-// output channels padded to an MMA width this file instantiates (16 / 32 / 64 / 96 / 128); wider layers to 256 = 2 x 128
-__host__ __device__ inline int cout_pad(int cout) {
-  return cout <= 16 ? 16 : (cout <= 32 ? 32 : (cout <= 64 ? 64 : (cout <= 96 ? 96 : (cout <= 128 ? 128 : 256))));
-}
+// output channels padded to the next multiple of 16 up to 128 (the MMA widths this file instantiates); wider layers to
+// 256 = 2 x 128
+__host__ __device__ inline int cout_pad(int cout) { return cout <= 128 ? (cout + 15) / 16 * 16 : 256; }
 // Narrow layers (N <= 64) fold the hi / lo weight images into ONE operand of 2N rows:
 //   D[:, 0:2N] += A_hi x [B_hi ; B_lo]      (N' = 2N)        D[:, 0:N] += A_lo x B_hi
 // two MMAs per product instead of three, and one A read fewer from shared memory; the epilogue adds the two column blocks.
@@ -95,6 +95,16 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// shared -> global bulk copy (async proxy), tracked per issuing thread in bulk groups
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 // wgmma shared-memory descriptor, no swizzle (layout type 0), K-major: 8-row x 16-byte core matrices; SBO = distance
 // between 8-row groups (M/N direction), LBO = distance between the two 8-element K groups of one k16 MMA.
 __device__ __forceinline__ uint64_t desc_hi(uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -130,6 +140,15 @@ __device__ __forceinline__ void wgmma_n32(float (&d)[S], uint64_t a, uint64_t b,
       : "l"(a), "l"(b), "r"(scale_d));
 }
 template <int S>
+__device__ __forceinline__ void wgmma_n48(float (&d)[S], uint64_t a, uint64_t b, uint32_t scale_d) {
+  static_assert(S >= 24, "accumulator too small");
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+template <int S>
 __device__ __forceinline__ void wgmma_n64(float (&d)[S], uint64_t a, uint64_t b, uint32_t scale_d) {
   static_assert(S >= 32, "accumulator too small");
   asm volatile(
@@ -139,12 +158,30 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[S], uint64_t a, uint64_t b,
       : "l"(a), "l"(b), "r"(scale_d));
 }
 template <int S>
+__device__ __forceinline__ void wgmma_n80(float (&d)[S], uint64_t a, uint64_t b, uint32_t scale_d) {
+  static_assert(S >= 40, "accumulator too small");
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+template <int S>
 __device__ __forceinline__ void wgmma_n96(float (&d)[S], uint64_t a, uint64_t b, uint32_t scale_d) {
   static_assert(S >= 48, "accumulator too small");
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+template <int S>
+__device__ __forceinline__ void wgmma_n112(float (&d)[S], uint64_t a, uint64_t b, uint32_t scale_d) {
+  static_assert(S >= 56, "accumulator too small");
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
       : "l"(a), "l"(b), "r"(scale_d));
 }
 template <int S>
@@ -160,8 +197,11 @@ template <int N, int S>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[S], uint64_t a, uint64_t b, uint32_t scale_d) {
   if constexpr (N == 16) wgmma_n16(d, a, b, scale_d);
   else if constexpr (N == 32) wgmma_n32(d, a, b, scale_d);
+  else if constexpr (N == 48) wgmma_n48(d, a, b, scale_d);
   else if constexpr (N == 64) wgmma_n64(d, a, b, scale_d);
+  else if constexpr (N == 80) wgmma_n80(d, a, b, scale_d);
   else if constexpr (N == 96) wgmma_n96(d, a, b, scale_d);
+  else if constexpr (N == 112) wgmma_n112(d, a, b, scale_d);
   else wgmma_n128(d, a, b, scale_d);
 }
 
@@ -177,6 +217,7 @@ struct SplitK {
   uint32_t magic_tp, magic_tx;
   int as_wide;   // input stages of the wide (single-tap weight stage) layers: 3 or 2 (smem_map)
   int ns;        // output-channel halves per tile: 1, or 2 for CoutP = 256
+  int stg;       // bytes of the staged epilogue's shared-memory rows; 0: whole tiles store from registers
 };
 __device__ __forceinline__ void decode_tile(int tile, int tilesX, int tilesY, const SplitK& sk, int& tx, int& ty, int& n) {
   if (sk.magic_tp) {
@@ -213,15 +254,20 @@ __device__ __forceinline__ Work decode_work(int w, const SplitK& sk, int nChunks
 }
 
 struct SmemMap {
-  int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, total, AS, WS;
+  int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, stg_off, total, AS, WS;
 };
-// stage counts from the shared-memory budget: 3 input stages when that still leaves >= 8 weight stages, else 2
-__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3) {
+// staged epilogue: per consumer warpgroup STG_CH output channels x MT pixels of fp32, row pitch SPITCH floats (the 4-float
+// pad makes the fragment stores bank-conflict-free and keeps every row 16-byte aligned for the bulk copies)
+constexpr int STG_CH = 32, SPITCH = MT + 4;
+constexpr int STG_BYTES = R * STG_CH * SPITCH * 4;
+// stage counts from the shared-memory budget: 3 input stages when that still leaves >= 8 weight stages, else 2.
+// stg: bytes of the epilogue staging rows (0 = the layer stores from registers)
+__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0) {
   SmemMap m;
   m.a_lo = 2 * E * 16;              // hi image: two 8-channel planes of E entries
   m.a_stage = 2 * m.a_lo;           // hi + lo
   m.w_tile = 64 * CoutP;            // [hi | lo][2 planes][CoutP][16 B]
-  const int budget = 227 * 1024 - BAR_BYTES;
+  const int budget = 227 * 1024 - BAR_BYTES - stg;
   m.w_stage = taps_per_stage(CoutP) * m.w_tile;
   // input stages: narrow layers (several taps per weight stage) take 4 when >= 4 weight stages still fit; wide layers keep
   // the weight ring deep (their weight stages are single taps) and take 3
@@ -233,7 +279,8 @@ __host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3) {
   m.WS = ws > MAX_WS ? MAX_WS : ws;
   m.w_off = m.AS * m.a_stage;
   m.bar_off = m.w_off + m.WS * m.w_stage;
-  m.total = m.bar_off + BAR_BYTES;
+  m.stg_off = m.bar_off + BAR_BYTES;
+  m.total = m.stg_off + stg;
   return m;
 }
 }  // namespace um
@@ -276,7 +323,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
     conv3x3_wgmma_kernel(const float* __restrict__ x, long long x_bs, const unsigned char* __restrict__ wpack,
                          const float* __restrict__ bias_arg, float* __restrict__ out_base, long long out_bs, int Cin, int H, int W,
                          int OH, int OW, int Cout, int CoutP, int nChunks, float slope_arg, int tilesX, int tilesY, int numWork,
-                         int stride, int dil, int out_mode_arg, int ext, um::SplitK sk) {
+                         int stride, int dil, int out_mode_arg, int ext, um::SplitK sk, int dbg) {
   using namespace um;
   // out_mode_arg = mode | (linear_prefix << 8): the first linear_prefix output channels are written WITHOUT the activation
   // (a second, linear head sharing the input pass of an activated layer: network.py folds pred_flow / pred_mask over the
@@ -284,11 +331,13 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   // Split-K (sk.k > 1): `numWork` counts WORK ITEMS.  Items below sk.from are whole tiles; the tiles from sk.from on are
   // cut into sk.k parts over the channel chunks -- part p walks chunks [p nChunks / k, (p + 1) nChunks / k) and writes its
   // RAW partial sums (no bias, no activation) to the workspace; conv3x3_wgmma_reduce_kernel finishes that region.
+  // dbg (tuning "conv_dbg", profiling only, results invalid): 2 = producers skip their global loads, 4 = no epilogue
+  // stores, 8 = no MMAs; the barrier protocol is unchanged, so each phase can be timed by removing it.
   constexpr int NCOL = FOLD ? NW / 2 : NW;   // output channels per work item
   const int out_mode_k = out_mode_arg & 0xff, lin_prefix_k = out_mode_arg >> 8;
   extern __shared__ __align__(128) unsigned char smem[];
   const int nslots = n_slots(stride, dil), PW = row_pitch(stride, dil), E = nslots * PW;
-  const SmemMap sm = smem_map(E, CoutP, sk.as_wide);
+  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg);
   const int AS = sm.AS, WS = sm.WS;
   const uint32_t s_base = smem_u32(smem);
   const uint32_t bar0 = s_base + sm.bar_off;
@@ -341,7 +390,22 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
       const uint32_t b_nh16 = (uint32_t)(wk.nh * NCOL);   // first weight row of this channel half (16 B rows)
       fence_acc(acc[0]);
       fence_acc(acc[1]);
-      for (int c = cb; c < ce; ++c) {
+      if (dbg & 8) {   // profiling: the same barrier traffic without MMAs
+        for (int c = cb; c < ce; ++c) {
+          mbar_wait(a_full + 8 * as, aph);
+          for (int tap = 0; tap < 9; ++tap) {
+            if (tap % TPS == 0) mbar_wait(w_full + 8 * ws, wph);
+            release();
+            if (tap % TPS == TPS - 1) {
+              rel_w = (int)ws;
+              if (++ws == (uint32_t)WS) { ws = 0; wph ^= 1; }
+            }
+            if (tap == 8) rel_a = (int)as;
+          }
+          if (++as == (uint32_t)AS) { as = 0; aph ^= 1; }
+        }
+      }
+      for (int c = (dbg & 8) ? ce : cb; c < ce; ++c) {
         mbar_wait(a_full + 8 * as, aph);
         const uint32_t a_st16 = s_base16 + as * a_stage16;
 #pragma unroll
@@ -396,7 +460,49 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
       const int y = ty * R + r;
       const int F = Cout >> 2;
       const size_t oplane2 = (size_t)(2 * OH) * (2 * OW);
-      if (y < OH) {
+      if (y < OH && !(dbg & 4) && sk.stg && !partial) {
+        // staged epilogue (plain NCHW output, 16-byte aligned rows): SCH channels at a time, the warpgroup writes
+        // bias + LeakyReLU'ed values into its staging rows ([channel][pixel], pitch SPITCH: conflict-free), and one thread
+        // per channel hands the row segment to a bulk copy (full 128-byte lines, asynchronous: the global writes drain
+        // while the next work item's MMAs run).  A piece waits only until the copies of the previous one have READ it.
+        constexpr int SCH = NCOL % STG_CH == 0 ? STG_CH : 16;   // channels per piece (divides NCOL: a multiple of 16)
+        float* const stg = reinterpret_cast<float*>(smem + sm.stg_off) + r * STG_CH * SPITCH;
+        const int t = wq * 32 + lane;   // thread of this warpgroup
+        const int x0 = tx * MT;
+        const uint32_t seg = (uint32_t)((OW - x0 < MT ? OW - x0 : MT) * 4);
+#pragma unroll
+        for (int pc = 0; pc < NCOL / SCH; ++pc) {
+          if (t < SCH) bulk_wait_read();                  // this thread's previous copies have read the staging rows
+          named_bar_sync(1 + r, 128);
+#pragma unroll
+          for (int jj = 0; jj < SCH / 8; ++jj) {
+            const int j = pc * (SCH / 8) + jj;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int f = wk.nh * NCOL + 8 * j + 2 * (lane & 3) + e;
+              const float b = (bias != nullptr && f < Cout) ? __ldg(bias + f) : 0.f;
+              const float sl = f < lin_prefix ? 1.f : slope;
+              float* const row = stg + (8 * jj + 2 * (lane & 3) + e) * SPITCH + 16 * wq + (lane >> 2);
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int i = 4 * j + 2 * h + e;
+                  float v = acc[mh][i];
+                  if constexpr (FOLD) v += acc[mh][i + NW / 4];
+                  row[64 * mh + 8 * h] = leaky(v + b, sl);
+                }
+            }
+          }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the copy
+          named_bar_sync(1 + r, 128);
+          const int f = wk.nh * NCOL + pc * SCH + t;
+          if (t < SCH && f < Cout) {
+            bulk_s2g(out + (size_t)f * oplane0 + (size_t)y * OW + x0, smem_u32(stg + t * SPITCH), seg);
+            bulk_commit();
+          }
+        }
+      } else if (y < OH && !(dbg & 4)) {
 #pragma unroll
         for (int mh = 0; mh < 2; ++mh) {
 #pragma unroll
@@ -427,6 +533,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         }
       }
     }
+    bulk_wait_all();   // the staged epilogue's last copies have completed before the CTA (and its shared memory) ends
   } else if (warp == 8) {
     // ============================ weight loader (one thread) ============================
     if (lane == 0) {
@@ -512,7 +619,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           y = y >= 0 ? band_map(y, H) : -1;
           xx = xx >= 0 ? band_map(xx, W) : -1;
         }
-        const bool ok = t < nItems && e < E && (unsigned)y < (unsigned)H && (unsigned)xx < (unsigned)W;
+        const bool ok = t < nItems && e < E && (unsigned)y < (unsigned)H && (unsigned)xx < (unsigned)W && !(dbg & 2);
         const int c0 = 16 * l_c + 8 * kc;
         uint32_t off = (uint32_t)(8 * kc) * planeu + (ok ? (uint32_t)(y * W + xx) : 0u);
         if (c0 + 8 <= Cin) {
@@ -677,18 +784,24 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const int CoutP = um::cout_pad(Cout), nChunks = (Cin + 15) / 16;
   const int E = n_slots(stride, dil) * row_pitch(stride, dil);
   const int as_wide = tuning().conv_as == 2 ? 2 : 3;
-  const SmemMap sm = smem_map(E, CoutP, as_wide);
-  if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
-  if ((long long)H * W >= (1LL << 27)) return -1;   // the producers address a 16-plane chunk with 32-bit element offsets
   const int grow = ext == 2 ? 8 : 2 * ext;   // ext 1: grid + 1 pixel per side; ext 2: + the six band rows / columns too
   const int OH = stride == 2 ? (H - 1) / 2 + 1 : H + grow, OW = stride == 2 ? (W - 1) / 2 + 1 : W + grow;
-  static SmemOptIn opt16, opt32, opt64, opt96, opt128;
+  // staged epilogue (bulk copies of whole output row segments): plain NCHW output whose rows start 16-byte aligned
+  const bool staged = (out_mode & 0xff) == 0 && ext == 0 && OW % 4 == 0 && out_bs % 4 == 0 && aligned(out, 16) &&
+                      smem_map(E, CoutP, as_wide, STG_BYTES).WS >= 2;
+  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0);
+  if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
+  if ((long long)H * W >= (1LL << 27)) return -1;   // the producers address a 16-plane chunk with 32-bit element offsets
+  static SmemOptIn opt[8];
   {
-    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9>, sm.total, opt16);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 9>, sm.total, opt32);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, true, 3>, sm.total, opt64);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1>, sm.total, opt96);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1>, sm.total, opt128);
+    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9>, sm.total, opt[0]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 9>, sm.total, opt[1]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, true, 3>, sm.total, opt[2]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, true, 3>, sm.total, opt[3]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1>, sm.total, opt[4]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1>, sm.total, opt[5]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1>, sm.total, opt[6]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1>, sm.total, opt[7]);
     if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(conv3x3_wgmma_kernel): %s", cudaGetErrorString(e));
   }
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;
@@ -704,6 +817,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const long long tiles = (long long)N * tilesX * tilesY;
   if (tiles * ns >= (1LL << 30)) return -1;
   sk.as_wide = as_wide;
+  sk.stg = staged ? STG_BYTES : 0;
   if (sk.k <= 1) sk.from = (int)tiles;
   {
     const unsigned long long tp = (unsigned long long)tilesX * tilesY;
@@ -719,14 +833,23 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
 #define MFN_WGMMA_LAUNCH(NW_, FOLD_, TPS_)                                                                                   \
   conv3x3_wgmma_kernel<NW_, FOLD_, TPS_><<<grid, NTHREADS, sm.total, st>>>(x, x_bs, wpack, bias, out, out_bs, Cin, H, W, OH, \
                                                                            OW, Cout, CoutP, nChunks, slope, tilesX, tilesY,  \
-                                                                           (int)numWork, stride, dil, out_mode, ext, sk)
-  if (CoutP == 16) MFN_WGMMA_LAUNCH(32, true, 9);
-  else if (CoutP == 32) MFN_WGMMA_LAUNCH(64, true, 9);
-  else if (CoutP == 64) MFN_WGMMA_LAUNCH(128, true, 3);
-  else if (CoutP == 96) MFN_WGMMA_LAUNCH(96, false, 1);
-  else MFN_WGMMA_LAUNCH(128, false, 1);
+                                                                           (int)numWork, stride, dil, out_mode, ext, sk,     \
+                                                                           tuning().conv_dbg)
+  // variant name (last_kernel): the padded output width, and whether the hi / lo weight images are folded
+  const char* name = "conv3x3_wgmma_kernel<CoutP=256>";
+  switch (CoutP) {
+    case 16: MFN_WGMMA_LAUNCH(32, true, 9); name = "conv3x3_wgmma_kernel<CoutP=16,fold>"; break;
+    case 32: MFN_WGMMA_LAUNCH(64, true, 9); name = "conv3x3_wgmma_kernel<CoutP=32,fold>"; break;
+    case 48: MFN_WGMMA_LAUNCH(96, true, 3); name = "conv3x3_wgmma_kernel<CoutP=48,fold>"; break;
+    case 64: MFN_WGMMA_LAUNCH(128, true, 3); name = "conv3x3_wgmma_kernel<CoutP=64,fold>"; break;
+    case 80: MFN_WGMMA_LAUNCH(80, false, 1); name = "conv3x3_wgmma_kernel<CoutP=80>"; break;
+    case 96: MFN_WGMMA_LAUNCH(96, false, 1); name = "conv3x3_wgmma_kernel<CoutP=96>"; break;
+    case 112: MFN_WGMMA_LAUNCH(112, false, 1); name = "conv3x3_wgmma_kernel<CoutP=112>"; break;
+    case 128: MFN_WGMMA_LAUNCH(128, false, 1); name = "conv3x3_wgmma_kernel<CoutP=128>"; break;
+    default: MFN_WGMMA_LAUNCH(128, false, 1);   // 256: two 128-channel halves per tile
+  }
 #undef MFN_WGMMA_LAUNCH
-  const int rc = check_launch("conv3x3_wgmma_kernel");
+  const int rc = check_launch(name);
   if (rc != 0 || sk.k <= 1) return rc;
   const long long total = sk.part_stride;
   long long blocks = (total + 255) / 256;
