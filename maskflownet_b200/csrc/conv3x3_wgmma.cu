@@ -23,9 +23,6 @@
 
 namespace mfn {
 namespace um {
-using c3::smem_u32;
-using c3::split_pair;
-
 constexpr int MT = 128;          // pixels per tile row (two 64-row wgmma M blocks)
 constexpr int R = 2;             // output rows per CTA tile
 constexpr int NTHREADS = 384;    // warps 0..3: row-0 warpgroup, 4..7: row-1 warpgroup, 8: weight loader, 9..11: producers
@@ -67,44 +64,6 @@ __host__ __device__ inline bool fold_hi_lo(int CoutP) { return CoutP <= 64; }
 // per bulk copy.
 __host__ __device__ inline int taps_per_stage(int CoutP) { return CoutP <= 32 ? 9 : (CoutP <= 64 ? 3 : 1); }
 
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes)
-               : "memory");
-}
-// Bounded wait (2^28 polls, each of which suspends for the hardware's try_wait window): a protocol bug fails the launch
-// with a trap instead of hanging the device.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (!done && ++spins > (1u << 28)) __trap();
-  }
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
-// shared -> global bulk copy (async proxy), tracked per issuing thread in bulk groups
-__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 // wgmma shared-memory descriptor, no swizzle (layout type 0), K-major: 8-row x 16-byte core matrices; SBO = distance
 // between 8-row groups (M/N direction), LBO = distance between the two 8-element K groups of one k16 MMA.
 __device__ __forceinline__ uint64_t desc_hi(uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -302,7 +261,7 @@ __global__ void conv3x3_pack_wgmma_kernel(const float* __restrict__ w, unsigned 
       if (ch + 1 < Cin) b = w[((size_t)f * Cin + ch + 1) * 9 + tap];
     }
     uint32_t hi, lo;
-    c3::split_pair(a, b, hi, lo);
+    split_pair(a, b, hi, lo);
     const int wt = 64 * CoutP;
     unsigned char* tile = packed + ((size_t)c * 9 + tap) * wt;
     if (um::fold_hi_lo(CoutP)) {   // [8-channel plane][hi rows | lo rows][16 B]

@@ -17,6 +17,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace mfn {
 
@@ -177,49 +178,6 @@ __host__ __device__ constexpr int halo_rows(int md) { return TH + 2 * md; }
 __host__ __device__ constexpr int stage_bytes(int md) { return halo_rows(md) * HWP * RS * 2; }  // hi + lo
 __host__ __device__ constexpr int smem_bytes(int md) {
   return 2 * stage_bytes(md) + NCONS * (2 * md + 1) * STG_STRIDE * 4 + 64;
-}
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {   // bounded: traps instead of hanging
-  uint32_t ok, spins = 0;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (!ok && ++spins > (1u << 28)) __trap();
-  } while (!ok);
-}
-
-// (a, b) fp32 -> packed bf16x2 "hi" (a in the low half) and the bf16x2 of the remainders "lo".
-__device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
-  const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - bh), "f"(a - ah));
-}
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr)
-               : "memory");
-}
-
-__device__ __forceinline__ void mma_bf16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
-                                         uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 }  // namespace tc
 
@@ -388,12 +346,13 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1)
             ldsm_x4(st + rowoff + off12 + LO_OFF, l);
             ldsm_x4(st + rowoff + off3, x3);
             // tile 0: rows = blocks 0,1 ; tile 1: rows = blocks 1,2
-            mma_bf16(acc[d][0], h[0], h[1], h[2], h[3], bl[kk][0][0], bl[kk][0][1]);
-            mma_bf16(acc[d][0], l[0], l[1], l[2], l[3], bh[kk][0][0], bh[kk][0][1]);
-            mma_bf16(acc[d][0], h[0], h[1], h[2], h[3], bh[kk][0][0], bh[kk][0][1]);
-            mma_bf16(acc[d][1], h[1], x3[0], h[3], x3[1], bl[kk][1][0], bl[kk][1][1]);
-            mma_bf16(acc[d][1], l[1], x3[2], l[3], x3[3], bh[kk][1][0], bh[kk][1][1]);
-            mma_bf16(acc[d][1], h[1], x3[0], h[3], x3[1], bh[kk][1][0], bh[kk][1][1]);
+            const uint32_t h1[4] = {h[1], x3[0], h[3], x3[1]}, l1[4] = {l[1], x3[2], l[3], x3[3]};
+            mma_bf16(acc[d][0], h, bl[kk][0][0], bl[kk][0][1]);
+            mma_bf16(acc[d][0], l, bh[kk][0][0], bh[kk][0][1]);
+            mma_bf16(acc[d][0], h, bh[kk][0][0], bh[kk][0][1]);
+            mma_bf16(acc[d][1], h1, bl[kk][1][0], bl[kk][1][1]);
+            mma_bf16(acc[d][1], l1, bh[kk][1][0], bh[kk][1][1]);
+            mma_bf16(acc[d][1], h1, bh[kk][1][0], bh[kk][1][1]);
           }
         }
         __syncwarp();
@@ -451,13 +410,6 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1)
 // configs[1]: 64 strips x 2 pieces of 7 tiles = 128 CTAs), so only the first tile of a CTA loads its full halo.
 // =====================================================================================================
 namespace r4 {
-using tc::ldsm_x4;
-using tc::mma_bf16;
-using tc::smem_u32;
-using tc::split_pair;
-using tc::mbar_init;
-using tc::mbar_arrive;
-using tc::mbar_wait;
 // Two shapes, selected by the tile height TH (template parameter of the kernel):
 //   TH = 8: 16 warps, 1 CTA per SM, 24-row ring, two data1 stages (the original shape)
 //   TH = 4:  8 warps, 2 CTAs per SM (<= 113 KB shared memory and 128 registers each), 16-row ring, one data1 stage
@@ -476,7 +428,6 @@ __host__ __device__ constexpr int stg_group_bytes(int md) { return 2 * PASS * (2
 __host__ __device__ constexpr int smem_bytes(int md, int th) {
   return 2 * ring_rows(th) * ROW_BYTES + f1_stages(th) * 2 * th * F1_ROW_BYTES + (th / 2) * stg_group_bytes(md) + 16;
 }
-__device__ __forceinline__ int swz(int p, int c) { return p * PXB + ((c ^ ((p >> 1) & 3)) << 4); }
 }  // namespace r4
 
 template <int MD, bool VEC, int TH>
@@ -843,15 +794,15 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
           uint32_t(&fl)[4] = al[st & 1];
           if (useA) {
             float(&a)[4] = acc[0][hh < PASS ? hh : 0];
-            mma_bf16(a, fh[0], fh[1], fh[2], fh[3], bq[0][kk][2], bq[0][kk][3]);
-            mma_bf16(a, fl[0], fl[1], fl[2], fl[3], bq[0][kk][0], bq[0][kk][1]);
-            mma_bf16(a, fh[0], fh[1], fh[2], fh[3], bq[0][kk][0], bq[0][kk][1]);
+            mma_bf16(a, fh, bq[0][kk][2], bq[0][kk][3]);
+            mma_bf16(a, fl, bq[0][kk][0], bq[0][kk][1]);
+            mma_bf16(a, fh, bq[0][kk][0], bq[0][kk][1]);
           }
           if (useB) {
             float(&a)[4] = acc[1][hh >= 1 ? hh - 1 : 0];
-            mma_bf16(a, fh[0], fh[1], fh[2], fh[3], bq[1][kk][2], bq[1][kk][3]);
-            mma_bf16(a, fl[0], fl[1], fl[2], fl[3], bq[1][kk][0], bq[1][kk][1]);
-            mma_bf16(a, fh[0], fh[1], fh[2], fh[3], bq[1][kk][0], bq[1][kk][1]);
+            mma_bf16(a, fh, bq[1][kk][2], bq[1][kk][3]);
+            mma_bf16(a, fl, bq[1][kk][0], bq[1][kk][1]);
+            mma_bf16(a, fh, bq[1][kk][0], bq[1][kk][1]);
           }
         }
       }

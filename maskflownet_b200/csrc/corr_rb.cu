@@ -19,29 +19,12 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace mfn {
 namespace rb {
 constexpr int NTHREADS = 256, NWARPS = 8, HX = 4;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
-  const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - bh), "f"(a - ah));
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr)
-               : "memory");
-}
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 // pixel pitch in bytes: 2 bytes x channels padded to 16, made an odd multiple of 16
 __host__ __device__ inline int pixel_pitch(int C) {
   const int cp = (C + 15) / 16 * 16;

@@ -32,6 +32,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace mfn {
 namespace ct {
@@ -62,63 +63,6 @@ enum {
 static_assert(B_COUNT * 8 <= 512, "barrier area");
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_n(uint32_t bar, uint32_t n) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(n) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes)
-               : "memory");
-}
-// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the device.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (!done && ++spins > (1u << 26)) __trap();
-  }
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, int c2, int c3,
-                                            uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::
-          "r"(dst),
-      "l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tm),
-               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
-  const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - bh), "f"(a - ah));
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr)
-               : "memory");
-}
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ int swz(int p, int c) { return p * PXB + ((c ^ ((p >> 1) & 3)) << 4); }
 __device__ __forceinline__ void put_chunk(unsigned char* dst, int lo_off, const float (&e)[8], float sc) {
   uint4 hi, lo;
   split_pair(e[0] * sc, e[1] * sc, hi.x, lo.x);
@@ -411,12 +355,12 @@ __global__ void __launch_bounds__(ct::NTHREADS, 1)
           const uint32_t sa = base + OFF_STG + (grp * STG_SLOTS + slot) * STG_SLOT;
           mbar_wait(sa + STG_BAR_FULL, fill & 1);
           tma_store_4d(&tmo, sa, x0, d * G, UR * g0, n);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+          bulk_commit();
+          bulk_wait_read();
           mbar_arrive(sa + STG_BAR_FREE);
         }
       }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+      bulk_wait_all();
     }
   }
 }

@@ -18,6 +18,7 @@
 #ifdef MFN_HOST_EMULATION
 #include "cuda_shim.h"
 #include "device_caps.h"
+#include "sampling.cuh"
 #else
 #include "common.cuh"
 #endif
@@ -41,17 +42,7 @@ struct Args {
   int num;
 };
 
-#ifdef MFN_HOST_EMULATION
-// Upsample(f) taps (network/MaskFlownet.py:35-62): the product's common.cuh defines these; restated for the host build
-__device__ __forceinline__ void upsample_taps(int o, int f, int n, int& i0, int& i1, float& w1) {
-  i0 = o / f;
-  const int r = o - i0 * f;
-  i1 = min(i0 + 1, n - 1);
-  w1 = (float)r / (float)f;
-}
-#endif
-
-// both channels of Upsample(f)(pred)[n] at (y, x); same interpolation order as upsample_at (common.cuh)
+// both channels of Upsample(f)(pred)[n] at (y, x); same interpolation order as upsample_at (sampling.cuh)
 __device__ __forceinline__ void upsample2_at(const float* __restrict__ p, int Hc, int Wc, int f, int y, int x, float& u0,
                                              float& u1) {
   int y0, y1, x0, x1;
