@@ -282,6 +282,29 @@ MFN_API int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, con
                                    int stride, int dilation, int out_mode, float leaky_slope, void* workspace,
                                    long long workspace_bytes, void* stream);
 
+/* Split activations (csrc/split_act.cuh): an activation of C channels stored as (N, 2, Cg, H, W, 8) bf16, Cg =
+ * ceil(C/16)*2 groups of 8 channels -- per sample the bf16 "hi" image of every group, then the "lo" image of the
+ * remainders (the operand split every tensor-core contraction here uses) -- 4 bytes per channel-pixel like fp32, with the
+ * channels past C zero.  Stored so, a value is converted once, when written, instead of by every convolution that reads
+ * it (the dense block makes each layer read everything written before it), and a convolution loads its input tiles with
+ * plain tensor copies.
+ * mfn_split_pack: channels [0, C) of an fp32 NCHW tensor (src_batch_stride elements between samples, 0 = C*H*W) into
+ *   channels [dst_c0, dst_c0 + C) of a split buffer of dst_channels channels; the slice starts at a multiple of 16 and
+ *   ends at one or at the buffer's last channel (whose pad up to the next multiple of 16 is then written as zeros).
+ * mfn_conv3x3_forward_split = mfn_conv3x3_forward_ws, stride 1, reading channels [x_c0, x_c0 + Cin) of the split buffer x
+ *   of x_channels channels (a slice that starts at a multiple of 16 and ends at one or at the last channel).  out_split == NULL: fp32 output to `out` as in mfn_conv3x3_forward_ws
+ *   (NCHW or depth-to-space).  Otherwise the output channels past the linear prefix k (out_mode = MFN_CONV_OUT_NCHW |
+ *   MFN_CONV_OUT_LINEAR_PREFIX(k), k even, Cout - k a multiple of 16) go to channels out_split_c0.. (a multiple of 16) of
+ *   the split buffer out_split of out_split_channels channels, and the k prefix channels to the fp32 (N, k, H, W) `out`.
+ *   Dilations >= 2 must be even.  The products and their order are those of mfn_conv3x3_forward_ws on the same fp32 values:
+ *   results are bit-identical. */
+MFN_API int mfn_split_pack(const float* src, long long src_batch_stride, int N, int C, int H, int W, void* dst,
+                           int dst_channels, int dst_c0, void* stream);
+MFN_API int mfn_conv3x3_forward_split(const void* x, int x_channels, int x_c0, const void* packed_weight, const float* bias,
+                                      float* out, long long out_batch_stride, void* out_split, int out_split_channels,
+                                      int out_split_c0, int N, int Cin, int H, int W, int Cout, int dilation, int out_mode,
+                                      float leaky_slope, void* workspace, long long workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * The step either side of the network (SURVEY.md section 8f, row N3).
  * mfn_preprocess_forward replaces PipelineFlownet.predict / do_batch_mx -- network/pipeline.py:206-212 (`/ 255.0`),

@@ -33,7 +33,7 @@ struct Tuning {
   int corr_ts_lo = 0, corr_ts_hi = 0;   // development: device pointer (two halves) of the timeline buffer of corr_tma_kernel, 0 = off
   int corr_dbg = 0;           // profiling aid for the ring kernel: 2 = producers idle, 4 = no epilogue, 8 = no MMA (results invalid)
   int conv_dbg = 0;           // profiling aid for the wgmma convolution: 2 = producers skip global loads, 4 = no epilogue
-                              // stores, 8 = no MMAs (results invalid; tools/conv_bound.py)
+                              // stores, 8 = no MMAs, 16 = no input path at all (results invalid; tools/conv_bound.py)
 };
 Tuning& tuning();
 

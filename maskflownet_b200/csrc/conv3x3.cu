@@ -377,3 +377,48 @@ extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, 
   if (nt <= 12) return launch_conv<2, 6>(x, xbs, wp, bias, out, obs, N, Cin, H, W, Cout, dilation, leaky_slope, lin_prefix, st);
   return launch_conv<2, 8>(x, xbs, wp, bias, out, obs, N, Cin, H, W, Cout, dilation, leaky_slope, lin_prefix, st);
 }
+
+extern "C" int mfn_conv3x3_forward_split(const void* x, int x_channels, int x_c0, const void* packed_weight,
+                                         const float* bias, float* out, long long out_batch_stride, void* out_split,
+                                         int out_split_channels, int out_split_c0, int N, int Cin, int H, int W, int Cout,
+                                         int dilation, int out_mode, float leaky_slope, void* workspace,
+                                         long long workspace_bytes, void* stream) {
+  using namespace mfn;
+  MFN_REQUIRE(workspace_bytes >= 0 && (workspace || workspace_bytes == 0) && aligned(workspace, 16), MFN_ERR_INVALID_ARG,
+              "mfn_conv3x3_forward_split: workspace must be 16-byte aligned (or null with 0 bytes)");
+  const int lin_prefix = out_mode >> 8, mode = out_mode & 0xff;
+  MFN_REQUIRE(x && packed_weight && (out || (out_split && lin_prefix == 0)), MFN_ERR_INVALID_ARG,
+              "mfn_conv3x3_forward_split: null pointer");
+  MFN_REQUIRE(N > 0 && Cin > 0 && H > 0 && W > 0 && Cout > 0 && Cout <= 256 && dilation >= 1, MFN_ERR_INVALID_ARG,
+              "mfn_conv3x3_forward_split: bad extent, Cout (<= 256) or dilation");
+  // the last chunk loads whole 16-channel groups: past the slice they must be the buffer's zero pad, not its next channels
+  MFN_REQUIRE(x_c0 >= 0 && x_c0 % 16 == 0 && x_c0 + Cin <= x_channels &&
+                  ((x_c0 + Cin) % 16 == 0 || x_c0 + Cin == x_channels),
+              MFN_ERR_INVALID_ARG,
+              "mfn_conv3x3_forward_split: input slice [%d, %d) of the %d channels must start at a multiple of 16 and end "
+              "at one or at the last channel", x_c0, x_c0 + Cin, x_channels);
+  MFN_REQUIRE(aligned(packed_weight, 16) && aligned(x, 16), MFN_ERR_ALIGNMENT,
+              "mfn_conv3x3_forward_split: packed weights and split input must be 16-byte aligned");
+  MFN_REQUIRE(lin_prefix >= 0 && lin_prefix <= Cout && (lin_prefix == 0 || mode == MFN_CONV_OUT_NCHW), MFN_ERR_INVALID_ARG,
+              "mfn_conv3x3_forward_split: linear prefix needs NCHW / split output and <= Cout");
+  MFN_REQUIRE(mode == MFN_CONV_OUT_NCHW || (mode == MFN_CONV_OUT_DEPTH_TO_SPACE2 && Cout % 4 == 0 && !out_split),
+              MFN_ERR_INVALID_ARG, "mfn_conv3x3_forward_split: depth-to-space output needs Cout %% 4 == 0 and fp32 output");
+  const int Fo = out_split ? lin_prefix : (mode ? Cout / 4 : Cout), OS = mode ? 4 : 1;
+  const long long obs = out_batch_stride ? out_batch_stride : (long long)Fo * H * W * OS;
+  MFN_REQUIRE(obs >= (long long)Fo * H * W * OS, MFN_ERR_INVALID_ARG, "mfn_conv3x3_forward_split: batch stride too small");
+  SplitIO sio;
+  sio.in = x;
+  sio.in_C = x_channels;
+  sio.in_c0 = x_c0;
+  sio.out = out_split;
+  sio.out_C = out_split_channels;
+  sio.out_c0 = out_split_c0;
+  const unsigned char* wp = static_cast<const unsigned char*>(packed_weight);
+  const int rc = conv3x3_wgmma_launch(nullptr, 0, wp + conv3x3_sync_packed_bytes(Cin, Cout), bias, out, obs, N, Cin, H, W,
+                                      Cout, 1, dilation, out_mode, leaky_slope, as_stream(stream), 0,
+                                      static_cast<float*>(workspace), workspace_bytes, sio);
+  MFN_REQUIRE(rc != -1, MFN_ERR_UNSUPPORTED,
+              "mfn_conv3x3_forward_split: unsupported (odd dilation >= 2, split output slice not 16-channel aligned "
+              "after an even linear prefix, or too large)");
+  return rc;
+}

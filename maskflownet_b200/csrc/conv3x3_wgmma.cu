@@ -19,7 +19,10 @@
 //     rows and asynchronous bulk copies when the output rows are 16-byte aligned, else from registers -- or, for the
 //     transposed convolutions, scatter 2x2 sub-pixel phases (depth-to-space).
 //   * layers wider than 128 output channels are cut into two 128-channel work items per tile (register budget).
+#include <cstring>
+
 #include "mma_tiles.cuh"
+#include "split_act.cuh"
 
 namespace mfn {
 namespace um {
@@ -190,6 +193,14 @@ __device__ __forceinline__ void decode_tile(int tile, int tilesX, int tilesY, co
     n = tile / (tilesX * tilesY);
   }
 }
+// split-activation operands on the device (SplitIO): in = the input tiles come from the tensor map (groups in_g0.. of a
+// buffer of in_Cg groups per plane); out != null = output channels >= the linear prefix go to channel out_c0.. of a split
+// buffer of out_Cg groups
+struct SplitDev {
+  int in, in_g0, in_Cg;
+  unsigned char* out;
+  int out_Cg, out_c0;
+};
 struct Work {
   int tile, part, cb, ce, nh;   // part < 0: a whole tile; nh: output-channel half
 };
@@ -282,7 +293,8 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
     conv3x3_wgmma_kernel(const float* __restrict__ x, long long x_bs, const unsigned char* __restrict__ wpack,
                          const float* __restrict__ bias_arg, float* __restrict__ out_base, long long out_bs, int Cin, int H, int W,
                          int OH, int OW, int Cout, int CoutP, int nChunks, float slope_arg, int tilesX, int tilesY, int numWork,
-                         int stride, int dil, int out_mode_arg, int ext, um::SplitK sk, int dbg) {
+                         int stride, int dil, int out_mode_arg, int ext, um::SplitK sk, um::SplitDev xs,
+                         const __grid_constant__ CUtensorMap tmx, int dbg) {
   using namespace um;
   // out_mode_arg = mode | (linear_prefix << 8): the first linear_prefix output channels are written WITHOUT the activation
   // (a second, linear head sharing the input pass of an activated layer: network.py folds pred_flow / pred_mask over the
@@ -291,7 +303,8 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   // cut into sk.k parts over the channel chunks -- part p walks chunks [p nChunks / k, (p + 1) nChunks / k) and writes its
   // RAW partial sums (no bias, no activation) to the workspace; conv3x3_wgmma_reduce_kernel finishes that region.
   // dbg (tuning "conv_dbg", profiling only, results invalid): 2 = producers skip their global loads, 4 = no epilogue
-  // stores, 8 = no MMAs; the barrier protocol is unchanged, so each phase can be timed by removing it.
+  // stores, 8 = no MMAs, 16 = producers skip loads, conversion and shared-memory stores (they only hand over each stage);
+  // the barrier protocol is unchanged, so each phase can be timed by removing it.
   constexpr int NCOL = FOLD ? NW / 2 : NW;   // output channels per work item
   const int out_mode_k = out_mode_arg & 0xff, lin_prefix_k = out_mode_arg >> 8;
   extern __shared__ __align__(128) unsigned char smem[];
@@ -308,7 +321,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
 
   if (tid == 0) {
     for (int i = 0; i < AS; ++i) {
-      mbar_init(a_full + 8 * i, NPROD);
+      mbar_init(a_full + 8 * i, xs.in ? 1 : NPROD);
       mbar_init(a_empty + 8 * i, NCONS);
     }
     for (int i = 0; i < WS; ++i) {
@@ -429,6 +442,49 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         const int t = wq * 32 + lane;   // thread of this warpgroup
         const int x0 = tx * MT;
         const uint32_t seg = (uint32_t)((OW - x0 < MT ? OW - x0 : MT) * 4);
+        if (xs.out != nullptr) {
+          // split output (no linear prefix): the piece's SCH / 8 groups x {hi, lo} are staged as rows of MT 16-byte
+          // entries -- exactly their layout in global memory, one contiguous row segment each -- and leave by one bulk copy
+          // per row.  A warp's pair stores cover 8 pixels x 4 words: 32 distinct banks.
+          unsigned char* const sst = reinterpret_cast<unsigned char*>(stg);
+#pragma unroll
+          for (int pc = 0; pc < NCOL / SCH; ++pc) {
+            if (t < SCH / 4) bulk_wait_read();
+            named_bar_sync(1 + r, 128);
+#pragma unroll
+            for (int jj = 0; jj < SCH / 8; ++jj) {
+              const int j = pc * (SCH / 8) + jj;
+              const int f = wk.nh * NCOL + 8 * j + 2 * (lane & 3);
+              const float b0 = (bias != nullptr && f < Cout) ? __ldg(bias + f) : 0.f;
+              const float b1 = (bias != nullptr && f + 1 < Cout) ? __ldg(bias + f + 1) : 0.f;
+              unsigned char* const row = sst + (2 * jj * MT + 16 * wq + (lane >> 2)) * 16 + (lane & 3) * 4;
+#pragma unroll
+              for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int i = 4 * j + 2 * h;
+                  float v0 = acc[mh][i], v1 = acc[mh][i + 1];
+                  if constexpr (FOLD) {
+                    v0 += acc[mh][i + NW / 4];
+                    v1 += acc[mh][i + 1 + NW / 4];
+                  }
+                  uint32_t hi, lo;
+                  split_pair(leaky(v0 + b0, slope), leaky(v1 + b1, slope), hi, lo);
+                  unsigned char* const e = row + (64 * mh + 8 * h) * 16;
+                  *reinterpret_cast<uint32_t*>(e) = hi;
+                  *reinterpret_cast<uint32_t*>(e + MT * 16) = lo;
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            named_bar_sync(1 + r, 128);
+            const int f = wk.nh * NCOL + pc * SCH + 8 * (t >> 1);   // first channel of row t = (group t / 2, plane t % 2)
+            if (t < SCH / 4 && f < Cout) {
+              const long long dst = sa::entry(n, t & 1, (xs.out_c0 + f) >> 3, (long long)y * OW + x0, xs.out_Cg, oplane0);
+              bulk_s2g(xs.out + dst, smem_u32(sst + t * MT * 16), seg * 4);
+              bulk_commit();
+            }
+          }
+        } else
 #pragma unroll
         for (int pc = 0; pc < NCOL / SCH; ++pc) {
           if (t < SCH) bulk_wait_read();                  // this thread's previous copies have read the staging rows
@@ -477,7 +533,16 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
                 if constexpr (FOLD) v += acc[mh][i + NW / 4];   // second column block: the hi * lo term
                 const int f = wk.nh * NCOL + 8 * j + 2 * (lane & 3) + e;
                 if (f >= Cout) continue;
-                if (out_mode == 0) {
+                if (xs.out != nullptr && !partial && f >= lin_prefix) {
+                  // split output: the pair (f, f + 1) as one hi and one lo word (f - lin_prefix is even, host-checked)
+                  if (e == 0) {
+                    const float b0 = bias != nullptr ? __ldg(bias + f) : 0.f, b1 = bias != nullptr ? __ldg(bias + f + 1) : 0.f;
+                    float v1 = acc[mh][i + 1];
+                    if constexpr (FOLD) v1 += acc[mh][i + 1 + NW / 4];
+                    sa::put_pair(xs.out, xs.out_Cg, oplane0, n, xs.out_c0 + f - lin_prefix, (size_t)y * OW + xx,
+                                 leaky(v + b0, slope), leaky(v1 + b1, slope));
+                  }
+                } else if (out_mode == 0) {
                   const float t = v + (bias != nullptr ? __ldg(bias + f) : 0.f);
                   out[(size_t)f * oplane0 + (size_t)y * OW + xx] = leaky(t, f < lin_prefix ? 1.f : slope);
                 } else {
@@ -512,10 +577,64 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
     }
   } else {
     // ============================ input producers (warps 9..11) ============================
+    if (xs.in) {
+      // split input (split_act.cuh): the buffer already holds the converted entries in the stage layout, so a chunk is a
+      // pure tensor copy -- hi and lo each one box {8 channels, PW pixels, nslots rows, 2 groups} (d < R), or one box of
+      // R rows per kernel row, group and plane (d >= R) -- issued by one thread.  Out-of-bounds rows / pixels read zero:
+      // the padding.
+      if (warp == 9 && lane == 0) {
+        uint32_t as = 0, aph = 0;
+        bool wrapped = false;
+        for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
+          const Work wk = decode_work(work, sk, nChunks);
+          int tx, ty, n;
+          decode_tile(wk.tile, tilesX, tilesY, sk, tx, ty, n);
+          const int x0 = tx * MT - dil, y0 = ty * R;
+          const int gb = n * 2 * xs.in_Cg + xs.in_g0;
+          for (int c = wk.cb; c < wk.ce; ++c) {
+            if (wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);
+            const uint32_t bar = a_full + 8 * as, dst = s_base + as * (uint32_t)sm.a_stage;
+            if (dbg & 16) {
+              mbar_arrive(bar);
+            } else {
+              mbar_arrive_expect_tx(bar, (uint32_t)sm.a_stage);
+              const int g = gb + 2 * c;
+              if (dil < R) {
+                tma_load_4d(dst, &tmx, 0, x0, y0 - dil, g, bar);
+                tma_load_4d(dst + (uint32_t)sm.a_lo, &tmx, 0, x0, y0 - dil, g + xs.in_Cg, bar);
+              } else {
+#pragma unroll 1
+                for (int k = 0; k < 12; ++k) {   // (kernel row ky, group kc, plane)
+                  const int ky = k >> 2, kc = (k >> 1) & 1, pl = k & 1;
+                  tma_load_4d(dst + (uint32_t)(pl * sm.a_lo + (kc * E + ky * R * PW) * 16), &tmx, 0, x0, y0 + (ky - 1) * dil,
+                              g + kc + pl * xs.in_Cg, bar);
+                }
+              }
+            }
+            if (++as == (uint32_t)AS) { as = 0; aph ^= 1; wrapped = true; }
+          }
+        }
+      }
+      return;
+    }
     // One instruction stream for every layer shape: the (work item, chunk, batch) space of this CTA is walked as ONE flat
     // sequence of batches (BATCH items of 32 entries x 8 channels per warp), software-pipelined over two register sets --
     // the loads of batch i+1 (possibly the next chunk, possibly the next TILE) are in flight while batch i is converted and
     // stored.  Geometry is arithmetic only (e / PW through a multiply-high).
+    if (dbg & 16) {   // profiling: no input path at all -- the same a_empty / a_full traffic per chunk, nothing loaded or stored
+      uint32_t as = 0, aph = 0;
+      bool wrapped = false;
+      for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
+        const Work wk = decode_work(work, sk, nChunks);
+        for (int c = wk.cb; c < wk.ce; ++c) {
+          if (wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(a_full + 8 * as);
+          if (++as == (uint32_t)AS) { as = 0; aph ^= 1; wrapped = true; }
+        }
+      }
+      return;
+    }
     const int pw = warp - 9;
     const int G = (E + 31) / 32;
     const bool one_plane = Cin <= 8;          // a single chunk whose channels 8..15 are zeros: plane 1 is cleared once, never loaded
@@ -660,8 +779,9 @@ int conv3x3_wgmma_pack(const float* weight, unsigned char* packed, int Cin, int 
 
 // Split-K second pass over the split region (samples n_lo.., rows y_lo..): out = act(sum_p parts[p] + bias), NCHW (with
 // the linear prefix) or depth-to-space.
-__global__ void conv3x3_wgmma_reduce_kernel(um::SplitK sk, int RN, const float* __restrict__ bias, float* __restrict__ out,
-                                            long long out_bs, int Cout, int OH, int OW, float slope, int out_mode_arg) {
+__global__ void conv3x3_wgmma_reduce_kernel(um::SplitK sk, um::SplitDev xs, int RN, const float* __restrict__ bias,
+                                            float* __restrict__ out, long long out_bs, int Cout, int OH, int OW, float slope,
+                                            int out_mode_arg) {
   const int out_mode = out_mode_arg & 0xff, lin_prefix = out_mode_arg >> 8;
   const long long total = (long long)RN * Cout * sk.rh * OW;
   const int F = Cout >> 2;
@@ -672,7 +792,11 @@ __global__ void conv3x3_wgmma_reduce_kernel(um::SplitK sk, int RN, const float* 
     const int n = sk.n_lo + (int)(i / ((long long)OW * sk.rh * Cout));
     if (out_mode == 0) {
       const float b = bias ? __ldg(bias + f) : 0.f;
-      out[(size_t)n * out_bs + ((size_t)f * OH + y) * OW + x] = leaky(s + b, f < lin_prefix ? 1.f : slope);
+      const float v = leaky(s + b, f < lin_prefix ? 1.f : slope);
+      if (xs.out != nullptr && f >= lin_prefix)
+        sa::put_one(xs.out, xs.out_Cg, (long long)OH * OW, n, xs.out_c0 + f - lin_prefix, (long long)y * OW + x, v);
+      else
+        out[(size_t)n * out_bs + ((size_t)f * OH + y) * OW + x] = v;
     } else {
       const int ph = f / F, ff = f - ph * F;
       const float b = bias ? __ldg(bias + ff) : 0.f;
@@ -732,11 +856,43 @@ long long conv3x3_wgmma_workspace_bytes(int N, int Cin, int H, int W, int Cout, 
   return sk.k > 1 ? sk.k * sk.part_stride * 4 : 0;
 }
 
-// returns -1 when the shape does not fit this kernel (caller falls back to the mma.sync kernel)
+// returns -1 when the shape does not fit this kernel (caller falls back to the mma.sync kernel; split operands have no
+// fall-back)
 int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wpack, const float* bias, float* out,
                          long long out_bs, int N, int Cin, int H, int W, int Cout, int stride, int dil, int out_mode,
-                         float slope, cudaStream_t st, int ext, float* ws, long long ws_bytes) {
+                         float slope, cudaStream_t st, int ext, float* ws, long long ws_bytes, const SplitIO& sio) {
   using namespace um;
+  SplitDev xs = {0, 0, 0, nullptr, 0, 0};
+  CUtensorMap tmx;
+  memset(&tmx, 0, sizeof tmx);
+  if (sio.in != nullptr) {
+    // the tensor copies need 128-byte aligned shared-memory destinations: every box offset is, unless an odd d >= R
+    if (stride != 1 || ext != 0 || sio.in_c0 % 16 != 0 || (dil >= R && dil % 2 != 0) || !aligned(sio.in, 16)) return -1;
+    EncodeTiledFn fn = encode_tiled_fn();
+    if (fn == nullptr) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
+    const int Cg = sa::groups(sio.in_C);
+    const cuuint64_t dim[4] = {8, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N * 2 * Cg};
+    const cuuint64_t strides[3] = {16, (cuuint64_t)W * 16, (cuuint64_t)W * H * 16};
+    const cuuint32_t box[4] = {8, (cuuint32_t)row_pitch(1, dil), (cuuint32_t)(dil < R ? n_slots(1, dil) : R), dil < R ? 2u : 1u};
+    const cuuint32_t es[4] = {1, 1, 1, 1};
+    const CUresult r = fn(&tmx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(sio.in), dim, strides, box, es,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
+    xs.in = 1;
+    xs.in_g0 = sio.in_c0 / 8;
+    xs.in_Cg = Cg;
+  }
+  if (sio.out != nullptr) {
+    // whole 16-channel chunks after the prefix: pairs stay pairs, and the buffer's pad channels are never written
+    const int lp = out_mode >> 8;
+    if ((out_mode & 0xff) != 0 || ext != 0 || sio.out_c0 % 16 != 0 || (Cout - lp) % 16 != 0 || lp % 2 != 0 ||
+        sio.out_c0 + Cout - lp > sio.out_C || !aligned(sio.out, 16))
+      return -1;
+    xs.out = static_cast<unsigned char*>(sio.out);
+    xs.out_Cg = sa::groups(sio.out_C);
+    xs.out_c0 = sio.out_c0;
+  }
   if (Cout > 256 || (stride != 1 && !(stride == 2 && dil == 1))) return -1;
   if (ext != 0 && !((ext == 1 || ext == 2) && stride == 1 && dil == 1 && out_mode == 0)) return -1;
   if ((out_mode >> 8) != 0 && (out_mode & 0xff) != 0) return -1;   // linear prefix only with plain NCHW output
@@ -746,7 +902,9 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const int grow = ext == 2 ? 8 : 2 * ext;   // ext 1: grid + 1 pixel per side; ext 2: + the six band rows / columns too
   const int OH = stride == 2 ? (H - 1) / 2 + 1 : H + grow, OW = stride == 2 ? (W - 1) / 2 + 1 : W + grow;
   // staged epilogue (bulk copies of whole output row segments): plain NCHW output whose rows start 16-byte aligned
-  const bool staged = (out_mode & 0xff) == 0 && ext == 0 && OW % 4 == 0 && out_bs % 4 == 0 && aligned(out, 16) &&
+  // (split output: every row segment is 16-byte aligned; the register epilogue takes the linear prefix)
+  const bool staged = (out_mode & 0xff) == 0 && ext == 0 &&
+                      (xs.out != nullptr ? (out_mode >> 8) == 0 : OW % 4 == 0 && out_bs % 4 == 0 && aligned(out, 16)) &&
                       smem_map(E, CoutP, as_wide, STG_BYTES).WS >= 2;
   const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0);
   if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
@@ -792,8 +950,8 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
 #define MFN_WGMMA_LAUNCH(NW_, FOLD_, TPS_)                                                                                   \
   conv3x3_wgmma_kernel<NW_, FOLD_, TPS_><<<grid, NTHREADS, sm.total, st>>>(x, x_bs, wpack, bias, out, out_bs, Cin, H, W, OH, \
                                                                            OW, Cout, CoutP, nChunks, slope, tilesX, tilesY,  \
-                                                                           (int)numWork, stride, dil, out_mode, ext, sk,     \
-                                                                           tuning().conv_dbg)
+                                                                           (int)numWork, stride, dil, out_mode, ext, sk, xs, \
+                                                                           tmx, tuning().conv_dbg)
   // variant name (last_kernel): the padded output width, and whether the hi / lo weight images are folded
   const char* name = "conv3x3_wgmma_kernel<CoutP=256>";
   switch (CoutP) {
@@ -813,7 +971,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const long long total = sk.part_stride;
   long long blocks = (total + 255) / 256;
   if (blocks > 4 * kNumSMs) blocks = 4 * kNumSMs;
-  conv3x3_wgmma_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(sk, N - sk.n_lo, bias, out, out_bs, Cout, OH, OW, slope, out_mode);
+  conv3x3_wgmma_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(sk, xs, N - sk.n_lo, bias, out, out_bs, Cout, OH, OW, slope, out_mode);
   return check_launch("conv3x3_wgmma_reduce_kernel");
 }
 

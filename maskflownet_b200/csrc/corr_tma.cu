@@ -32,6 +32,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "mma_tiles.cuh"
 #include "ptx.cuh"
 
 namespace mfn {
@@ -368,10 +369,7 @@ __global__ void __launch_bounds__(ct::NTHREADS, 1)
 // =====================================================================================================
 // Host side: tensor maps (cuTensorMapEncodeTiled through the runtime's driver entry point: no link against libcuda)
 // =====================================================================================================
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
+EncodeTiledFn encode_tiled_fn() {
   static EncodeTiledFn fn = [] {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;

@@ -23,9 +23,24 @@ __host__ __device__ constexpr int cout_pad(int cout) { return cout <= 32 ? 32 : 
 long long conv3x3_sync_packed_bytes(int Cin, int Cout);
 long long conv3x3_wgmma_packed_bytes(int Cin, int Cout);
 int conv3x3_wgmma_pack(const float* weight, unsigned char* packed, int Cin, int Cout, cudaStream_t st);
+// Split-activation operands (split_act.cuh) of one launch.  in != null: the input is channels [in_c0, in_c0 + Cin) of a
+// split buffer of in_C channels (x is unused).  out != null: the output channels past the linear prefix go to channels
+// out_c0.. of a split buffer of out_C channels; the prefix channels go to the fp32 `out` of the launch.
+struct SplitIO {
+  const void* in = nullptr;
+  int in_C = 0, in_c0 = 0;
+  void* out = nullptr;
+  int out_C = 0, out_c0 = 0;
+};
 int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wpack, const float* bias, float* out,
                         long long out_bs, int N, int Cin, int H, int W, int Cout, int stride, int dil, int out_mode,
-                        float slope, cudaStream_t st, int ext = 0, float* ws = nullptr, long long ws_bytes = 0);
+                        float slope, cudaStream_t st, int ext = 0, float* ws = nullptr, long long ws_bytes = 0,
+                        const SplitIO& sio = SplitIO());
+// cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda); null when unavailable
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn encode_tiled_fn();
 // split-K over the input-channel chunks for layers with fewer tiles than SMs: the plan (1 = none) and the fp32 workspace
 // the caller has to lend to conv3x3_wgmma_launch for it
 long long conv3x3_wgmma_workspace_bytes(int N, int Cin, int H, int W, int Cout, int stride, int dil);

@@ -1,22 +1,16 @@
 // ptx.cuh -- the sm_90a inline-PTX primitives the tensor-core kernels are built from (corr_fwd.cu, corr_tma.cu, corr_rb.cu,
-// conv3x3.cu, conv3x3_wgmma.cu, warp_mma.cu): the bf16 hi/lo split, ldmatrix / mma.sync, the XOR swizzle of 64-byte rows,
-// cp.async, mbarriers, bulk and tensor (TMA) copies and named barriers.  One definition of each, so that a change to one
-// (the split, a wait bound, a barrier form) reaches every kernel.
+// conv3x3.cu, conv3x3_wgmma.cu, warp_mma.cu): the bf16 hi/lo split (in bf16_split.cuh), ldmatrix / mma.sync, the XOR
+// swizzle of 64-byte rows, cp.async, mbarriers, bulk and tensor (TMA) copies and named barriers.  One definition of each, so
+// that a change to one (the split, a wait bound, a barrier form) reaches every kernel.
 #pragma once
 #include <cuda.h>
 #include <cstdint>
 
+#include "bf16_split.cuh"
+
 namespace mfn {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// (a, b) fp32 -> packed bf16x2 "hi" (a in the low half: the lower k index of an MMA fragment register) and the bf16x2 of
-// the remainders "lo".  Every contraction sums hi*hi + hi*lo + lo*hi in fp32 (DESIGN section 4).
-__device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));
-  const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xffff0000u);
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(b - bh), "f"(a - ah));
-}
 
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"

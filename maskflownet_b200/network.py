@@ -69,19 +69,16 @@ class DeformParams(nn.Module):
 
 
 class _Slab:
-    """Inference view of a dense block's output inside its concat buffer: x = buf[:, c0:], and -- when the block's last
-    convolution also produced them -- the linear heads' partial sums over everything but that convolution's own output
-    in buf[:, :c0] (see _FlowNetBase._dense_inplace)."""
+    """Inference form of a dense block's output: its concat buffer as a split activation (ops.SplitAct), and -- when the
+    block's last convolution also produced them -- the linear heads' partial sums over everything but that convolution's
+    own last_oc output channels, in the fp32 tensor `prefix` (see _FlowNetBase._dense_split)."""
 
-    def __init__(self, buf: torch.Tensor, c0: int, last_oc: int):
-        self.buf, self.c0, self.last_oc = buf, c0, last_oc
+    def __init__(self, act: "ops.SplitAct", prefix: Optional[torch.Tensor], last_oc: int):
+        self.act, self.prefix, self.last_oc = act, prefix, last_oc
 
     @property
     def channels(self) -> int:
-        return self.buf.shape[1] - self.c0
-
-    def tensor(self) -> torch.Tensor:
-        return self.buf[:, self.c0:]
+        return self.act.channels
 
 
 class _FlowNetBase(nn.Module):
@@ -120,18 +117,16 @@ class _FlowNetBase(nn.Module):
     def _heads(self, lvl, x, with_mask):
         """pred_flow{lvl} (2 channels) and pred_mask{lvl} (1 channel) read the same block output
         (network/MaskFlownet.py:224, 226 ...): inference runs them as ONE 3-output convolution, no activation -- and, when
-        the dense block left their partial sums (a _Slab with c0 > 0), only over the block's last 32 channels."""
+        the dense block left their partial sums (a _Slab with a prefix tensor), only over the block's last 32 channels."""
         convs = self._head_convs(lvl, with_mask)
         pm = convs[1] if len(convs) > 1 else None
         if not isinstance(x, _Slab):
-            if not self._fast(x):
-                return (self._conv_act(f"pred_flow{lvl}", x, 1.0),
-                        self._conv_act(f"pred_mask{lvl}", x, 1.0) if pm is not None else None)
-            x = _Slab(x, 0, 0)
+            return (self._conv_act(f"pred_flow{lvl}", x, 1.0),
+                    self._conv_act(f"pred_mask{lvl}", x, 1.0) if pm is not None else None)
         nh = 2 + (1 if pm is not None else 0)
-        buf, c0 = x.buf, x.c0
-        N, _, H, W = buf.shape
-        if c0 == nh and x.last_oc:   # partial sums present: finish with the tiny convolution over conv{L}_4's output
+        N, _, H, W = x.act.shape
+        dev = x.act.buf.device
+        if x.prefix is not None and x.prefix.shape[1] >= nh:   # partial sums present: finish over conv{L}_4's output
             oc = x.last_oc
 
             def build_tail():
@@ -139,17 +134,17 @@ class _FlowNetBase(nn.Module):
                 b = torch.cat([c.bias.detach() for c in convs], dim=0).contiguous()
                 return ops.conv3x3_pack(w), b
             packed, b = self._packed_fn(f"heads_tail{lvl}", [p for c in convs for p in (c.weight, c.bias)], build_tail)
-            y = torch.empty((N, nh, H, W), device=buf.device, dtype=torch.float32)
-            ops.conv3x3_slices(buf, c0, oc, packed, b, y, 0, nh, 1.0)
-            y += buf[:, :nh]
+            y = torch.empty((N, nh, H, W), device=dev, dtype=torch.float32)
+            ops.conv3x3_split(x.act, 0, oc, packed, b, nh, 1.0, out=y)
+            y += x.prefix[:, :nh]
         else:
             def build():
                 w = torch.cat([c.weight.detach() for c in convs], dim=0).contiguous()
                 b = torch.cat([c.bias.detach() for c in convs], dim=0).contiguous()
                 return ops.conv3x3_pack(w), b
             packed, b = self._packed_fn(f"heads{lvl}", [p for c in convs for p in (c.weight, c.bias)], build)
-            y = torch.empty((N, nh, H, W), device=buf.device, dtype=torch.float32)
-            ops.conv3x3_slices(buf, c0, x.channels, packed, b, y, 0, nh, 1.0)
+            y = torch.empty((N, nh, H, W), device=dev, dtype=torch.float32)
+            ops.conv3x3_split(x.act, 0, x.channels, packed, b, nh, 1.0, out=y)
         if pm is None:
             return y, None
         return y[:, :2].contiguous(), y[:, 2:3].contiguous()
@@ -159,14 +154,12 @@ class _FlowNetBase(nn.Module):
         tensor-core kernel (ops.conv_transpose4x4_pack)."""
         up = getattr(self, f"upfeat{lvl}")
         if not isinstance(x, _Slab):
-            if not self._fast(x):
-                return tF.leaky_relu(up(x), SLOPE)
-            x = _Slab(x, 0, 0)
+            return tF.leaky_relu(up(x), SLOPE)
         packed = self._packed_fn(f"upfeat{lvl}", [up.weight], lambda: ops.conv_transpose4x4_pack(up.weight))
-        N, _, H, W = x.buf.shape
+        N, _, H, W = x.act.shape
         F = up.out_channels
-        out = torch.empty((N, F, 2 * H, 2 * W), device=x.buf.device, dtype=torch.float32)
-        ops.conv3x3_slices(x.buf, x.c0, x.channels, packed, up.bias, out, 0, 4 * F, SLOPE, depth_to_space=True)
+        out = torch.empty((N, F, 2 * H, 2 * W), device=x.act.buf.device, dtype=torch.float32)
+        ops.conv3x3_split(x.act, 0, x.channels, packed, up.bias, 4 * F, SLOPE, out=out, depth_to_space=True)
         return out
 
     def _plain(self, name, x):
@@ -214,62 +207,70 @@ class _FlowNetBase(nn.Module):
         return self._pyramid(im1, names), self._pyramid(im2, names)
 
     def _dense(self, lvl, x):
-        """x = concat(leaky(conv_i(x)), x) five times (network/MaskFlownet.py:219-223 ...).  Inference: one pre-allocated
-        buffer, every convolution reads its input channels in place and writes its output in front of them."""
+        """x = concat(leaky(conv_i(x)), x) five times (network/MaskFlownet.py:219-223 ...).  Inference: see _dense_split."""
         if self._fast(x):
-            N, Cb, H, W = x.shape
-            tot = sum(DECODER_CH) + self._heads_front(lvl)
-            buf = torch.empty((N, tot + Cb, H, W), device=x.device, dtype=torch.float32)
-            buf[:, tot:].copy_(x)
-            return self._dense_inplace(lvl, buf, tot)
+            return self._dense_split(lvl, x)
         for i in range(5):
             x = torch.cat([self._conv_act(f"conv{lvl}_{i}", x, SLOPE), x], dim=1)
         return x
 
-    def _heads_front(self, lvl) -> int:
-        """Extra leading channels of the block's concat buffer that receive the heads' partial sums (0 = not fused)."""
-        if not self.fuse_heads:
-            return 0
-        return 2 + (1 if hasattr(self, f"pred_mask{lvl}") else 0)
-
-    def _dense_inplace(self, lvl, buf, off):
-        """buf[:, off:] holds the block's input; fills buf front to back and returns the block output as a _Slab.
-        With fuse_heads the last convolution also carries the nh linear head channels over ITS input (everything the heads
-        read except that convolution's own 32 output channels): weights [W_heads[:, 32:] ; W_4], written as channels
-        [partial (nh, no activation) | conv{lvl}_4 (32, LeakyReLU)] -- one pass over the ~550-channel input instead of two."""
-        Ctot = buf.shape[1]
-        nh = self._heads_front(lvl)
+    def _dense_split(self, lvl, base):
+        """Inference dense block.  One concat buffer in the split format (ops.SplitAct) holds [conv{lvl}_4 | ... |
+        conv{lvl}_0 | base]: the fp32 base (correlation, features, flow) is packed into it once, and every convolution reads
+        its input channels in place (a pure tensor copy per chunk) and writes its output, already split, in front of them.
+        Every slice starts at a multiple of 16 channels.  With fuse_heads the last convolution also carries the linear
+        heads over ITS input (everything the heads read except that convolution's own 32 output channels): weights
+        [W_heads[:, 32:] ; 0 (to an even count) ; W_4]; the heads' partial sums go to a separate fp32 tensor (split storage
+        would round them) -- one pass over the ~550-channel input instead of two.  Returns the block output as a _Slab."""
+        N, Cb, H, W = base.shape
+        front = sum(DECODER_CH)
+        act = ops.SplitAct(N, front + Cb, H, W, base.device)
+        act.pack(base, front)
+        nh = (2 + (1 if hasattr(self, f"pred_mask{lvl}") else 0)) if self.fuse_heads else 0
+        lp = nh + nh % 2   # the kernel writes split channels in pairs: an even prefix
+        prefix = None
+        off = front
         for i, oc in enumerate(DECODER_CH):
+            assert off % 16 == 0 and (off - oc) % 16 == 0
             conv = getattr(self, f"conv{lvl}_{i}")
             if i == len(DECODER_CH) - 1 and nh:
                 heads = self._head_convs(lvl, True)
 
                 def build():
-                    w = torch.cat([h.weight.detach()[:, oc:] for h in heads] + [conv.weight.detach()], dim=0).contiguous()
-                    b = torch.cat([torch.zeros(nh, device=w.device), conv.bias.detach()]).contiguous()
+                    w = conv.weight.detach()
+                    w = torch.cat([h.weight.detach()[:, oc:] for h in heads] + [w.new_zeros((lp - nh,) + w.shape[1:]), w],
+                                  dim=0).contiguous()
+                    b = torch.cat([torch.zeros(lp, device=w.device), conv.bias.detach()]).contiguous()
                     return ops.conv3x3_pack(w), b
                 packed, b = self._packed_fn(f"conv{lvl}_4+heads", [conv.weight, conv.bias] + [h.weight for h in heads], build)
-                assert off - oc - nh == 0
-                ops.conv3x3_slices(buf, off, Ctot - off, packed, b, buf, 0, oc + nh, SLOPE, linear_prefix=nh)
+                prefix = torch.empty((N, lp, H, W), device=base.device, dtype=torch.float32)
+                ops.conv3x3_split(act, off, act.channels - off, packed, b, lp + oc, SLOPE, out=prefix, out_split=act,
+                                  out_c0=off - oc, linear_prefix=lp)
             else:
-                ops.conv3x3_slices(buf, off, Ctot - off, self._packed(f"conv{lvl}_{i}"), conv.bias, buf, off - oc, oc, SLOPE)
+                ops.conv3x3_split(act, off, act.channels - off, self._packed(f"conv{lvl}_{i}"), conv.bias, oc, SLOPE,
+                                  out_split=act, out_c0=off - oc)
             off -= oc
-        return _Slab(buf, nh, DECODER_CH[-1] if nh else 0)
+        return _Slab(act, prefix, DECODER_CH[-1] if nh else 0)
 
     def _context(self, x):
-        fast = isinstance(x, _Slab) or self._fast(x)
+        if isinstance(x, _Slab):
+            # inference: dc_conv1 reads the block's split buffer in place, dc_conv1..6 chain in the split format, dc_conv7
+            # writes the fp32 flow
+            act = x.act
+            N, _, H, W = act.shape
+            for i in range(1, 8):
+                conv = getattr(self, f"dc_conv{i}")
+                if i == 7:
+                    y = torch.empty((N, conv.out_channels, H, W), device=act.buf.device, dtype=torch.float32)
+                    ops.conv3x3_split(act, 0, act.channels, self._packed("dc_conv7"), conv.bias, conv.out_channels, 1.0,
+                                      conv.dilation[0], out=y)
+                    return y
+                nxt = ops.SplitAct(N, conv.out_channels, H, W, act.buf.device)
+                ops.conv3x3_split(act, 0, act.channels, self._packed(f"dc_conv{i}"), conv.bias, conv.out_channels, SLOPE,
+                                  conv.dilation[0], out_split=nxt)
+                act = nxt
         for i in range(1, 7):
-            conv = getattr(self, f"dc_conv{i}")
-            if isinstance(x, _Slab):      # first layer reads the block output in place
-                N, _, H, W = x.buf.shape
-                y = torch.empty((N, conv.out_channels, H, W), device=x.buf.device, dtype=torch.float32)
-                ops.conv3x3_slices(x.buf, x.c0, x.channels, self._packed(f"dc_conv{i}"), conv.bias, y, 0, conv.out_channels,
-                                   SLOPE, conv.dilation[0])
-                x = y
-            elif fast:
-                x = ops.conv3x3(x, self._packed(f"dc_conv{i}"), conv.bias, conv.out_channels, SLOPE, conv.dilation[0])
-            else:
-                x = self._conv_act(f"dc_conv{i}", x, SLOPE)
+            x = self._conv_act(f"dc_conv{i}", x, SLOPE)
         return self._plain("dc_conv7", x)
 
     def _make_decoder(self, in_ch: Dict[int, int], with_mask: bool, upfeat_ch):
@@ -331,22 +332,17 @@ class MaskFlownetS(_FlowNetBase):
             corr = ops.correlation(f1, f2, pad_size=self.md, max_displacement=self.md, leaky_slope=SLOPE)
             return self._dense(lvl, torch.cat([corr] + extras, dim=1) if extras else corr)
         tot = D + sum(e.shape[1] for e in extras)
-        # room for the dense block's outputs (written in place) and the heads' partial sums
-        front = (sum(DECODER_CH) + self._heads_front(lvl)) if self.use_tc_conv else 0
-        buf = torch.empty((N, front + tot, H, W), device=f1.device, dtype=torch.float32)
+        buf = torch.empty((N, tot, H, W), device=f1.device, dtype=torch.float32)
         hook = self.event_hook
         if hook is not None:
             hook("corr", lvl, 0)
-        ops.correlation(f1, f2, pad_size=self.md, max_displacement=self.md, leaky_slope=SLOPE,
-                        out=buf[:, front:front + D])
+        ops.correlation(f1, f2, pad_size=self.md, max_displacement=self.md, leaky_slope=SLOPE, out=buf[:, :D])
         if hook is not None:
             hook("corr", lvl, 1)
-        c = front + D
+        c = D
         for e in extras:
             buf[:, c:c + e.shape[1]].copy_(e)
             c += e.shape[1]
-        if front:
-            return self._dense_inplace(lvl, buf, front)
         return self._dense(lvl, buf)
 
     def forward(self, im1: torch.Tensor, im2: torch.Tensor, want_cascade_inputs: bool = False):

@@ -567,6 +567,69 @@ def conv3x3_slices(buf_in: torch.Tensor, c_in0: int, Cin: int, packed: torch.Ten
           _p(ws), ws_bytes)
 
 
+class SplitAct:
+    """An activation of `channels` channels in the split format the convolutions read with tensor copies
+    (include/maskflow_b200.h, mfn_split_pack): per sample, the bf16 hi images of ceil(C/16)*2 groups of 8 channels, then
+    their lo images, 16 bytes per (group, pixel); pad channels are zero.  Writers: pack() and conv3x3_split()."""
+
+    def __init__(self, N: int, channels: int, H: int, W: int, device):
+        self.channels = int(channels)
+        self.buf = torch.empty((N, 2, (self.channels + 15) // 16 * 2, H, W, 16), dtype=torch.uint8, device=device)
+
+    @property
+    def shape(self):
+        N, _, _, H, W, _ = self.buf.shape
+        return N, self.channels, H, W
+
+    def pack(self, src: torch.Tensor, c0: int) -> None:
+        """Channels [c0, c0 + C) = the fp32 NCHW tensor src (C channels; c0 a multiple of 16)."""
+        s = _chk(src, "SplitAct.pack.src")
+        N, C, H, W = s.shape
+        if (N, H, W) != (self.shape[0], self.shape[2], self.shape[3]):
+            raise MaskflowError("SplitAct.pack: src disagrees in N/H/W")
+        _call("mfn_split_pack", s.device, _p(s), C * H * W, N, C, H, W, _p(self.buf), self.channels, int(c0))
+
+    def hi_lo(self):
+        """(hi, lo) as fp32 (N, C, H, W) tensors: the two bf16 terms of every value."""
+        N, C, H, W = self.shape
+        t = self.buf.view(torch.bfloat16).view(N, 2, -1, H, W, 8).permute(0, 1, 2, 5, 3, 4).reshape(N, 2, -1, H, W)
+        return t[:, 0, :C].float(), t[:, 1, :C].float()
+
+
+def conv3x3_split(x: SplitAct, c_in0: int, Cin: int, packed: torch.Tensor, bias: Optional[torch.Tensor], Cout: int,
+                  leaky_slope: float = 0.1, dilation: int = 1, out: Optional[torch.Tensor] = None,
+                  out_split: Optional[SplitAct] = None, out_c0: int = 0, depth_to_space: bool = False,
+                  linear_prefix: int = 0) -> None:
+    """conv3x3_slices reading channels [c_in0, c_in0 + Cin) of a split activation (c_in0 a multiple of 16).  Output: the
+    fp32 NCHW (or depth-to-space) tensor `out`, or -- out_split given -- channels out_c0.. of that split activation, the
+    linear_prefix channels (even) going to the fp32 (N, linear_prefix, H, W) `out`.  Bit-identical to conv3x3_slices on
+    the same values.  Inference only."""
+    N, Cx, H, W = x.shape
+    if not (0 <= c_in0 and c_in0 + Cin <= Cx):
+        raise MaskflowError("conv3x3_split: channel slice out of range")
+    if out is not None:
+        f = Cout // 4 if depth_to_space else (linear_prefix if out_split is not None else Cout)
+        s = 2 if depth_to_space else 1
+        if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.shape == (N, f, s * H, s * W)):
+            raise MaskflowError(f"conv3x3_split: out must be a contiguous CUDA float32 tensor of shape {(N, f, s * H, s * W)}")
+    if out_split is not None and (out_split.shape[0], out_split.shape[2], out_split.shape[3]) != (N, H, W):
+        raise MaskflowError("conv3x3_split: out_split disagrees in N/H/W")
+    if out_split is not None and out_split.buf.data_ptr() == x.buf.data_ptr():
+        # the input is read in whole 16-channel groups, the output written in them
+        r0, r1 = c_in0, -(-(c_in0 + Cin) // 16) * 16
+        w0, w1 = out_c0, out_c0 + Cout - linear_prefix
+        if not (w1 <= r0 or r1 <= w0):
+            raise MaskflowError("conv3x3_split: input and output slices overlap")
+    b = _chk(bias, "conv3x3_split.bias", optional=True)
+    _no_grad_path("conv3x3_split", x.buf, b)
+    ws_bytes = int(_lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, 1, int(dilation)))
+    ws = torch.empty(ws_bytes // 4, device=x.buf.device, dtype=torch.float32) if ws_bytes else None
+    _call("mfn_conv3x3_forward_split", x.buf.device, _p(x.buf), Cx, int(c_in0), _p(packed), _p(b), _p(out), 0,
+          _p(out_split.buf if out_split is not None else None), out_split.channels if out_split is not None else 0,
+          int(out_c0), N, Cin, H, W, Cout, int(dilation), (1 if depth_to_space else 0) | (int(linear_prefix) << 8),
+          float(leaky_slope), _p(ws), ws_bytes)
+
+
 def conv_transpose4x4_as_conv3x3(weight: torch.Tensor) -> torch.Tensor:
     """nn.ConvTranspose2d(Cin, F, kernel 4, stride 2, pad 1) (the decoder's `upfeat` layers, network/MaskFlownet.py:225 ...)
     re-arranged as the weight (4F, Cin, 3, 3) of a 3x3 convolution followed by depth-to-space: output pixel (2y+py, 2x+px)

@@ -3,11 +3,13 @@
     python tools/conv_bound.py [--batch 8] [--height 448] [--width 1024] [--reps 5] [--levels 2,3] [--json FILE]
 
 Runs one eager MaskFlownet-S forward (BASELINE configs[1]: batch 8, 1024x448, seeded inputs and weights) and records every
-convolution launch (ops.conv3x3_slices) with the layer that issued it.  Each recorded launch is then replayed on its own,
-bracketed by CUDA events (median of --reps), in four variants of the profiling knob `conv_dbg` of the wgmma kernel:
+convolution launch (ops.conv3x3_slices / ops.conv3x3_split) with the layer that issued it.  Each recorded launch is then replayed on its own,
+bracketed by CUDA events (median of --reps), in five variants of the profiling knob `conv_dbg` of the wgmma kernel:
 
     full      the real kernel
     -load     producers skip their global loads (they still convert and hand over every stage)
+    -input    producers skip loads, conversion and shared-memory stores (they only hand over every stage): what a free
+              input path would cost
     -store    no epilogue stores
     -mma      no tensor-core MMAs (the barrier protocol is unchanged)
 
@@ -18,7 +20,7 @@ Per launch the table prints the shape, the time, and two lower bounds:
            products per fp32 product, whole rounds of one work item per SM) at the 989 TFLOP/s dense-bf16 data-sheet rate
     hbm    input + output + packed weights once over the 3.35 TB/s data-sheet bandwidth
 
-and `frac` = max(mma, hbm) / time.  The three deltas (time minus the time without a phase) show what each phase adds to
+and `frac` = max(mma, hbm) / time.  The four deltas (time minus the time without a phase) show what each phase adds to
 the critical path.  Both rates are for a 700 W part; a card with a lower power limit runs slower clocks.
 """
 from __future__ import annotations
@@ -37,7 +39,7 @@ from maskflownet_b200 import _lib, network, ops  # noqa: E402
 
 PEAK_FLOPS, PEAK_BW, SMS = 989e12, 3.35e12, 132
 MT, R = 128, 2   # pixels per tile row, rows per tile (csrc/conv3x3_wgmma.cu)
-MODES = (("full", 0), ("-load", 2), ("-store", 4), ("-mma", 8))
+MODES = (("full", 0), ("-load", 2), ("-input", 16), ("-store", 4), ("-mma", 8))
 
 
 def cout_pad(cin: int, cout: int) -> int:
@@ -122,8 +124,23 @@ def main():
                           "args": (buf_in, c_in0, Cin, packed_w, bias, buf_out, c_out0, Cout, leaky_slope, dilation, stride,
                                    depth_to_space, linear_prefix)})
 
+    orig_split = ops.conv3x3_split
+
+    def split(x, c_in0, Cin, packed_w, bias, Cout, leaky_slope=0.1, dilation=1, out=None, out_split=None, out_c0=0,
+              depth_to_space=False, linear_prefix=0):
+        args = (x, c_in0, Cin, packed_w, bias, Cout, leaky_slope, dilation, out, out_split, out_c0, depth_to_space,
+                linear_prefix)
+        orig_split(*args)
+        if recording["on"]:
+            N, _, H, W = x.shape
+            calls.append({"layer": current["name"], "N": N, "Cin": Cin, "H": H, "W": W, "Cout": Cout, "stride": 1,
+                          "dil": dilation, "d2s": depth_to_space, "lin": linear_prefix,
+                          "ws_bytes": int(_lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, 1, dilation)),
+                          "fn": orig_split, "args": args})
+
     network._FlowNetBase._packed, network._FlowNetBase._packed_fn = packed, packed_fn
     ops.conv3x3_slices = slices
+    ops.conv3x3_split = split
     with torch.no_grad():
         for _ in range(2):
             network.predict_flow(model, a, b)            # warm-up: packing, kernel attributes
@@ -134,7 +151,7 @@ def main():
         network.predict_flow(model, a, b)
         e1.record()
         recording["on"] = False
-    ops.conv3x3_slices = orig_slices
+    ops.conv3x3_slices, ops.conv3x3_split = orig_slices, orig_split
     torch.cuda.synchronize()
     step = e0.elapsed_time(e1)
 
@@ -143,7 +160,7 @@ def main():
         for _ in range(args.reps + 1):
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record()
-            orig_slices(*c["args"])
+            c.get("fn", orig_slices)(*c["args"])
             t1.record()
             ts.append((t0, t1))
         torch.cuda.synchronize()
@@ -164,7 +181,7 @@ def main():
           f"times in us (median of {args.reps}); bounds at 989 TFLOP/s bf16 and 3.35 TB/s")
     want = {int(x) for x in args.levels.split(",") if x.strip()}
     hdr = (f"{'layer':16s} {'N':>2s} {'Cin':>4s} {'Cout':>4s} {'H':>4s} {'W':>5s} s d {'time':>8s} {'mma':>8s} {'hbm':>7s} "
-           f"{'frac':>5s} {'load':>7s} {'store':>7s} {'mma':>7s}")
+           f"{'frac':>5s} {'load':>7s} {'input':>7s} {'store':>7s} {'mma':>7s}")
     print(hdr)
     per_level = collections.OrderedDict()
     rows = []
@@ -175,29 +192,30 @@ def main():
         lvl = 2 if c["layer"].startswith("dc_conv") else (int(m.group()) if m else 0)
         kind = "pyramid" if re.fullmatch(r"conv\d[abc]", c["layer"]) else "decoder"
         grp = f"{kind} L{lvl}"
-        d = {k: c["full"] - c[k] for k in ("-load", "-store", "-mma")}
-        row = {k: v for k, v in c.items() if k != "args"}
+        d = {k: c["full"] - c[k] for k in ("-load", "-input", "-store", "-mma")}
+        row = {k: v for k, v in c.items() if k not in ("args", "fn")}
         row.update(level=lvl, group=grp, mma_us=mma * 1e6, hbm_us=hbm * 1e6, useful_us=useful * 1e6,
                    frac=max(mma, hbm) / t)
         rows.append(row)
-        agg = per_level.setdefault(grp, [0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0])
-        for i, v in enumerate((c["full"], mma * 1e3, hbm * 1e3, useful * 1e3, d["-load"], d["-store"], d["-mma"])):
+        agg = per_level.setdefault(grp, [0.0] * 8 + [0])
+        for i, v in enumerate((c["full"], mma * 1e3, hbm * 1e3, useful * 1e3, d["-load"], d["-input"], d["-store"],
+                               d["-mma"])):
             agg[i] += v
-        agg[7] += 1
+        agg[8] += 1
         if want and lvl not in want:
             continue
         print(f"{c['layer']:16s} {c['N']:2d} {c['Cin']:4d} {c['Cout']:4d} {c['H']:4d} {c['W']:5d} {c['stride']} "
               f"{c['dil']:<2d}{c['full'] * 1e3:7.0f} {mma * 1e6:8.0f} {hbm * 1e6:7.0f} {max(mma, hbm) / t:5.2f} "
-              f"{d['-load'] * 1e3:7.0f} {d['-store'] * 1e3:7.0f} {d['-mma'] * 1e3:7.0f}")
+              f"{d['-load'] * 1e3:7.0f} {d['-input'] * 1e3:7.0f} {d['-store'] * 1e3:7.0f} {d['-mma'] * 1e3:7.0f}")
     print(f"\n{'group':12s} {'calls':>5s} {'time':>8s} {'mma':>8s} {'useful':>8s} {'hbm':>7s} {'frac':>5s} "
-          f"{'load':>7s} {'store':>7s} {'mma':>7s}   (us; frac = mma bound / time)")
-    tot = [0.0] * 7 + [0]
+          f"{'load':>7s} {'input':>7s} {'store':>7s} {'mma':>7s}   (us; frac = mma bound / time)")
+    tot = [0.0] * 8 + [0]
     for grp, v in sorted(per_level.items(), key=lambda kv: -kv[1][0]):
         tot = [x + y for x, y in zip(tot, v)]
-        print(f"{grp:12s} {v[7]:5d} {v[0] * 1e3:8.0f} {v[1] * 1e3:8.0f} {v[3] * 1e3:8.0f} {v[2] * 1e3:7.0f} "
-              f"{v[1] / v[0]:5.2f} {v[4] * 1e3:7.0f} {v[5] * 1e3:7.0f} {v[6] * 1e3:7.0f}")
-    print(f"{'all':12s} {tot[7]:5d} {tot[0] * 1e3:8.0f} {tot[1] * 1e3:8.0f} {tot[3] * 1e3:8.0f} {tot[2] * 1e3:7.0f} "
-          f"{tot[1] / tot[0]:5.2f} {tot[4] * 1e3:7.0f} {tot[5] * 1e3:7.0f} {tot[6] * 1e3:7.0f}")
+        print(f"{grp:12s} {v[8]:5d} {v[0] * 1e3:8.0f} {v[1] * 1e3:8.0f} {v[3] * 1e3:8.0f} {v[2] * 1e3:7.0f} "
+              f"{v[1] / v[0]:5.2f} {v[4] * 1e3:7.0f} {v[5] * 1e3:7.0f} {v[6] * 1e3:7.0f} {v[7] * 1e3:7.0f}")
+    print(f"{'all':12s} {tot[8]:5d} {tot[0] * 1e3:8.0f} {tot[1] * 1e3:8.0f} {tot[3] * 1e3:8.0f} {tot[2] * 1e3:7.0f} "
+          f"{tot[1] / tot[0]:5.2f} {tot[4] * 1e3:7.0f} {tot[5] * 1e3:7.0f} {tot[6] * 1e3:7.0f} {tot[7] * 1e3:7.0f}")
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"device": dev, "eager_forward_ms": step, "rows": rows}, f, indent=1)
