@@ -1,4 +1,4 @@
-"""Differentiable torch-CPU restatement of the hot-path operators.  TEST INFRASTRUCTURE ONLY.
+"""Differentiable torch restatement of the hot-path operators.  TEST INFRASTRUCTURE ONLY.
 
 Same semantics as oracle/mfn_oracle.c (which it is checked against in tests/test_oracle.py), written as
 plain torch expressions so that torch.autograd yields the analytic backward used to check the CUDA
@@ -84,8 +84,8 @@ def deformable_conv(x, offset, weight, bias=None, border_mode: int = 0):
     N, C, H, W = x.shape
     Fo = weight.shape[0]
     assert weight.shape[1:] == (C, 3, 3) and offset.shape == (N, 18, H, W)
-    ys = torch.arange(H, dtype=x.dtype).view(1, H, 1)
-    xs = torch.arange(W, dtype=x.dtype).view(1, 1, W)
+    ys = torch.arange(H, dtype=x.dtype, device=x.device).view(1, H, 1)
+    xs = torch.arange(W, dtype=x.dtype, device=x.device).view(1, 1, W)
     cols = []
     for i in range(3):
         for j in range(3):
@@ -107,7 +107,7 @@ def upsample(x: torch.Tensor, factor: int) -> torch.Tensor:
     N, C, H, W = x.shape
     f = factor
     c = f - 1
-    t = torch.arange(2 * f - 1, dtype=x.dtype)
+    t = torch.arange(2 * f - 1, dtype=x.dtype, device=x.device)
     k1 = 1 - (c - t).abs() / (c + 1)
     k2 = (k1[:, None] * k1[None, :]).view(1, 1, 2 * f - 1, 2 * f - 1)
     b = x.reshape(N * C, 1, H, W)
@@ -119,8 +119,8 @@ def upsample(x: torch.Tensor, factor: int) -> torch.Tensor:
 def reconstruction2d(x: torch.Tensor, flow_yx: torch.Tensor) -> torch.Tensor:
     """layer.Reconstruction2D: sample x at (y + flow[:,0], x + flow[:,1]), zero outside."""
     N, C, H, W = x.shape
-    ys = torch.arange(H, dtype=x.dtype).view(1, H, 1)
-    xs = torch.arange(W, dtype=x.dtype).view(1, 1, W)
+    ys = torch.arange(H, dtype=x.dtype, device=x.device).view(1, H, 1)
+    xs = torch.arange(W, dtype=x.dtype, device=x.device).view(1, 1, W)
     gx = (flow_yx[:, 1] + xs) / ((W - 1) / 2) - 1
     gy = (flow_yx[:, 0] + ys) / ((H - 1) / 2) - 1
     grid = torch.stack([gx, gy], dim=-1)

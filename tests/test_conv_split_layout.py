@@ -1,8 +1,9 @@
 """Split activations (ops.SplitAct, include/maskflow_b200.h: mfn_split_pack / mfn_conv3x3_forward_split): the packed
 values are the bf16 hi/lo split of the fp32 values, and a convolution that reads its input from a split buffer (tensor
 copies) and / or writes its output into one gives bit for bit the result of the fp32 path (conv3x3_slices) -- for partial
-and whole input chunks, linear prefixes, dilations 1, 2 and 16, staged and register epilogues, the split-K plan and capped
-persistent grids.  Whole networks: the flows equal those of the fp32 dense block exactly."""
+and whole input chunks, linear prefixes, dilations 1, 2, 4, 8 and 16, staged and register epilogues, the split-K plans
+(small images, and a short last round reduced into split output) and capped persistent grids.  Whole networks: the flows
+equal those of the fp32 dense block exactly."""
 import pytest
 import torch
 
@@ -32,7 +33,7 @@ def test_pack_round_trip():
     assert int(raw[:, :, 6, :, :, 6:].abs().sum()) == 0 and int(raw[:, :, 7].abs().sum()) == 0
 
 
-CASES = [   # (N, Cin, H, W, Cout, linear prefix, dilation)
+CASES = [   # (N, Cin, H, W, Cout, linear prefix, dilation[, grid cap that makes the last round short])
     (2, 131, 6, 256, 32, 0, 1),     # partial last chunk, staged fp32 epilogue
     (2, 547, 4, 256, 34, 2, 1),     # conv2_4 + heads
     (2, 547, 5, 130, 36, 4, 1),     # conv3_4 + heads (padded prefix), register epilogue
@@ -42,15 +43,24 @@ CASES = [   # (N, Cin, H, W, Cout, linear prefix, dilation)
     (8, 675, 14, 32, 64, 0, 1),     # level 5: split-K over the input chunks
     (8, 547, 7, 16, 34, 2, 1),      # level 6 conv6_4 + heads: split-K with a linear prefix and split output (reduce kernel)
     (1, 128, 40, 130, 128, 0, 16),  # dilation 16 with in-bounds rows for every tap
+    (1, 128, 10, 130, 128, 0, 4),   # dc_conv3: dilation 4, rows partly in bounds
+    (2, 128, 18, 130, 96, 0, 8),    # dc_conv4: dilation 8, rows partly in bounds
+    # short last round on a 12-CTA grid (28 tiles = 2 x 12 + 4): the last sample's tail rows split over 3 parts and
+    # reduced into the split output (y_lo > 0, n_lo > 0)
+    (2, 259, 14, 130, 96, 0, 1, 12),
 ]
 
 
 @pytest.mark.parametrize("cap", [0, 1, 3])
 @pytest.mark.parametrize("case", CASES)
 def test_split_conv_is_bit_identical(case, cap):
-    N, Cin, H, W, Cout, lp, dil = case
+    N, Cin, H, W, Cout, lp, dil, *last_round_cap = case
     if cap and N * Cin * H > 20000:
         pytest.skip("grid caps: the small shapes suffice")
+    if last_round_cap:
+        if cap:
+            pytest.skip("the case brings its own grid cap")
+        cap = last_round_cap[0]
     g = torch.Generator().manual_seed(Cin + Cout)
     x = leaky((N, Cin + 16, H, W), g)          # the convolution reads channels [16, 16 + Cin)
     w = torch.randn((Cout, Cin, 3, 3), generator=g).to(DEV) / (3 * Cin ** 0.5)
@@ -58,6 +68,8 @@ def test_split_conv_is_bit_identical(case, cap):
     packed = ops.conv3x3_pack(w)
     _lib.set_tuning("conv_grid_cap", cap)
     try:
+        if last_round_cap:    # the tail of the last sample only: a proper part of the output
+            assert 0 < _lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, 1, dil) < 4 * N * Cout * H * W
         ref = torch.empty((N, Cout, H, W), device=DEV)
         ops.conv3x3_slices(x, 16, Cin, packed, b, ref, 0, Cout, 0.1, dil, linear_prefix=lp)
         xs = ops.SplitAct(N, Cin + 16, H, W, DEV)

@@ -582,7 +582,8 @@ def test_conv3x3_persistent_tile_loop(cap):
 @pytest.mark.parametrize("border", [0, 1])
 @pytest.mark.parametrize("lin", [1, 0])
 @pytest.mark.parametrize("N,C,H,W,flow_mag", [(2, 32, 28, 64, 0.3), (1, 64, 30, 132, 1.5), (1, 16, 12, 20, 4.0), (1, 40, 16, 24, 0.0),
-                                              (2, 128, 14, 32, 0.6), (1, 96, 28, 64, 2.5), (1, 8, 4, 6, 0.8)])
+                                              (2, 128, 14, 32, 0.6), (1, 96, 28, 64, 2.5), (1, 8, 4, 6, 0.8),
+                                              (2, 196, 8, 16, 1.2)])    # F = 196: CoutP 256, two 128-channel halves
 def test_warp_mask_through_linearity_matches_tap_by_tap(N, C, H, W, flow_mag, border, lin):
     """mfn_warp_mask_forward_resample == the oracle's deformable convolution, both border rules, flows from sub-pixel to far
     outside the image.  lin=1: every pixel through linearity (extended wgmma convolution + band tables, warp_lin.cu);
