@@ -528,33 +528,49 @@ class PipelinedFlowPredictor:
         --D2H (copy stream)--> pinned fp32 flow
     with `depth` staging slots, so the H2D copy of request i+1 and the D2H copy of result i-1 run under the forward of
     request i (PCIe is full duplex; 22 MB in / 29 MB out per batch of 8 at 1024x448).
+    One set of slots per input shape (and dtype), keyed like FlowPredictor's graphs: requests of different batch sizes or
+    frame sizes may be interleaved, and each shape's slots rotate on their own.
     Results are complete after synchronize() (or after waiting on the event infer() returns)."""
 
     def __init__(self, net: nn.Module, depth: int = 2):
         self.pred = FlowPredictor(net)
         self.depth = depth
-        self._slots = None
-        self._i = 0
+        self._slots = {}          # (shape, dtype) -> [slots of that shape, requests enqueued with it]
+        self.h2d = self.d2h = None
 
     def _setup(self, img1, dev):
         shp = tuple(img1.shape)
         N, _, H, W = shp
-        self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
-        self._slots = []
+        if self.h2d is None:
+            self.h2d, self.d2h = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
+        slots = []
         for _ in range(self.depth):
-            self._slots.append({
+            slots.append({
                 "in1": torch.empty(shp, dtype=img1.dtype, device=dev), "in2": torch.empty(shp, dtype=img1.dtype, device=dev),
                 "out": torch.empty((N, 2, H, W), dtype=torch.float32, device=dev),
                 "ev_h2d": torch.cuda.Event(), "ev_in_free": torch.cuda.Event(), "ev_out": torch.cuda.Event(),
                 "ev_out_free": torch.cuda.Event(), "used": False})
+        # the slots come from the allocator on the current stream (their memory may still be in use there, and under
+        # torch.use_deterministic_algorithms a fill is queued on it): the copy streams start after that
+        cur = torch.cuda.current_stream(dev)
+        self.h2d.wait_stream(cur)
+        self.d2h.wait_stream(cur)
+        return [slots, 0]
 
     @torch.no_grad()
     def infer(self, img1_host: torch.Tensor, img2_host: torch.Tensor, out_host: torch.Tensor) -> torch.cuda.Event:
         dev = next(self.pred.net.parameters()).device
-        if self._slots is None:
-            self._setup(img1_host, dev)
-        s = self._slots[self._i % self.depth]
-        self._i += 1
+        if img2_host.shape != img1_host.shape or img2_host.dtype != img1_host.dtype:
+            raise ValueError(f"infer: img1 {tuple(img1_host.shape)} and img2 {tuple(img2_host.shape)} differ")
+        key = (tuple(img1_host.shape), img1_host.dtype)
+        entry = self._slots.get(key)
+        if entry is None:
+            entry = self._slots[key] = self._setup(img1_host, dev)
+        N, _, H, W = key[0]
+        if tuple(out_host.shape) != (N, 2, H, W):
+            raise ValueError(f"infer: out_host is {tuple(out_host.shape)}, the flow of this request is {(N, 2, H, W)}")
+        s = entry[0][entry[1] % self.depth]
+        entry[1] += 1
         cur = torch.cuda.current_stream(dev)
         with torch.cuda.stream(self.h2d):
             if s["used"]:
@@ -577,7 +593,7 @@ class PipelinedFlowPredictor:
         return s["ev_out_free"]
 
     def synchronize(self) -> None:
-        if self._slots is not None:
+        if self.h2d is not None:
             self.h2d.synchronize()
             self.d2h.synchronize()
         torch.cuda.current_stream().synchronize()

@@ -11,6 +11,7 @@ The references are plain torch in float64 on the GPU (cuDNN fp64 convolutions, o
 Bound, per output element, with Q = sqrt(x^2 (*) w^2) (the scale of random rounding errors) and S = |x| (*) |w| + |b|:
     tensor-core launches (bf16 hi/lo split operands, fp32 accumulation)    |got - ref| <= 2^-12 Q + 2^-20 S
     exact-fp32 launches (SIMT warp, sampler, upsample)                      |got - ref| <= 2^-20 S
+    plus, where the output is stored as a split activation (bf16 hi + lo), its rounding 2^-16 |ref| (split_storage_term).
 The split's expected error is ~2^-17 Q; a bf16-only product errs by ~2^-9 Q and a dropped tap by ~Q / 3.  Where the
 reference's pre-activation is below -bound the LeakyReLU scales the error by its slope, and so the bound.
 
@@ -49,6 +50,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "gol
 from make_golden import named_init, seeded_images  # noqa: E402
 
 EPS_Q, EPS_S = 2.0 ** -12, 2.0 ** -20
+EPS_STORE = 2.0 ** -16
 CONTROL_MARGIN = 3.0
 
 
@@ -92,6 +94,19 @@ def conv_terms(x, w, b, stride=1, dilation=1, transposed=False):
     Q = op(x * x, w * w).sqrt()
     S = op(x.abs(), w.abs()) + (b.abs().view(1, -1, 1, 1) if b is not None else 0.0)
     return pre, Q, S
+
+
+def split_storage_term(pre, store_from):
+    """Bound on the rounding of an output stored as a split activation: hi = bf16(v), lo = bf16(v - hi), both rounded to
+    nearest with 8-bit significands, so |v - hi - lo| <= 2^-8 |v - hi| <= 2^-16 |v|.  Channels >= store_from (a linear
+    prefix stays fp32); 0 for an fp32 output (store_from None).  In pre-activation units, so that judge's slope scaling
+    applies to it as to the rest of the bound.  It matters where Q is small next to |v|: a bias-dominated output, e.g.
+    a 1x1 level whose correlation input is zero but for the centre displacement."""
+    if store_from is None:
+        return 0.0
+    t = EPS_STORE * pre.abs()
+    t[:, :store_from] = 0
+    return t
 
 
 def conv_near_misses(x, w, b, stride=1, dilation=1, transposed=False):
@@ -265,7 +280,7 @@ class Recorder:
 
     # ---- convolutions -----------------------------------------------------------------------------------------
     def _check_conv(self, op, packed, bias, Cout, slope, dil, stride, d2s, lp, x_of, got_of, N, Cin, H, W, ws, kern,
-                    tags):
+                    tags, store_from=None):
         w, transposed = self.packs[packed.data_ptr()]
         name = self.names.get(packed.data_ptr(), "?")
         assert transposed == d2s, name
@@ -278,7 +293,7 @@ class Recorder:
             for n in range(N):
                 x = x_of(n)
                 pre, Q, S = conv_terms(x, w, b, stride, dil, transposed)
-                bound = EPS_Q * Q + EPS_S * S
+                bound = EPS_Q * Q + EPS_S * S + split_storage_term(pre, store_from)
                 r, rq = judge(got_of(n), pre, sl, bound, Q)
                 worst, worst_q = max(worst, r), max(worst_q, rq)
                 for tag in tags:
@@ -342,7 +357,8 @@ class Recorder:
         tags = (["split"] if out_split is not None else []) + (["d2s"] if d2s else []) + (["lin"] if lp else []) + \
             (["dil>=4"] if dil >= 4 else [])
         self._check_conv("conv3x3_split", a["packed"], a["bias"], Cout, a["leaky_slope"], dil, 1, d2s, lp,
-                         lambda n: _split_values(x, n, c_in0, c_in0 + Cin), got_of, N, Cin, H, W, ws, kern, tags)
+                         lambda n: _split_values(x, n, c_in0, c_in0 + Cin), got_of, N, Cin, H, W, ws, kern, tags,
+                         lp if out_split is not None else None)
 
     def split_pack(self, act, src, c0):
         N, C, H, W = src.shape
@@ -414,6 +430,13 @@ class Recorder:
         N, C, H, W = x.shape
         F = w.shape[0]
         exact = kern.startswith("deform_fwd_kernel")          # the SIMT kernel of the training graph
+        # warp_mma_kernel (below 4 px, F <= 128) gathers tap by tap at the SIMT kernel's positions: its offsets are
+        # fl(fl(f * scale) / stride) from the up-sampled flow it also returns, its positions fl((y - 1 + i) + d), so the
+        # reference's positions are its own.  Each bilinear sample is formed in fp32 (corner weights (1 - l) * (1 - l'),
+        # four products, three sums: <= 6u of sum |w_corner v_corner|, inside 2^-20 S), then split into bf16 hi + lo
+        # and multiplied hi*hi + hi*lo + lo*hi into fp32 accumulators, as the wgmma convolution does: the tensor-core
+        # bound holds with no position term.
+        through_linearity = not exact and not kern.startswith("warp_mma_kernel")
         eps_q = 0.0 if exact else EPS_Q
         sl = channel_slopes(F, slope, 0, x.device)
         worst = worst_q = worst_up = worst_fixed = 0.0
@@ -438,7 +461,7 @@ class Recorder:
                     pre, S = pre + tn, S + tn.abs()
                 bound = eps_q * Q + EPS_S * S
                 worst_fixed = max(worst_fixed, judge(out[n:n + 1], pre, sl, bound, Q)[0])
-                if not exact:
+                if through_linearity:
                     # through linearity every tap row samples the zero-corner operator at the one rounded position
                     # fl(y + d) shifted by whole pixels, and the MXNet-1.5 band correction at fl((y - 1 + i) + d), the
                     # tap-by-tap operator's positions: each part is off by up to one ulp of |y| + |d| + 1 (likewise
