@@ -267,6 +267,13 @@ MFN_API int mfn_conv3x3_forward(const float* x, long long x_batch_stride, const 
 /* out_mode | (k << 8), NCHW only: the first k output channels are written without the activation (a linear head that shares
  * the input pass of an activated layer; network.py folds pred_flow / pred_mask over the dense block's input into conv{L}_4) */
 #define MFN_CONV_OUT_LINEAR_PREFIX(k) ((k) << 8)
+/* out_mode | MFN_CONV_BF16 (mfn_conv3x3_forward_ex, _ws, _split): opt-in bf16 inference arithmetic.  The input and the
+ * weights are each rounded once to bf16 (nearest even: the "hi" of the split), each product is the one MMA hi*hi, exact
+ * in fp32, and products accumulate in fp32; bias, activation, linear prefix, depth-to-space and split-K are unchanged.
+ * Each product errs by up to about 2^-7 relative (two roundings to 8 significant bits) instead of about 2^-17.  Only the wgmma kernel has this variant: the bit
+ * returns MFN_ERR_UNSUPPORTED where the mma.sync kernel would run (tuning "conv_wgmma" = 0, or W < "conv_wgmma_min_w").
+ * mfn_conv3x3_workspace_bytes does not depend on it. */
+#define MFN_CONV_BF16 0x10
 MFN_API int mfn_conv3x3_forward_ex(const float* x, long long x_batch_stride, const void* packed_weight, const float* bias,
                                    float* out, long long out_batch_stride, int N, int Cin, int H, int W, int Cout,
                                    int stride, int dilation, int out_mode, float leaky_slope, void* stream);
@@ -300,6 +307,13 @@ MFN_API int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, con
  *   results are bit-identical. */
 MFN_API int mfn_split_pack(const float* src, long long src_batch_stride, int N, int C, int H, int W, void* dst,
                            int dst_channels, int dst_c0, void* stream);
+/* bf16 activations (MFN_CONV_BF16): the split layout with ONE plane, (N, 1, Cg, H, W, 8) bf16 -- the hi image alone, every
+ * value rounded once to bf16, nearest even -- 2 bytes per channel-pixel, channels past C zero.
+ * mfn_bf16_pack: mfn_split_pack into a bf16-activation buffer (same arguments and slice rules).
+ * mfn_conv3x3_forward_split with out_mode | MFN_CONV_BF16 reads x and writes out_split as bf16 activations; its fp32
+ *   outputs (`out`: NCHW, depth-to-space or the linear prefix) stay fp32. */
+MFN_API int mfn_bf16_pack(const float* src, long long src_batch_stride, int N, int C, int H, int W, void* dst,
+                          int dst_channels, int dst_c0, void* stream);
 MFN_API int mfn_conv3x3_forward_split(const void* x, int x_channels, int x_c0, const void* packed_weight, const float* bias,
                                       float* out, long long out_batch_stride, void* out_split, int out_split_channels,
                                       int out_split_c0, int N, int Cin, int H, int W, int Cout, int dilation, int out_mode,

@@ -55,6 +55,7 @@ SIGNATURES = {
     "mfn_conv3x3_forward_ws": [_f, _ll, _f, _f, _f, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _fl, _f, _ll, _f],
     "mfn_conv3x3_forward_split": [_f, _i, _i, _f, _f, _f, _ll, _f, _i, _i] + [_i] * 7 + [_fl, _f, _ll, _f],
     "mfn_split_pack": [_f, _ll, _i, _i, _i, _i, _f, _i, _i, _f],
+    "mfn_bf16_pack": [_f, _ll, _i, _i, _i, _i, _f, _i, _i, _f],
 }
 
 

@@ -23,4 +23,15 @@ __device__ __forceinline__ void split_pair(float a, float b, uint32_t& hi, uint3
 #endif
 }
 
+// (a, b) fp32 -> packed bf16x2 rounded to nearest even: the "hi" of split_pair alone, the operand of the bf16 mode
+__device__ __forceinline__ uint32_t bf16_pair(float a, float b) {
+  uint32_t r;
+#ifndef MFN_HOST_EMULATION
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+#else
+  r = cvt_bf16x2_rn(a, b);
+#endif
+  return r;
+}
+
 }  // namespace mfn

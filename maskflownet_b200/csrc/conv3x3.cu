@@ -350,6 +350,8 @@ extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, 
   MFN_REQUIRE(stride == 1 || (stride == 2 && dilation == 1), MFN_ERR_UNSUPPORTED,
               "mfn_conv3x3_forward: stride must be 1, or 2 with dilation 1 (got stride %d, dilation %d)", stride, dilation);
   MFN_REQUIRE(aligned(packed_weight, 16), MFN_ERR_ALIGNMENT, "mfn_conv3x3_forward: packed weights must be 16-byte aligned");
+  const int bf16 = out_mode & MFN_CONV_BF16;   // passed on to the wgmma kernel, the only one with the bf16 variant
+  out_mode &= ~MFN_CONV_BF16;
   const int lin_prefix = out_mode >> 8, mode = out_mode & 0xff;
   MFN_REQUIRE(mode == MFN_CONV_OUT_NCHW || (mode == MFN_CONV_OUT_DEPTH_TO_SPACE2 && stride == 1 && Cout % 4 == 0),
               MFN_ERR_INVALID_ARG, "mfn_conv3x3_forward: depth-to-space output needs stride 1 and Cout %% 4 == 0");
@@ -365,12 +367,15 @@ extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, 
   const bool sync_ok = Cout <= 128 && stride == 1 && mode == MFN_CONV_OUT_NCHW;   // what the mma.sync kernels cover
   if ((tuning().conv_wgmma && W >= tuning().conv_wgmma_min_w) || !sync_ok) {   // wgmma kernel
     const int rc = conv3x3_wgmma_launch(x, xbs, wp + conv3x3_sync_packed_bytes(Cin, Cout), bias, out, obs, N, Cin, H, W,
-                                       Cout, stride, dilation, out_mode, leaky_slope, st, 0, static_cast<float*>(workspace),
-                                       workspace_bytes);
+                                       Cout, stride, dilation, out_mode | bf16, leaky_slope, st, 0,
+                                       static_cast<float*>(workspace), workspace_bytes);
     if (rc != -1) return rc;
     MFN_REQUIRE(sync_ok, MFN_ERR_UNSUPPORTED, "mfn_conv3x3_forward: shape fits neither kernel (Cout=%d stride=%d dilation=%d)",
                 Cout, stride, dilation);
   }
+  MFN_REQUIRE(!bf16, MFN_ERR_UNSUPPORTED,
+              "mfn_conv3x3_forward: MFN_CONV_BF16 runs on the wgmma kernel only, and this launch would take the mma.sync "
+              "kernel (tuning conv_wgmma = 0, or W = %d < conv_wgmma_min_w)", W);
   const int nt = (Cout + 7) / 8;   // n8 tiles needed
   if (nt <= 4) return launch_conv<1, 4>(x, xbs, wp, bias, out, obs, N, Cin, H, W, Cout, dilation, leaky_slope, lin_prefix, st);
   if (nt <= 8) return launch_conv<1, 8>(x, xbs, wp, bias, out, obs, N, Cin, H, W, Cout, dilation, leaky_slope, lin_prefix, st);
@@ -386,6 +391,8 @@ extern "C" int mfn_conv3x3_forward_split(const void* x, int x_channels, int x_c0
   using namespace mfn;
   MFN_REQUIRE(workspace_bytes >= 0 && (workspace || workspace_bytes == 0) && aligned(workspace, 16), MFN_ERR_INVALID_ARG,
               "mfn_conv3x3_forward_split: workspace must be 16-byte aligned (or null with 0 bytes)");
+  const int bf16 = out_mode & MFN_CONV_BF16;   // x and out_split are bf16 activations
+  out_mode &= ~MFN_CONV_BF16;
   const int lin_prefix = out_mode >> 8, mode = out_mode & 0xff;
   MFN_REQUIRE(x && packed_weight && (out || (out_split && lin_prefix == 0)), MFN_ERR_INVALID_ARG,
               "mfn_conv3x3_forward_split: null pointer");
@@ -415,7 +422,7 @@ extern "C" int mfn_conv3x3_forward_split(const void* x, int x_channels, int x_c0
   sio.out_c0 = out_split_c0;
   const unsigned char* wp = static_cast<const unsigned char*>(packed_weight);
   const int rc = conv3x3_wgmma_launch(nullptr, 0, wp + conv3x3_sync_packed_bytes(Cin, Cout), bias, out, obs, N, Cin, H, W,
-                                      Cout, 1, dilation, out_mode, leaky_slope, as_stream(stream), 0,
+                                      Cout, 1, dilation, out_mode | bf16, leaky_slope, as_stream(stream), 0,
                                       static_cast<float*>(workspace), workspace_bytes, sio);
   MFN_REQUIRE(rc != -1, MFN_ERR_UNSUPPORTED,
               "mfn_conv3x3_forward_split: unsupported (odd dilation >= 2, split output slice not 16-channel aligned "

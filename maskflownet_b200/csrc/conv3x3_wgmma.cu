@@ -19,6 +19,9 @@
 //     rows and asynchronous bulk copies when the output rows are 16-byte aligned, else from registers -- or, for the
 //     transposed convolutions, scatter 2x2 sub-pixel phases (depth-to-space).
 //   * layers wider than 128 output channels are cut into two 128-channel work items per tile (register budget).
+//   * TERMS (template argument) = products per multiply-add: 3 is the hi/lo split above; 1 is the opt-in bf16 mode
+//     (MFN_CONV_BF16): only A_hi x B_hi, the input stage holds the hi plane alone, the weight ring streams the hi half of
+//     the same packed image, and split outputs are bf16 activations (one plane, split_act.cuh).
 #include <cstring>
 
 #include "mma_tiles.cuh"
@@ -231,12 +234,14 @@ struct SmemMap {
 constexpr int STG_CH = 32, SPITCH = MT + 4;
 constexpr int STG_BYTES = R * STG_CH * SPITCH * 4;
 // stage counts from the shared-memory budget: 3 input stages when that still leaves >= 8 weight stages, else 2.
-// stg: bytes of the epilogue staging rows (0 = the layer stores from registers)
-__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0) {
+// stg: bytes of the epilogue staging rows (0 = the layer stores from registers).  terms = 1: the input and weight stages
+// hold the hi images alone (half the bytes; w_tile is then the hi tile [2 planes][CoutP][16 B] in shared memory, while
+// the packed image in global memory keeps its 64 CoutP bytes per tap)
+__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0, int terms = 3) {
   SmemMap m;
   m.a_lo = 2 * E * 16;              // hi image: two 8-channel planes of E entries
-  m.a_stage = 2 * m.a_lo;           // hi + lo
-  m.w_tile = 64 * CoutP;            // [hi | lo][2 planes][CoutP][16 B]
+  m.a_stage = terms == 1 ? m.a_lo : 2 * m.a_lo;   // hi (+ lo)
+  m.w_tile = terms == 1 ? 32 * CoutP : 64 * CoutP;   // [hi (| lo)][2 planes][CoutP][16 B]
   const int budget = 227 * 1024 - BAR_BYTES - stg;
   m.w_stage = taps_per_stage(CoutP) * m.w_tile;
   // input stages: narrow layers (several taps per weight stage) take 4 when >= 4 weight stages still fit; wide layers keep
@@ -287,8 +292,9 @@ __global__ void conv3x3_pack_wgmma_kernel(const float* __restrict__ w, unsigned 
   }
 }
 
-// NW: accumulator columns per 64-pixel block (FOLD: 2 x CoutP, else CoutP or 128 per channel half)
-template <int NW, bool FOLD, int TPS>
+// NW: accumulator columns per 64-pixel block (FOLD and TERMS = 3: 2 x CoutP, else CoutP or 128 per channel half).
+// FOLD: the packed image has the folded layout (CoutP <= 64).  TERMS: 3 (hi/lo split) or 1 (bf16: hi x hi only).
+template <int NW, bool FOLD, int TPS, int TERMS>
 __global__ void __launch_bounds__(um::NTHREADS, 1)
     conv3x3_wgmma_kernel(const float* __restrict__ x, long long x_bs, const unsigned char* __restrict__ wpack,
                          const float* __restrict__ bias_arg, float* __restrict__ out_base, long long out_bs, int Cin, int H, int W,
@@ -305,11 +311,14 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   // dbg (tuning "conv_dbg", profiling only, results invalid): 2 = producers skip their global loads, 4 = no epilogue
   // stores, 8 = no MMAs, 16 = producers skip loads, conversion and shared-memory stores (they only hand over each stage);
   // the barrier protocol is unchanged, so each phase can be timed by removing it.
-  constexpr int NCOL = FOLD ? NW / 2 : NW;   // output channels per work item
+  static_assert(TERMS == 1 || TERMS == 3, "one or three products per multiply-add");
+  constexpr bool FOLD_ACC = FOLD && TERMS == 3;   // the accumulator holds the [hi*hi | hi*lo] column blocks
+  constexpr int P = TERMS == 1 ? 1 : 2;           // planes of the input stage and of a split output
+  constexpr int NCOL = FOLD_ACC ? NW / 2 : NW;    // output channels per work item
   const int out_mode_k = out_mode_arg & 0xff, lin_prefix_k = out_mode_arg >> 8;
   extern __shared__ __align__(128) unsigned char smem[];
   const int nslots = n_slots(stride, dil), PW = row_pitch(stride, dil), E = nslots * PW;
-  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg);
+  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg, TERMS);
   const int AS = sm.AS, WS = sm.WS;
   const uint32_t s_base = smem_u32(smem);
   const uint32_t bar0 = s_base + sm.bar_off;
@@ -335,7 +344,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   if (warp < 8) {
     // ============================ consumers: warpgroup r computes output row r of the tile ============================
     const int r = warp >> 2, wq = warp & 3;
-    const uint32_t a_lbo = (uint32_t)E * 16u, b_lbo = (uint32_t)(FOLD ? 2 * CoutP : CoutP) * 16u;
+    const uint32_t a_lbo = (uint32_t)E * 16u, b_lbo = (uint32_t)(FOLD_ACC ? 2 * CoutP : CoutP) * 16u;
     // descriptor low words (address >> 4) of the nine taps live in registers (the tap loop is fully unrolled)
     uint32_t a_off[9];
 #pragma unroll
@@ -391,7 +400,9 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           for (int mh = 0; mh < 2; ++mh) {
             const uint32_t a16 = a_st16 + a_off[tap] + (uint32_t)(64 * mh);
             const uint64_t a_hi = dh_a | (uint64_t)a16, a_lo = dh_a | (uint64_t)(a16 + a_lo16);
-            if constexpr (FOLD) {
+            if constexpr (TERMS == 1) {
+              wgmma_bf16<NW>(acc[mh], a_hi, b_hi, sc);
+            } else if constexpr (FOLD) {
               wgmma_bf16<NW>(acc[mh], a_hi, b_hi, sc);       // [hi*hi | hi*lo]
               wgmma_bf16<NW / 2>(acc[mh], a_lo, b_hi, 1u);   // += lo*hi into the first block
             } else {
@@ -443,13 +454,13 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         const int x0 = tx * MT;
         const uint32_t seg = (uint32_t)((OW - x0 < MT ? OW - x0 : MT) * 4);
         if (xs.out != nullptr) {
-          // split output (no linear prefix): the piece's SCH / 8 groups x {hi, lo} are staged as rows of MT 16-byte
-          // entries -- exactly their layout in global memory, one contiguous row segment each -- and leave by one bulk copy
-          // per row.  A warp's pair stores cover 8 pixels x 4 words: 32 distinct banks.
+          // split output (no linear prefix): the piece's SCH / 8 groups x P planes ({hi, lo}, or hi alone) are staged as
+          // rows of MT 16-byte entries -- exactly their layout in global memory, one contiguous row segment each -- and
+          // leave by one bulk copy per row.  A warp's pair stores cover 8 pixels x 4 words: 32 distinct banks.
           unsigned char* const sst = reinterpret_cast<unsigned char*>(stg);
 #pragma unroll
           for (int pc = 0; pc < NCOL / SCH; ++pc) {
-            if (t < SCH / 4) bulk_wait_read();
+            if (t < SCH * P / 8) bulk_wait_read();
             named_bar_sync(1 + r, 128);
 #pragma unroll
             for (int jj = 0; jj < SCH / 8; ++jj) {
@@ -457,29 +468,35 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
               const int f = wk.nh * NCOL + 8 * j + 2 * (lane & 3);
               const float b0 = (bias != nullptr && f < Cout) ? __ldg(bias + f) : 0.f;
               const float b1 = (bias != nullptr && f + 1 < Cout) ? __ldg(bias + f + 1) : 0.f;
-              unsigned char* const row = sst + (2 * jj * MT + 16 * wq + (lane >> 2)) * 16 + (lane & 3) * 4;
+              unsigned char* const row = sst + (P * jj * MT + 16 * wq + (lane >> 2)) * 16 + (lane & 3) * 4;
 #pragma unroll
               for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   const int i = 4 * j + 2 * h;
                   float v0 = acc[mh][i], v1 = acc[mh][i + 1];
-                  if constexpr (FOLD) {
+                  if constexpr (FOLD_ACC) {
                     v0 += acc[mh][i + NW / 4];
                     v1 += acc[mh][i + 1 + NW / 4];
                   }
-                  uint32_t hi, lo;
-                  split_pair(leaky(v0 + b0, slope), leaky(v1 + b1, slope), hi, lo);
                   unsigned char* const e = row + (64 * mh + 8 * h) * 16;
-                  *reinterpret_cast<uint32_t*>(e) = hi;
-                  *reinterpret_cast<uint32_t*>(e + MT * 16) = lo;
+                  if constexpr (TERMS == 1) {
+                    *reinterpret_cast<uint32_t*>(e) = bf16_pair(leaky(v0 + b0, slope), leaky(v1 + b1, slope));
+                  } else {
+                    uint32_t hi, lo;
+                    split_pair(leaky(v0 + b0, slope), leaky(v1 + b1, slope), hi, lo);
+                    *reinterpret_cast<uint32_t*>(e) = hi;
+                    *reinterpret_cast<uint32_t*>(e + MT * 16) = lo;
+                  }
                 }
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             named_bar_sync(1 + r, 128);
-            const int f = wk.nh * NCOL + pc * SCH + 8 * (t >> 1);   // first channel of row t = (group t / 2, plane t % 2)
-            if (t < SCH / 4 && f < Cout) {
-              const long long dst = sa::entry(n, t & 1, (xs.out_c0 + f) >> 3, (long long)y * OW + x0, xs.out_Cg, oplane0);
+            // first channel of row t = (group t / P, plane t % P)
+            const int f = wk.nh * NCOL + pc * SCH + 8 * (t >> (P - 1));
+            if (t < SCH * P / 8 && f < Cout) {
+              const long long dst = sa::entry<P>(n, t & (P - 1), (xs.out_c0 + f) >> 3, (long long)y * OW + x0, xs.out_Cg,
+                                                 oplane0);
               bulk_s2g(xs.out + dst, smem_u32(sst + t * MT * 16), seg * 4);
               bulk_commit();
             }
@@ -504,7 +521,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
                 for (int h = 0; h < 2; ++h) {
                   const int i = 4 * j + 2 * h + e;
                   float v = acc[mh][i];
-                  if constexpr (FOLD) v += acc[mh][i + NW / 4];
+                  if constexpr (FOLD_ACC) v += acc[mh][i + NW / 4];
                   row[64 * mh + 8 * h] = leaky(v + b, sl);
                 }
             }
@@ -530,7 +547,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
               for (int e = 0; e < 2; ++e) {
                 const int i = 4 * j + 2 * h + e;
                 float v = acc[mh][i];
-                if constexpr (FOLD) v += acc[mh][i + NW / 4];   // second column block: the hi * lo term
+                if constexpr (FOLD_ACC) v += acc[mh][i + NW / 4];   // second column block: the hi * lo term
                 const int f = wk.nh * NCOL + 8 * j + 2 * (lane & 3) + e;
                 if (f >= Cout) continue;
                 if (xs.out != nullptr && !partial && f >= lin_prefix) {
@@ -538,8 +555,8 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
                   if (e == 0) {
                     const float b0 = bias != nullptr ? __ldg(bias + f) : 0.f, b1 = bias != nullptr ? __ldg(bias + f + 1) : 0.f;
                     float v1 = acc[mh][i + 1];
-                    if constexpr (FOLD) v1 += acc[mh][i + 1 + NW / 4];
-                    sa::put_pair(xs.out, xs.out_Cg, oplane0, n, xs.out_c0 + f - lin_prefix, (size_t)y * OW + xx,
+                    if constexpr (FOLD_ACC) v1 += acc[mh][i + 1 + NW / 4];
+                    sa::put_pair<P>(xs.out, xs.out_Cg, oplane0, n, xs.out_c0 + f - lin_prefix, (size_t)y * OW + xx,
                                  leaky(v + b0, slope), leaky(v1 + b1, slope));
                   }
                 } else if (out_mode == 0) {
@@ -566,12 +583,34 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
       for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
         const Work wk = decode_work(work, sk, nChunks);
         const int cb = wk.cb, ce = wk.ce;
-        const unsigned char* src = wpack + (size_t)cb * 9 * sm.w_tile;
-        for (int it = 9 * cb; it < 9 * ce; it += TPS, src += sm.w_stage) {
-          if (wrapped) mbar_wait(w_empty + 8 * ws, wph ^ 1);
-          mbar_arrive_expect_tx(w_full + 8 * ws, (uint32_t)sm.w_stage);
-          bulk_g2s(s_base + (uint32_t)sm.w_off + ws * (uint32_t)sm.w_stage, src, (uint32_t)sm.w_stage, w_full + 8 * ws);
-          if (++ws == (uint32_t)WS) { ws = 0; wph ^= 1; wrapped = true; }
+        if constexpr (TERMS == 3) {
+          const unsigned char* src = wpack + (size_t)cb * 9 * sm.w_tile;
+          for (int it = 9 * cb; it < 9 * ce; it += TPS, src += sm.w_stage) {
+            if (wrapped) mbar_wait(w_empty + 8 * ws, wph ^ 1);
+            mbar_arrive_expect_tx(w_full + 8 * ws, (uint32_t)sm.w_stage);
+            bulk_g2s(s_base + (uint32_t)sm.w_off + ws * (uint32_t)sm.w_stage, src, (uint32_t)sm.w_stage, w_full + 8 * ws);
+            if (++ws == (uint32_t)WS) { ws = 0; wph ^= 1; wrapped = true; }
+          }
+        } else {
+          // the hi half of each tap's packed tile (64 CoutP bytes in global memory): one contiguous run, or -- folded
+          // layout, [plane][hi rows | lo rows] -- one run of CoutP rows per 8-channel plane
+          const int gt = 64 * CoutP, run = 16 * CoutP;
+          const unsigned char* src = wpack + (size_t)cb * 9 * gt;
+          for (int it = 9 * cb; it < 9 * ce; it += TPS, src += TPS * gt) {
+            if (wrapped) mbar_wait(w_empty + 8 * ws, wph ^ 1);
+            mbar_arrive_expect_tx(w_full + 8 * ws, (uint32_t)sm.w_stage);
+            const uint32_t dst = s_base + (uint32_t)sm.w_off + ws * (uint32_t)sm.w_stage;
+#pragma unroll 1
+            for (int t = 0; t < TPS; ++t) {
+              if constexpr (FOLD) {
+                bulk_g2s(dst + (uint32_t)(t * sm.w_tile), src + t * gt, (uint32_t)run, w_full + 8 * ws);
+                bulk_g2s(dst + (uint32_t)(t * sm.w_tile + run), src + t * gt + 2 * run, (uint32_t)run, w_full + 8 * ws);
+              } else {
+                bulk_g2s(dst + (uint32_t)(t * sm.w_tile), src + t * gt, (uint32_t)sm.w_tile, w_full + 8 * ws);
+              }
+            }
+            if (++ws == (uint32_t)WS) { ws = 0; wph ^= 1; wrapped = true; }
+          }
         }
       }
     }
@@ -590,7 +629,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           int tx, ty, n;
           decode_tile(wk.tile, tilesX, tilesY, sk, tx, ty, n);
           const int x0 = tx * MT - dil, y0 = ty * R;
-          const int gb = n * 2 * xs.in_Cg + xs.in_g0;
+          const int gb = n * P * xs.in_Cg + xs.in_g0;
           for (int c = wk.cb; c < wk.ce; ++c) {
             if (wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);
             const uint32_t bar = a_full + 8 * as, dst = s_base + as * (uint32_t)sm.a_stage;
@@ -601,7 +640,13 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
               const int g = gb + 2 * c;
               if (dil < R) {
                 tma_load_4d(dst, &tmx, 0, x0, y0 - dil, g, bar);
-                tma_load_4d(dst + (uint32_t)sm.a_lo, &tmx, 0, x0, y0 - dil, g + xs.in_Cg, bar);
+                if constexpr (P == 2) tma_load_4d(dst + (uint32_t)sm.a_lo, &tmx, 0, x0, y0 - dil, g + xs.in_Cg, bar);
+              } else if constexpr (P == 1) {
+#pragma unroll 1
+                for (int k = 0; k < 6; ++k) {    // (kernel row ky, group kc), hi plane only
+                  const int ky = k >> 1, kc = k & 1;
+                  tma_load_4d(dst + (uint32_t)((kc * E + ky * R * PW) * 16), &tmx, 0, x0, y0 + (ky - 1) * dil, g + kc, bar);
+                }
               } else {
 #pragma unroll 1
                 for (int k = 0; k < 12; ++k) {   // (kernel row ky, group kc, plane)
@@ -646,7 +691,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         for (int e = pw * 32 + lane; e < E; e += NPROD * 32) {
           unsigned char* d = smem + st * sm.a_stage + (E + e) * 16;
           *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
-          *reinterpret_cast<uint4*>(d + sm.a_lo) = make_uint4(0u, 0u, 0u, 0u);
+          if constexpr (P == 2) *reinterpret_cast<uint4*>(d + sm.a_lo) = make_uint4(0u, 0u, 0u, 0u);
         }
     }
     // load cursor (runs one batch ahead of the store cursor)
@@ -727,14 +772,19 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         const int kc = one_plane ? 0 : (t & 1);
         const int e = (one_plane ? t : (t >> 1)) * 32 + lane;
         if (t < nItems && e < E) {
-          uint4 hi, lo;
-          split_pair(v[b][0], v[b][1], hi.x, lo.x);
-          split_pair(v[b][2], v[b][3], hi.y, lo.y);
-          split_pair(v[b][4], v[b][5], hi.z, lo.z);
-          split_pair(v[b][6], v[b][7], hi.w, lo.w);
-          unsigned char* dst = a_st + (kc * E + e) * 16;
-          *reinterpret_cast<uint4*>(dst) = hi;
-          *reinterpret_cast<uint4*>(dst + sm.a_lo) = lo;
+          if constexpr (P == 1) {
+            *reinterpret_cast<uint4*>(a_st + (kc * E + e) * 16) = make_uint4(
+                bf16_pair(v[b][0], v[b][1]), bf16_pair(v[b][2], v[b][3]), bf16_pair(v[b][4], v[b][5]), bf16_pair(v[b][6], v[b][7]));
+          } else {
+            uint4 hi, lo;
+            split_pair(v[b][0], v[b][1], hi.x, lo.x);
+            split_pair(v[b][2], v[b][3], hi.y, lo.y);
+            split_pair(v[b][4], v[b][5], hi.z, lo.z);
+            split_pair(v[b][6], v[b][7], hi.w, lo.w);
+            unsigned char* dst = a_st + (kc * E + e) * 16;
+            *reinterpret_cast<uint4*>(dst) = hi;
+            *reinterpret_cast<uint4*>(dst + sm.a_lo) = lo;
+          }
         }
       }
       if (kb == nb - 1) {
@@ -778,7 +828,8 @@ int conv3x3_wgmma_pack(const float* weight, unsigned char* packed, int Cin, int 
 }
 
 // Split-K second pass over the split region (samples n_lo.., rows y_lo..): out = act(sum_p parts[p] + bias), NCHW (with
-// the linear prefix) or depth-to-space.
+// the linear prefix) or depth-to-space.  TERMS as in the main kernel: split outputs have 2 / TERMS planes.
+template <int TERMS>
 __global__ void conv3x3_wgmma_reduce_kernel(um::SplitK sk, um::SplitDev xs, int RN, const float* __restrict__ bias,
                                             float* __restrict__ out, long long out_bs, int Cout, int OH, int OW, float slope,
                                             int out_mode_arg) {
@@ -794,7 +845,7 @@ __global__ void conv3x3_wgmma_reduce_kernel(um::SplitK sk, um::SplitDev xs, int 
       const float b = bias ? __ldg(bias + f) : 0.f;
       const float v = leaky(s + b, f < lin_prefix ? 1.f : slope);
       if (xs.out != nullptr && f >= lin_prefix)
-        sa::put_one(xs.out, xs.out_Cg, (long long)OH * OW, n, xs.out_c0 + f - lin_prefix, (long long)y * OW + x, v);
+        sa::put_one<TERMS == 1 ? 1 : 2>(xs.out, xs.out_Cg, (long long)OH * OW, n, xs.out_c0 + f - lin_prefix, (long long)y * OW + x, v);
       else
         out[(size_t)n * out_bs + ((size_t)f * OH + y) * OW + x] = v;
     } else {
@@ -862,6 +913,8 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
                          long long out_bs, int N, int Cin, int H, int W, int Cout, int stride, int dil, int out_mode,
                          float slope, cudaStream_t st, int ext, float* ws, long long ws_bytes, const SplitIO& sio) {
   using namespace um;
+  const int terms = (out_mode & MFN_CONV_BF16) ? 1 : 3;   // products per multiply-add; split operands have 2 / 1 planes
+  out_mode &= ~MFN_CONV_BF16;
   SplitDev xs = {0, 0, 0, nullptr, 0, 0};
   CUtensorMap tmx;
   memset(&tmx, 0, sizeof tmx);
@@ -871,7 +924,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
     EncodeTiledFn fn = encode_tiled_fn();
     if (fn == nullptr) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
     const int Cg = sa::groups(sio.in_C);
-    const cuuint64_t dim[4] = {8, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N * 2 * Cg};
+    const cuuint64_t dim[4] = {8, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N * (terms == 1 ? 1 : 2) * Cg};
     const cuuint64_t strides[3] = {16, (cuuint64_t)W * 16, (cuuint64_t)W * H * 16};
     const cuuint32_t box[4] = {8, (cuuint32_t)row_pitch(1, dil), (cuuint32_t)(dil < R ? n_slots(1, dil) : R), dil < R ? 2u : 1u};
     const cuuint32_t es[4] = {1, 1, 1, 1};
@@ -905,20 +958,30 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   // (split output: every row segment is 16-byte aligned; the register epilogue takes the linear prefix)
   const bool staged = (out_mode & 0xff) == 0 && ext == 0 &&
                       (xs.out != nullptr ? (out_mode >> 8) == 0 : OW % 4 == 0 && out_bs % 4 == 0 && aligned(out, 16)) &&
-                      smem_map(E, CoutP, as_wide, STG_BYTES).WS >= 2;
-  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0);
+                      smem_map(E, CoutP, as_wide, STG_BYTES, terms).WS >= 2;
+  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms);
   if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
   if ((long long)H * W >= (1LL << 27)) return -1;   // the producers address a 16-plane chunk with 32-bit element offsets
-  static SmemOptIn opt[8];
-  {
-    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9>, sm.total, opt[0]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 9>, sm.total, opt[1]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, true, 3>, sm.total, opt[2]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, true, 3>, sm.total, opt[3]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1>, sm.total, opt[4]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1>, sm.total, opt[5]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1>, sm.total, opt[6]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1>, sm.total, opt[7]);
+  static SmemOptIn opt[8], opt1[8];
+  if (terms == 3) {
+    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9, 3>, sm.total, opt[0]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 9, 3>, sm.total, opt[1]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, true, 3, 3>, sm.total, opt[2]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, true, 3, 3>, sm.total, opt[3]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1, 3>, sm.total, opt[4]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1, 3>, sm.total, opt[5]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1, 3>, sm.total, opt[6]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1, 3>, sm.total, opt[7]);
+    if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(conv3x3_wgmma_kernel): %s", cudaGetErrorString(e));
+  } else {
+    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<16, true, 9, 1>, sm.total, opt1[0]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9, 1>, sm.total, opt1[1]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<48, true, 3, 1>, sm.total, opt1[2]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 3, 1>, sm.total, opt1[3]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1, 1>, sm.total, opt1[4]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1, 1>, sm.total, opt1[5]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1, 1>, sm.total, opt1[6]);
+    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1, 1>, sm.total, opt1[7]);
     if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(conv3x3_wgmma_kernel): %s", cudaGetErrorString(e));
   }
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;
@@ -947,23 +1010,38 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const long long numWork = (sk.from + (tiles - sk.from) * sk.k) * ns;
   const int cap = tuning().conv_grid_cap > 0 ? tuning().conv_grid_cap : kNumSMs;
   const unsigned grid = (unsigned)(numWork < cap ? numWork : cap);
-#define MFN_WGMMA_LAUNCH(NW_, FOLD_, TPS_)                                                                                   \
-  conv3x3_wgmma_kernel<NW_, FOLD_, TPS_><<<grid, NTHREADS, sm.total, st>>>(x, x_bs, wpack, bias, out, out_bs, Cin, H, W, OH, \
-                                                                           OW, Cout, CoutP, nChunks, slope, tilesX, tilesY,  \
-                                                                           (int)numWork, stride, dil, out_mode, ext, sk, xs, \
-                                                                           tmx, tuning().conv_dbg)
-  // variant name (last_kernel): the padded output width, and whether the hi / lo weight images are folded
+#define MFN_WGMMA_LAUNCH(NW_, FOLD_, TPS_, TERMS_)                                                                      \
+  conv3x3_wgmma_kernel<NW_, FOLD_, TPS_, TERMS_><<<grid, NTHREADS, sm.total, st>>>(                                    \
+      x, x_bs, wpack, bias, out, out_bs, Cin, H, W, OH, OW, Cout, CoutP, nChunks, slope, tilesX, tilesY, (int)numWork, \
+      stride, dil, out_mode, ext, sk, xs, tmx, tuning().conv_dbg)
+  // variant name (last_kernel): the padded output width, whether the hi / lo weight images are folded, and bf16 for the
+  // one-product variant (whose accumulator is CoutP wide in every layout)
   const char* name = "conv3x3_wgmma_kernel<CoutP=256>";
-  switch (CoutP) {
-    case 16: MFN_WGMMA_LAUNCH(32, true, 9); name = "conv3x3_wgmma_kernel<CoutP=16,fold>"; break;
-    case 32: MFN_WGMMA_LAUNCH(64, true, 9); name = "conv3x3_wgmma_kernel<CoutP=32,fold>"; break;
-    case 48: MFN_WGMMA_LAUNCH(96, true, 3); name = "conv3x3_wgmma_kernel<CoutP=48,fold>"; break;
-    case 64: MFN_WGMMA_LAUNCH(128, true, 3); name = "conv3x3_wgmma_kernel<CoutP=64,fold>"; break;
-    case 80: MFN_WGMMA_LAUNCH(80, false, 1); name = "conv3x3_wgmma_kernel<CoutP=80>"; break;
-    case 96: MFN_WGMMA_LAUNCH(96, false, 1); name = "conv3x3_wgmma_kernel<CoutP=96>"; break;
-    case 112: MFN_WGMMA_LAUNCH(112, false, 1); name = "conv3x3_wgmma_kernel<CoutP=112>"; break;
-    case 128: MFN_WGMMA_LAUNCH(128, false, 1); name = "conv3x3_wgmma_kernel<CoutP=128>"; break;
-    default: MFN_WGMMA_LAUNCH(128, false, 1);   // 256: two 128-channel halves per tile
+  if (terms == 3) {
+    switch (CoutP) {
+      case 16: MFN_WGMMA_LAUNCH(32, true, 9, 3); name = "conv3x3_wgmma_kernel<CoutP=16,fold>"; break;
+      case 32: MFN_WGMMA_LAUNCH(64, true, 9, 3); name = "conv3x3_wgmma_kernel<CoutP=32,fold>"; break;
+      case 48: MFN_WGMMA_LAUNCH(96, true, 3, 3); name = "conv3x3_wgmma_kernel<CoutP=48,fold>"; break;
+      case 64: MFN_WGMMA_LAUNCH(128, true, 3, 3); name = "conv3x3_wgmma_kernel<CoutP=64,fold>"; break;
+      case 80: MFN_WGMMA_LAUNCH(80, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=80>"; break;
+      case 96: MFN_WGMMA_LAUNCH(96, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=96>"; break;
+      case 112: MFN_WGMMA_LAUNCH(112, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=112>"; break;
+      case 128: MFN_WGMMA_LAUNCH(128, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=128>"; break;
+      default: MFN_WGMMA_LAUNCH(128, false, 1, 3);   // 256: two 128-channel halves per tile
+    }
+  } else {
+    name = "conv3x3_wgmma_kernel<CoutP=256,bf16>";
+    switch (CoutP) {
+      case 16: MFN_WGMMA_LAUNCH(16, true, 9, 1); name = "conv3x3_wgmma_kernel<CoutP=16,fold,bf16>"; break;
+      case 32: MFN_WGMMA_LAUNCH(32, true, 9, 1); name = "conv3x3_wgmma_kernel<CoutP=32,fold,bf16>"; break;
+      case 48: MFN_WGMMA_LAUNCH(48, true, 3, 1); name = "conv3x3_wgmma_kernel<CoutP=48,fold,bf16>"; break;
+      case 64: MFN_WGMMA_LAUNCH(64, true, 3, 1); name = "conv3x3_wgmma_kernel<CoutP=64,fold,bf16>"; break;
+      case 80: MFN_WGMMA_LAUNCH(80, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=80,bf16>"; break;
+      case 96: MFN_WGMMA_LAUNCH(96, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=96,bf16>"; break;
+      case 112: MFN_WGMMA_LAUNCH(112, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=112,bf16>"; break;
+      case 128: MFN_WGMMA_LAUNCH(128, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=128,bf16>"; break;
+      default: MFN_WGMMA_LAUNCH(128, false, 1, 1);
+    }
   }
 #undef MFN_WGMMA_LAUNCH
   const int rc = check_launch(name);
@@ -971,8 +1049,12 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const long long total = sk.part_stride;
   long long blocks = (total + 255) / 256;
   if (blocks > 4 * kNumSMs) blocks = 4 * kNumSMs;
-  conv3x3_wgmma_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(sk, xs, N - sk.n_lo, bias, out, out_bs, Cout, OH, OW, slope, out_mode);
-  return check_launch("conv3x3_wgmma_reduce_kernel");
+  if (terms == 3) {
+    conv3x3_wgmma_reduce_kernel<3><<<(unsigned)blocks, 256, 0, st>>>(sk, xs, N - sk.n_lo, bias, out, out_bs, Cout, OH, OW, slope, out_mode);
+    return check_launch("conv3x3_wgmma_reduce_kernel");
+  }
+  conv3x3_wgmma_reduce_kernel<1><<<(unsigned)blocks, 256, 0, st>>>(sk, xs, N - sk.n_lo, bias, out, out_bs, Cout, OH, OW, slope, out_mode);
+  return check_launch("conv3x3_wgmma_reduce_kernel<bf16>");
 }
 
 }  // namespace mfn

@@ -35,6 +35,7 @@ PYRAMID_CH = {1: 16, 2: 32, 3: 64, 4: 96, 5: 128, 6: 196}   # network/MaskFlowne
 DECODER_CH = (128, 128, 96, 64, 32)                           # convL_0 .. convL_4 (:102-130)
 STRIDES = {6: 64, 5: 32, 4: 16, 3: 8, 2: 4}                   # self.strides (:71)
 SLOPE = 0.1
+PRECISIONS = ("fp32", "bf16")                                 # _FlowNetBase.inference_precision
 
 
 def _conv(cin, cout, k=3, s=1, p=1, d=1):
@@ -90,6 +91,26 @@ class _FlowNetBase(nn.Module):
     # False: cuDNN both ways.
     train_tc_forward = True
 
+    @property
+    def inference_precision(self) -> str:
+        """Arithmetic of the inference forward's 3x3 convolutions: "fp32" (default: the fp32-accurate bf16 hi/lo split)
+        or "bf16" (opt-in: one bf16 product per multiply-add, fp32 accumulation, and the dense blocks' and context
+        network's activations stored as bf16 -- ops.conv3x3_slices(bf16=True), include/maskflow_b200.h MFN_CONV_BF16).
+        Correlation, warps, sampling and pre/post-processing stay fp32-accurate; training (autograd recording) is not
+        affected.  Setting it on the cascade also sets it on its MaskFlownet_S head."""
+        return self.__dict__.get("_inference_precision", "fp32")
+
+    @inference_precision.setter
+    def inference_precision(self, value: str) -> None:
+        if value not in PRECISIONS:
+            raise ops.MaskflowError(f"inference_precision must be one of {PRECISIONS}, got {value!r}")
+        for m in self.modules():
+            if isinstance(m, _FlowNetBase):
+                m.__dict__["_inference_precision"] = value
+
+    def _bf16(self) -> bool:
+        return self.inference_precision == "bf16"
+
     def _packed(self, name):
         """Packed split-bf16 weight image of conv `name`, rebuilt when the parameter changes."""
         cache = self.__dict__.setdefault("_pack_cache", {})
@@ -135,7 +156,7 @@ class _FlowNetBase(nn.Module):
                 return ops.conv3x3_pack(w), b
             packed, b = self._packed_fn(f"heads_tail{lvl}", [p for c in convs for p in (c.weight, c.bias)], build_tail)
             y = torch.empty((N, nh, H, W), device=dev, dtype=torch.float32)
-            ops.conv3x3_split(x.act, 0, oc, packed, b, nh, 1.0, out=y)
+            ops.conv3x3_split(x.act, 0, oc, packed, b, nh, 1.0, out=y, bf16=self._bf16())
             y += x.prefix[:, :nh]
         else:
             def build():
@@ -144,7 +165,7 @@ class _FlowNetBase(nn.Module):
                 return ops.conv3x3_pack(w), b
             packed, b = self._packed_fn(f"heads{lvl}", [p for c in convs for p in (c.weight, c.bias)], build)
             y = torch.empty((N, nh, H, W), device=dev, dtype=torch.float32)
-            ops.conv3x3_split(x.act, 0, x.channels, packed, b, nh, 1.0, out=y)
+            ops.conv3x3_split(x.act, 0, x.channels, packed, b, nh, 1.0, out=y, bf16=self._bf16())
         if pm is None:
             return y, None
         return y[:, :2].contiguous(), y[:, 2:3].contiguous()
@@ -159,7 +180,8 @@ class _FlowNetBase(nn.Module):
         N, _, H, W = x.act.shape
         F = up.out_channels
         out = torch.empty((N, F, 2 * H, 2 * W), device=x.act.buf.device, dtype=torch.float32)
-        ops.conv3x3_split(x.act, 0, x.channels, packed, up.bias, 4 * F, SLOPE, out=out, depth_to_space=True)
+        ops.conv3x3_split(x.act, 0, x.channels, packed, up.bias, 4 * F, SLOPE, out=out, depth_to_space=True,
+                          bf16=self._bf16())
         return out
 
     def _plain(self, name, x):
@@ -167,7 +189,7 @@ class _FlowNetBase(nn.Module):
         conv = getattr(self, name)
         if not self._fast(x):
             return self._conv_act(name, x, 1.0)
-        return ops.conv3x3(x, self._packed(name), conv.bias, conv.out_channels, 1.0, conv.dilation[0])
+        return ops.conv3x3(x, self._packed(name), conv.bias, conv.out_channels, 1.0, conv.dilation[0], bf16=self._bf16())
 
     def _conv_act(self, name, x, slope):
         """Autograd path of one 3x3 convolution (+ LeakyReLU when slope != 1): torch.nn.functional (cuDNN both ways), or --
@@ -192,7 +214,8 @@ class _FlowNetBase(nn.Module):
                 name = f"conv{lvl}{sfx}"
                 conv = getattr(self, name)
                 if fast:
-                    x = ops.conv3x3(x, self._packed(name), conv.bias, conv.out_channels, SLOPE, 1, 2 if j == 0 else 1)
+                    x = ops.conv3x3(x, self._packed(name), conv.bias, conv.out_channels, SLOPE, 1, 2 if j == 0 else 1,
+                                    bf16=self._bf16())
                 else:
                     x = self._conv_act(name, x, SLOPE)
             feats.append(x)
@@ -224,7 +247,8 @@ class _FlowNetBase(nn.Module):
         would round them) -- one pass over the ~550-channel input instead of two.  Returns the block output as a _Slab."""
         N, Cb, H, W = base.shape
         front = sum(DECODER_CH)
-        act = ops.SplitAct(N, front + Cb, H, W, base.device)
+        bf16 = self._bf16()
+        act = ops.SplitAct(N, front + Cb, H, W, base.device, bf16=bf16)
         act.pack(base, front)
         nh = (2 + (1 if hasattr(self, f"pred_mask{lvl}") else 0)) if self.fuse_heads else 0
         lp = nh + nh % 2   # the kernel writes split channels in pairs: an even prefix
@@ -245,10 +269,10 @@ class _FlowNetBase(nn.Module):
                 packed, b = self._packed_fn(f"conv{lvl}_4+heads", [conv.weight, conv.bias] + [h.weight for h in heads], build)
                 prefix = torch.empty((N, lp, H, W), device=base.device, dtype=torch.float32)
                 ops.conv3x3_split(act, off, act.channels - off, packed, b, lp + oc, SLOPE, out=prefix, out_split=act,
-                                  out_c0=off - oc, linear_prefix=lp)
+                                  out_c0=off - oc, linear_prefix=lp, bf16=bf16)
             else:
                 ops.conv3x3_split(act, off, act.channels - off, self._packed(f"conv{lvl}_{i}"), conv.bias, oc, SLOPE,
-                                  out_split=act, out_c0=off - oc)
+                                  out_split=act, out_c0=off - oc, bf16=bf16)
             off -= oc
         return _Slab(act, prefix, DECODER_CH[-1] if nh else 0)
 
@@ -258,16 +282,17 @@ class _FlowNetBase(nn.Module):
             # writes the fp32 flow
             act = x.act
             N, _, H, W = act.shape
+            bf16 = self._bf16()
             for i in range(1, 8):
                 conv = getattr(self, f"dc_conv{i}")
                 if i == 7:
                     y = torch.empty((N, conv.out_channels, H, W), device=act.buf.device, dtype=torch.float32)
                     ops.conv3x3_split(act, 0, act.channels, self._packed("dc_conv7"), conv.bias, conv.out_channels, 1.0,
-                                      conv.dilation[0], out=y)
+                                      conv.dilation[0], out=y, bf16=bf16)
                     return y
-                nxt = ops.SplitAct(N, conv.out_channels, H, W, act.buf.device)
+                nxt = ops.SplitAct(N, conv.out_channels, H, W, act.buf.device, bf16=bf16)
                 ops.conv3x3_split(act, 0, act.channels, self._packed(f"dc_conv{i}"), conv.bias, conv.out_channels, SLOPE,
-                                  conv.dilation[0], out_split=nxt)
+                                  conv.dilation[0], out_split=nxt, bf16=bf16)
                 act = nxt
         for i in range(1, 7):
             x = self._conv_act(f"dc_conv{i}", x, SLOPE)
@@ -481,9 +506,16 @@ def predict(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, resize=None)
     return flow, mask
 
 
+def precision_key(net: nn.Module) -> Tuple[str, ...]:
+    """The inference_precision of every flow network inside `net` (the cascade's head may be set on its own): what a
+    captured graph depends on besides the input shape."""
+    return tuple(m.inference_precision for m in net.modules() if isinstance(m, _FlowNetBase))
+
+
 class FlowPredictor:
-    """predict_flow captured in a CUDA graph: one graph per input shape, static uint8 input buffers, one cudaGraphLaunch
-    per call (the eager step is ~115 dependent launches; the graph removes the launch gaps between them).
+    """predict_flow captured in a CUDA graph: one graph per input shape (and precision_key of the model), static uint8
+    input buffers, one cudaGraphLaunch per call (the eager step is ~115 dependent launches; the graph removes the launch
+    gaps between them).  After a precision switch the next call captures (or reuses) a graph of the new precision.
     Weights are read through the packed images cached in the model: call invalidate() after changing parameters.
     The returned tensor is the graph's STATIC output buffer: the next call overwrites it -- clone() it (or copy it to the
     host) before calling again if the previous result is still needed."""
@@ -497,7 +529,7 @@ class FlowPredictor:
     @torch.no_grad()
     def __call__(self, img1_u8: torch.Tensor, img2_u8: torch.Tensor) -> torch.Tensor:
         dev = next(self.net.parameters()).device      # inputs may live on the host (pinned): the static buffers do not
-        key = (tuple(img1_u8.shape), img1_u8.dtype)
+        key = (tuple(img1_u8.shape), img1_u8.dtype, precision_key(self.net))
         entry = self._graphs.get(key)
         if entry is None:
             in1 = torch.empty(img1_u8.shape, dtype=img1_u8.dtype, device=dev)

@@ -532,14 +532,23 @@ def conv3x3_pack(weight: torch.Tensor) -> torch.Tensor:
     return packed
 
 
+MFN_CONV_BF16 = 0x10   # include/maskflow_b200.h
+
+
+def _out_mode(depth_to_space: bool, linear_prefix: int, bf16: bool) -> int:
+    return (1 if depth_to_space else 0) | (int(linear_prefix) << 8) | (MFN_CONV_BF16 if bf16 else 0)
+
+
 def conv3x3_slices(buf_in: torch.Tensor, c_in0: int, Cin: int, packed: torch.Tensor, bias: Optional[torch.Tensor],
                    buf_out: torch.Tensor, c_out0: int, Cout: int, leaky_slope: float = 0.1, dilation: int = 1,
-                   stride: int = 1, depth_to_space: bool = False, linear_prefix: int = 0) -> None:
+                   stride: int = 1, depth_to_space: bool = False, linear_prefix: int = 0, bf16: bool = False) -> None:
     """out = LeakyReLU(conv3x3(buf_in[:, c_in0:c_in0+Cin]) + bias) written to buf_out[:, c_out0:c_out0+Cout]; both buffers
     dense NCHW (they may be the same tensor: the dense block's concat buffer).  stride 2 (pad 1) = the pyramid's
     down-sampling convolutions: buf_out is then ((H-1)//2+1, (W-1)//2+1).  depth_to_space: the Cout = 4F conv channels
     are written as F channels of a (2H, 2W) image (sub-pixel phases; see conv_transpose4x4_pack).  linear_prefix: the first
-    k output channels skip the activation (MFN_CONV_OUT_LINEAR_PREFIX).  Inference only."""
+    k output channels skip the activation (MFN_CONV_OUT_LINEAR_PREFIX).  bf16: one bf16 product per multiply-add
+    (MFN_CONV_BF16: input and weights rounded once to bf16, fp32 accumulation) instead of the fp32-accurate split; the
+    output stays fp32.  Inference only."""
     for t, nm in ((buf_in, "buf_in"), (buf_out, "buf_out")):
         if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 4):
             raise MaskflowError(f"conv3x3_slices: {nm} must be a contiguous CUDA float32 NCHW tensor")
@@ -563,18 +572,23 @@ def conv3x3_slices(buf_in: torch.Tensor, c_in0: int, Cin: int, packed: torch.Ten
     ws_bytes = int(_lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, int(stride), int(dilation)))
     ws = torch.empty(ws_bytes // 4, device=buf_in.device, dtype=torch.float32) if ws_bytes else None
     _call("mfn_conv3x3_forward_ws", buf_in.device, xin, Cti * H * W, _p(packed), _p(b), xout, Cto * OH * OW, N, Cin, H, W,
-          Cout, int(stride), int(dilation), (1 if depth_to_space else 0) | (int(linear_prefix) << 8), float(leaky_slope),
-          _p(ws), ws_bytes)
+          Cout, int(stride), int(dilation), _out_mode(depth_to_space, linear_prefix, bf16), float(leaky_slope), _p(ws),
+          ws_bytes)
 
 
 class SplitAct:
     """An activation of `channels` channels in the split format the convolutions read with tensor copies
     (include/maskflow_b200.h, mfn_split_pack): per sample, the bf16 hi images of ceil(C/16)*2 groups of 8 channels, then
-    their lo images, 16 bytes per (group, pixel); pad channels are zero.  Writers: pack() and conv3x3_split()."""
+    their lo images, 16 bytes per (group, pixel); pad channels are zero.  bf16=True: a bf16 activation (mfn_bf16_pack),
+    the hi images alone -- every value rounded once to bf16 -- read and written by the convolutions' bf16 mode.
+    Writers: pack() and conv3x3_split()."""
+    bf16 = False
 
-    def __init__(self, N: int, channels: int, H: int, W: int, device):
+    def __init__(self, N: int, channels: int, H: int, W: int, device, bf16: bool = False):
         self.channels = int(channels)
-        self.buf = torch.empty((N, 2, (self.channels + 15) // 16 * 2, H, W, 16), dtype=torch.uint8, device=device)
+        self.bf16 = bool(bf16)
+        self.buf = torch.empty((N, 1 if self.bf16 else 2, (self.channels + 15) // 16 * 2, H, W, 16), dtype=torch.uint8,
+                               device=device)
 
     @property
     def shape(self):
@@ -587,23 +601,30 @@ class SplitAct:
         N, C, H, W = s.shape
         if (N, H, W) != (self.shape[0], self.shape[2], self.shape[3]):
             raise MaskflowError("SplitAct.pack: src disagrees in N/H/W")
-        _call("mfn_split_pack", s.device, _p(s), C * H * W, N, C, H, W, _p(self.buf), self.channels, int(c0))
+        _call("mfn_bf16_pack" if self.bf16 else "mfn_split_pack", s.device, _p(s), C * H * W, N, C, H, W, _p(self.buf),
+              self.channels, int(c0))
 
     def hi_lo(self):
-        """(hi, lo) as fp32 (N, C, H, W) tensors: the two bf16 terms of every value."""
+        """(hi, lo) as fp32 (N, C, H, W) tensors: the two bf16 terms of every value (lo = zeros for a bf16 activation)."""
         N, C, H, W = self.shape
-        t = self.buf.view(torch.bfloat16).view(N, 2, -1, H, W, 8).permute(0, 1, 2, 5, 3, 4).reshape(N, 2, -1, H, W)
-        return t[:, 0, :C].float(), t[:, 1, :C].float()
+        P = self.buf.shape[1]
+        t = self.buf.view(torch.bfloat16).view(N, P, -1, H, W, 8).permute(0, 1, 2, 5, 3, 4).reshape(N, P, -1, H, W)
+        hi = t[:, 0, :C].float()
+        return hi, (t[:, 1, :C].float() if P == 2 else torch.zeros_like(hi))
 
 
 def conv3x3_split(x: SplitAct, c_in0: int, Cin: int, packed: torch.Tensor, bias: Optional[torch.Tensor], Cout: int,
                   leaky_slope: float = 0.1, dilation: int = 1, out: Optional[torch.Tensor] = None,
                   out_split: Optional[SplitAct] = None, out_c0: int = 0, depth_to_space: bool = False,
-                  linear_prefix: int = 0) -> None:
+                  linear_prefix: int = 0, bf16: bool = False) -> None:
     """conv3x3_slices reading channels [c_in0, c_in0 + Cin) of a split activation (c_in0 a multiple of 16).  Output: the
     fp32 NCHW (or depth-to-space) tensor `out`, or -- out_split given -- channels out_c0.. of that split activation, the
     linear_prefix channels (even) going to the fp32 (N, linear_prefix, H, W) `out`.  Bit-identical to conv3x3_slices on
-    the same values.  Inference only."""
+    the same values.  bf16: the bf16 mode (see conv3x3_slices); x and out_split must then be bf16 activations
+    (SplitAct(..., bf16=True)), and must not be otherwise.  Inference only."""
+    for a, nm in ((x, "x"), (out_split, "out_split")):
+        if a is not None and a.bf16 != bool(bf16):
+            raise MaskflowError(f"conv3x3_split: {nm} is a {'bf16' if a.bf16 else 'split'} activation but bf16={bool(bf16)}")
     N, Cx, H, W = x.shape
     if not (0 <= c_in0 and c_in0 + Cin <= Cx):
         raise MaskflowError("conv3x3_split: channel slice out of range")
@@ -626,7 +647,7 @@ def conv3x3_split(x: SplitAct, c_in0: int, Cin: int, packed: torch.Tensor, bias:
     ws = torch.empty(ws_bytes // 4, device=x.buf.device, dtype=torch.float32) if ws_bytes else None
     _call("mfn_conv3x3_forward_split", x.buf.device, _p(x.buf), Cx, int(c_in0), _p(packed), _p(b), _p(out), 0,
           _p(out_split.buf if out_split is not None else None), out_split.channels if out_split is not None else 0,
-          int(out_c0), N, Cin, H, W, Cout, int(dilation), (1 if depth_to_space else 0) | (int(linear_prefix) << 8),
+          int(out_c0), N, Cin, H, W, Cout, int(dilation), _out_mode(depth_to_space, linear_prefix, bf16),
           float(leaky_slope), _p(ws), ws_bytes)
 
 
@@ -657,12 +678,13 @@ def conv_transpose4x4_pack(weight: torch.Tensor) -> torch.Tensor:
 
 
 def conv3x3(x: torch.Tensor, packed: torch.Tensor, bias: Optional[torch.Tensor], Cout: int, leaky_slope: float = 0.1,
-            dilation: int = 1, stride: int = 1):
-    """3x3 convolution, padding = dilation, stride 1 (decoder / context network) or 2 (pyramid), + LeakyReLU."""
+            dilation: int = 1, stride: int = 1, bf16: bool = False):
+    """3x3 convolution, padding = dilation, stride 1 (decoder / context network) or 2 (pyramid), + LeakyReLU.  bf16: the
+    bf16 mode of conv3x3_slices."""
     x = _chk(x, "conv3x3.x")
     out = torch.empty((x.shape[0], Cout, (x.shape[2] - 1) // stride + 1, (x.shape[3] - 1) // stride + 1), device=x.device,
                       dtype=torch.float32)
-    conv3x3_slices(x, 0, x.shape[1], packed, bias, out, 0, Cout, leaky_slope, dilation, stride)
+    conv3x3_slices(x, 0, x.shape[1], packed, bias, out, 0, Cout, leaky_slope, dilation, stride, bf16=bf16)
     return out
 
 

@@ -45,12 +45,17 @@ class PipelineFlownet:
     torch.use_deterministic_algorithms(True) (restored afterwards), so this library's ops take their *_det kernels and torch
     picks deterministic cuDNN algorithms.  torch.backends.cudnn.benchmark must stay off (it may pick a different algorithm
     per run; the pipeline raises if it is on), and the process must be started with CUBLAS_WORKSPACE_CONFIG=:4096:8 (or
-    :16:8) in the environment, which torch requires for deterministic cuBLAS calls."""
+    :16:8) in the environment, which torch requires for deterministic cuBLAS calls.
+    precision: the network's inference_precision ("fp32" or the opt-in "bf16") for do_batch_mx, do_batch, validate and
+    predict; train_batch always trains with fp32-accurate arithmetic."""
     _lr = None
 
     def __init__(self, device=None, network_class: str = "MaskFlownet_S", lr_schedule: Optional[Sequence[Tuple[int, float]]] = None,
                  multiscale_weights: Sequence[float] = losses.WEIGHTS, q: Optional[float] = None, learning_rate: float = 1e-4,
-                 deterministic: bool = False):
+                 deterministic: bool = False, precision: str = "fp32"):
+        if precision not in network.PRECISIONS:
+            raise MaskflowError(f"PipelineFlownet: precision must be one of {network.PRECISIONS}, got {precision!r}")
+        self.precision = precision
         self.deterministic = bool(deterministic)
         self._check_deterministic_settings()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -58,6 +63,8 @@ class PipelineFlownet:
         if cls is None:
             raise MaskflowError(f"PipelineFlownet: unknown network class {network_class!r} (MaskFlownet_S | MaskFlownet)")
         self.network = cls().to(self.device)                       # MSRAPrelu(slope=0.1) initialisation (pipeline.py:26)
+        if precision != "fp32":
+            self.network.inference_precision = precision
         self.trainer = torch.optim.Adam(self.network.parameters(), lr=learning_rate)      # gluon.Trainer 'adam' 1e-4 (:27)
         self._lr = learning_rate
         self.strides = list(STRIDES)
@@ -185,6 +192,8 @@ class PipelineFlownet:
     def do_batch_mx(self, img1, img2, resize=None):
         """img1 / img2 in [0,1] float32 (or uint8): centralize, resize to multiples of 64 (or `resize`), network."""
         H, W = img1.shape[2:]
+        if getattr(self.network, "inference_precision", "fp32") != self.precision:
+            self.network.inference_precision = self.precision
         with self._determinism():
             a, b, _ = ops.preprocess(img1.contiguous(), img2.contiguous(), ops.padded_size(H, W, resize))
             return self.network(a, b)

@@ -20,7 +20,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import network, ops
 from ._lib import MaskflowError
 
 _WARMUP = 2
@@ -35,7 +35,7 @@ class VideoFlowPredictor:
     partial batch repeats the last frame in its unused slots and yields only its real pairs.  resize: the network input
     size (H', W'), default the next multiples of 64.  max_radius / bgr: as ops.flow_to_color; a fixed max_radius keeps the
     colours of successive frames comparable.  Weights are read through the packed images cached in the model: call
-    invalidate() after changing parameters."""
+    invalidate() after changing parameters.  Graphs are kept per frame size and network.precision_key of the model."""
 
     def __init__(self, net: nn.Module, batch: int = 8, resize=None, max_radius=None, bgr: bool = False,
                  want_flow: bool = False, depth: int = 2):
@@ -62,7 +62,8 @@ class VideoFlowPredictor:
         return rgb, flow
 
     def _state(self, H: int, W: int, dev: torch.device):
-        st = self._states.get((H, W))
+        key = (H, W, network.precision_key(self.net))
+        st = self._states.get(key)
         if st is not None:
             return st
         B = self.batch
@@ -88,7 +89,7 @@ class VideoFlowPredictor:
                 s["flow"] = torch.empty_like(flow)
                 s["flow_host"] = torch.empty(flow.shape, dtype=torch.float32, pin_memory=True)
             slots.append(s)
-        st = self._states[(H, W)] = {"graph": graph, "F": F, "rgb": rgb, "flow": flow, "slots": slots, "i": 0}
+        st = self._states[key] = {"graph": graph, "F": F, "rgb": rgb, "flow": flow, "slots": slots, "i": 0}
         return st
 
     # ---- one batch ---------------------------------------------------------------------------------------------

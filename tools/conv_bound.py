@@ -1,6 +1,7 @@
 """Where the time of the 3x3 / transposed convolutions goes, set against what the H100 can do.
 
     python tools/conv_bound.py [--batch 8] [--height 448] [--width 1024] [--reps 5] [--levels 2,3] [--json FILE]
+                               [--precision fp32|bf16]
 
 Runs one eager MaskFlownet-S forward (BASELINE configs[1]: batch 8, 1024x448, seeded inputs and weights) and records every
 convolution launch (ops.conv3x3_slices / ops.conv3x3_split) with the layer that issued it.  Each recorded launch is then replayed on its own,
@@ -20,7 +21,9 @@ Per launch the table prints the shape, the time, and two lower bounds:
            products per fp32 product, whole rounds of one work item per SM) at the 989 TFLOP/s dense-bf16 data-sheet rate
     hbm    input + output + packed weights once over the 3.35 TB/s data-sheet bandwidth
 
-and `frac` = max(mma, hbm) / time.  The four deltas (time minus the time without a phase) show what each phase adds to
+and `frac` = max(mma, hbm) / time.  --precision bf16 runs the forward in the opt-in bf16 mode (inference_precision):
+its launches issue one bf16 product per fp32 product, so the mma bound counts one (and the hbm bound reads bf16
+activations at 2 bytes per channel-pixel).  The four deltas (time minus the time without a phase) show what each phase adds to
 the critical path.  Both rates are for a 700 W part; a card with a lower power limit runs slower clocks.
 """
 from __future__ import annotations
@@ -49,15 +52,16 @@ def cout_pad(cin: int, cout: int) -> int:
     return (int(_lib.lib().mfn_conv3x3_packed_bytes(cin, cout)) - sync) // (((cin + 15) // 16) * 9 * 64)
 
 
-def mma_columns(cout_p: int) -> int:
+def mma_columns(cout_p: int, terms: int = 3) -> int:
     """Accumulator columns the MMAs of one 64-pixel block issue per tap and 16-channel chunk: three products over CoutP,
-    or -- folded narrow layers -- hi x [hi; lo] over 2 CoutP plus lo x hi over CoutP."""
+    or -- folded narrow layers -- hi x [hi; lo] over 2 CoutP plus lo x hi over CoutP; terms = 1 (bf16 mode): hi x hi over
+    CoutP."""
     if cout_p > 128:
-        return 2 * 3 * 128
-    return 3 * cout_p
+        return 2 * terms * 128
+    return terms * cout_p
 
 
-def bounds(c):
+def bounds(c, terms=3):
     N, Cin, H, W, Cout, stride, dil = c["N"], c["Cin"], c["H"], c["W"], c["Cout"], c["stride"], c["dil"]
     OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
     tiles = N * ((OW + MT - 1) // MT) * ((OH + R - 1) // R)
@@ -69,12 +73,14 @@ def bounds(c):
     ns = 2 if cp > 128 else 1
     items = tiles * k * ns
     rounds = -(-items // SMS)
-    per_item_flop = 2 * (2 * R * 64) * 16 * mma_columns(cp) // ns * 9 * (-(-chunks // k))
+    per_item_flop = 2 * (2 * R * 64) * 16 * mma_columns(cp, terms) // ns * 9 * (-(-chunks // k))
     mma = rounds * per_item_flop / (PEAK_FLOPS / SMS)
-    useful = 3 * 2 * N * OH * OW * Cout * Cin * 9 / PEAK_FLOPS
+    useful = terms * 2 * N * OH * OW * Cout * Cin * 9 / PEAK_FLOPS
     Fo = Cout // 4 if c["d2s"] else Cout
     out_px = N * OH * OW * (4 if c["d2s"] else 1)
-    nbytes = 4 * (N * Cin * H * W + Fo * out_px) + int(_lib.lib().mfn_conv3x3_packed_bytes(Cin, Cout))
+    ib = 2 if terms == 1 and "fn" in c else 4                                         # a bf16 activation in
+    ob = 2 if terms == 1 and "fn" in c and c["args"][9] is not None else 4            # a bf16 activation out
+    nbytes = ib * N * Cin * H * W + ob * Fo * out_px + int(_lib.lib().mfn_conv3x3_packed_bytes(Cin, Cout))
     return mma, nbytes / PEAK_BW, useful
 
 
@@ -86,13 +92,16 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--levels", default="", help="comma-separated levels to list per layer (default: all)")
     ap.add_argument("--json", default="", help="also write the rows as JSON to this file")
+    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32", help="the model's inference_precision")
     args = ap.parse_args()
+    terms = 1 if args.precision == "bf16" else 3
     if not torch.cuda.is_available():
         sys.exit("conv_bound.py times GPU kernels: no CUDA device")
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.manual_seed(0)
     model = network.MaskFlownetS().cuda().eval()
+    model.inference_precision = args.precision
     g = torch.Generator().manual_seed(0)
     a = torch.randint(0, 256, (args.batch, 3, args.height, args.width), dtype=torch.uint8, generator=g).cuda()
     b = torch.randint(0, 256, (args.batch, 3, args.height, args.width), dtype=torch.uint8, generator=g).cuda()
@@ -113,23 +122,23 @@ def main():
     orig_slices = ops.conv3x3_slices
 
     def slices(buf_in, c_in0, Cin, packed_w, bias, buf_out, c_out0, Cout, leaky_slope=0.1, dilation=1, stride=1,
-               depth_to_space=False, linear_prefix=0):
+               depth_to_space=False, linear_prefix=0, bf16=False):
         orig_slices(buf_in, c_in0, Cin, packed_w, bias, buf_out, c_out0, Cout, leaky_slope, dilation, stride, depth_to_space,
-                    linear_prefix)
+                    linear_prefix, bf16)
         if recording["on"]:
             N, _, H, W = buf_in.shape
             calls.append({"layer": current["name"], "N": N, "Cin": Cin, "H": H, "W": W, "Cout": Cout, "stride": stride,
                           "dil": dilation, "d2s": depth_to_space, "lin": linear_prefix,
                           "ws_bytes": int(_lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, stride, dilation)),
                           "args": (buf_in, c_in0, Cin, packed_w, bias, buf_out, c_out0, Cout, leaky_slope, dilation, stride,
-                                   depth_to_space, linear_prefix)})
+                                   depth_to_space, linear_prefix, bf16)})
 
     orig_split = ops.conv3x3_split
 
     def split(x, c_in0, Cin, packed_w, bias, Cout, leaky_slope=0.1, dilation=1, out=None, out_split=None, out_c0=0,
-              depth_to_space=False, linear_prefix=0):
+              depth_to_space=False, linear_prefix=0, bf16=False):
         args = (x, c_in0, Cin, packed_w, bias, Cout, leaky_slope, dilation, out, out_split, out_c0, depth_to_space,
-                linear_prefix)
+                linear_prefix, bf16)
         orig_split(*args)
         if recording["on"]:
             N, _, H, W = x.shape
@@ -177,8 +186,8 @@ def main():
         _lib.set_tuning("conv_dbg", 0)
 
     dev = torch.cuda.get_device_name()
-    print(f"# {dev}; eager forward {step:.3f} ms; {len(calls)} convolution launches; "
-          f"times in us (median of {args.reps}); bounds at 989 TFLOP/s bf16 and 3.35 TB/s")
+    print(f"# {dev}; {args.precision}; eager forward {step:.3f} ms; {len(calls)} convolution launches; "
+          f"times in us (median of {args.reps}); bounds at 989 TFLOP/s bf16 and 3.35 TB/s, {terms} product(s) per MAC")
     want = {int(x) for x in args.levels.split(",") if x.strip()}
     hdr = (f"{'layer':16s} {'N':>2s} {'Cin':>4s} {'Cout':>4s} {'H':>4s} {'W':>5s} s d {'time':>8s} {'mma':>8s} {'hbm':>7s} "
            f"{'frac':>5s} {'load':>7s} {'input':>7s} {'store':>7s} {'mma':>7s}")
@@ -186,7 +195,7 @@ def main():
     per_level = collections.OrderedDict()
     rows = []
     for c in calls:
-        mma, hbm, useful = bounds(c)
+        mma, hbm, useful = bounds(c, terms)
         t = c["full"] * 1e-3
         m = re.search(r"\d", c["layer"])
         lvl = 2 if c["layer"].startswith("dc_conv") else (int(m.group()) if m else 0)
@@ -218,7 +227,7 @@ def main():
           f"{tot[1] / tot[0]:5.2f} {tot[4] * 1e3:7.0f} {tot[5] * 1e3:7.0f} {tot[6] * 1e3:7.0f} {tot[7] * 1e3:7.0f}")
     if args.json:
         with open(args.json, "w") as f:
-            json.dump({"device": dev, "eager_forward_ms": step, "rows": rows}, f, indent=1)
+            json.dump({"device": dev, "precision": args.precision, "eager_forward_ms": step, "rows": rows}, f, indent=1)
 
 
 if __name__ == "__main__":

@@ -113,11 +113,14 @@ def main(argv=None):
     ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
     ap.add_argument("--max_radius", type=float, default=None,
                     help="fixed flow magnitude (pixels) of the colour wheel's rim; default: each frame's largest flow")
+    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
+                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
     a = ap.parse_args(argv)
     if a.video_filepath is None and (a.image_1 is None or a.image_2 is None):
         ap.error("give --image_1 and --image_2, or --video_filepath")
     resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
     model = load_model(a.network, a.checkpoint)
+    model.inference_precision = a.precision
     n = predict_files(model, a.flow_filepath, a.image_1, a.image_2, a.video_filepath, a.batch, resize, a.max_radius)
     print(f"wrote {n} image(s) to {a.flow_filepath}")
 

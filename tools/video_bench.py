@@ -77,6 +77,7 @@ def main():
     ap.add_argument("--frames", type=int, default=65)
     ap.add_argument("--host-frames", type=int, default=17)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32", help="the models' inference_precision")
     a = ap.parse_args()
     H, W = map(int, a.hw.split("x"))
     resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
@@ -84,10 +85,12 @@ def main():
     torch.backends.cuda.matmul.allow_tf32 = False
     rng = np.random.default_rng(a.seed)
     frames = rng.integers(0, 256, (a.frames, H, W, 3), dtype=np.uint8)
-    res = {"gpu": gpu_info(), "hw": [H, W], "resize": resize, "batch": a.batch, "video_fps": {}, "host_color_fps": {}}
+    res = {"gpu": gpu_info(), "hw": [H, W], "resize": resize, "batch": a.batch, "precision": a.precision, "video_fps": {},
+           "host_color_fps": {}}
     for name, cls in (("MaskFlownet_S", network.MaskFlownetS), ("MaskFlownet", network.MaskFlownet)):
         torch.manual_seed(a.seed)
         model = cls().cuda().eval()
+        model.inference_precision = a.precision
         res["video_fps"][name] = round(video_rate(VideoFlowPredictor(model, a.batch, resize), frames, False), 1)
         host = VideoFlowPredictor(model, a.batch, resize, want_flow=True)
         res["host_color_fps"][name] = round(video_rate(host, frames[:a.host_frames], True), 1)
