@@ -4,8 +4,9 @@
 // hi/lo split: three MMAs hi*lo + lo*hi + hi*hi per product); reference call sites network/MaskFlownet.py:147-300.
 //
 // Implicit GEMM without im2col:   D[pixel, f] = sum_{tap, c} X[pixel + tap offset, c] * Wt[tap][c][f]
-//   * a work tile is R = 2 image rows x 128 consecutive output pixels x (up to 128) output channels.  PERSISTENT kernel,
-//     one CTA per SM, tiles dealt round-robin; the producers / weight loader run ahead across tile boundaries.
+//   * a work tile is R = 2 image rows x MT consecutive output pixels x (up to 128) output channels; MT = 128, or 64 where
+//     the output is at most 64 pixels wide (levels 4-6).  PERSISTENT kernel, one CTA per SM, tiles dealt round-robin; the
+//     producers / weight loader run ahead across tile boundaries.
 //   * K is walked as (16-channel chunk) x (tap).  Per chunk the producer warps convert the input rows the nine taps touch
 //     from fp32 NCHW into split bf16 in the *no-swizzle K-major core-matrix layout*: plane [8-channel group][pixel] with
 //     16 bytes per entry.  In that layout a tap shift is nothing but a different start address (+16 bytes per pixel), so
@@ -13,8 +14,8 @@
 //     Stride 2 de-interleaves even / odd pixels so the same holds (see the geometry helpers).
 //   * weights are pre-packed (mfn_conv3x3_pack_weights) into per-(chunk, tap) images of the same layout and streamed by
 //     one thread with 1-D bulk copies (cp.async.bulk + mbarrier complete_tx) through a deep ring (up to 24 stages).
-//   * two consumer warpgroups, one per output row, each issue m64nNk16 MMAs (bf16 x bf16 -> fp32) for the two 64-pixel
-//     halves of their row; after each tap's group they wait for the previous group and release the weight / input
+//   * two consumer warpgroups, one per output row, each issue m64nNk16 MMAs (bf16 x bf16 -> fp32) for the MT / 64
+//     64-pixel blocks of their row; after each tap's group they wait for the previous group and release the weight / input
 //     stages it read, and at the end of a tile apply bias + LeakyReLU and store NCHW -- through shared-memory staging
 //     rows and asynchronous bulk copies when the output rows are 16-byte aligned, else from registers -- or, for the
 //     transposed convolutions, scatter 2x2 sub-pixel phases (depth-to-space).
@@ -23,13 +24,17 @@
 //     (MFN_CONV_BF16): only A_hi x B_hi, the input stage holds the hi plane alone, the weight ring streams the hi half of
 //     the same packed image, and split outputs are bf16 activations (one plane, split_act.cuh).
 #include <cstring>
+#include <type_traits>
 
 #include "mma_tiles.cuh"
 #include "split_act.cuh"
 
 namespace mfn {
 namespace um {
-constexpr int MT = 128;          // pixels per tile row (two 64-row wgmma M blocks)
+// pixels per tile row MT (template argument of the kernel): 128 = two 64-row wgmma M blocks per output row; outputs at most
+// 64 pixels wide (levels 4-6) take MT = 64, one M block per row, so that no MMA is issued for pixels right of the image
+constexpr int MT_WIDE = 128, MT_NARROW = 64;
+inline int tile_width(int OW) { return OW <= MT_NARROW && tuning().conv_narrow ? MT_NARROW : MT_WIDE; }
 constexpr int R = 2;             // output rows per CTA tile
 constexpr int NTHREADS = 384;    // warps 0..3: row-0 warpgroup, 4..7: row-1 warpgroup, 8: weight loader, 9..11: producers
 constexpr int NCONS = 8;         // consumer warps: each arrives once on every stage it releases
@@ -41,16 +46,16 @@ constexpr int BAR_BYTES = 1024;  // a_full/a_empty [MAX_AS], w_full/w_empty [MAX
 // Geometry of the converted input tile: `nslots` image rows of PW entries each.
 //   stride 1 (any dilation d): rows y0 - d .. y0 + R - 1 + d (or the 3R rows the taps touch when d >= R); entry p of a row is
 //     pixel x0 - d + p; tap (ky, kx) of output row r starts at entry slot(r, ky) * PW + kx * d.
-//   stride 2 (d = 1): rows 2 y0 - 1 .. 2 y0 + 2R - 1; a row is de-interleaved into its even pixels 2 (x0 + p), p < 128, and
-//     its odd pixels 2 (x0 - 1 + p - 128) + 1, p >= 128, so that "next output pixel" is again "next entry": tap kx reads
+//   stride 2 (d = 1): rows 2 y0 - 1 .. 2 y0 + 2R - 1; a row is de-interleaved into its even pixels 2 (x0 + p), p < MT, and
+//     its odd pixels 2 (x0 - 1 + p - MT) + 1, p >= MT, so that "next output pixel" is again "next entry": tap kx reads
 //     the odd block from 0 (kx = 0), the even block (kx = 1) or the odd block from 1 (kx = 2).
 __host__ __device__ inline int n_slots(int stride, int dil) { return stride == 2 ? 2 * R + 1 : (dil >= R ? 3 * R : R + 2 * dil); }
-__host__ __device__ inline int row_pitch(int stride, int dil) { return stride == 2 ? 2 * MT + 1 : MT + 2 * dil; }
+__host__ __device__ inline int row_pitch(int mt, int stride, int dil) { return stride == 2 ? 2 * mt + 1 : mt + 2 * dil; }
 __host__ __device__ inline int slot_of(int r, int ky, int stride, int dil) {
   return stride == 2 ? 2 * r + ky : (dil >= R ? ky * R + r : r + ky * dil);
 }
-__host__ __device__ inline int tap_xoff(int kx, int stride, int dil) {
-  return stride == 2 ? (kx == 1 ? 0 : (kx == 0 ? MT : MT + 1)) : kx * dil;
+__host__ __device__ inline int tap_xoff(int mt, int kx, int stride, int dil) {
+  return stride == 2 ? (kx == 1 ? 0 : (kx == 0 ? mt : mt + 1)) : kx * dil;
 }
 // ext = 2 ("band" mode of K3 through linearity, warp_lin.cu): the input is a VIRTUAL image of (n + 6) rows / columns --
 // the n real ones followed by [0, 0, first, 0, 0, last] -- so that ONE convolution also yields the 1-D convolutions of the
@@ -230,8 +235,9 @@ struct SmemMap {
   int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, stg_off, total, AS, WS;
 };
 // staged epilogue: per consumer warpgroup STG_CH output channels x MT pixels of fp32, row pitch SPITCH floats (the 4-float
-// pad makes the fragment stores bank-conflict-free and keeps every row 16-byte aligned for the bulk copies)
-constexpr int STG_CH = 32, SPITCH = MT + 4;
+// pad makes the fragment stores bank-conflict-free and keeps every row 16-byte aligned for the bulk copies; the 64-pixel
+// tiles use the first half of each row)
+constexpr int STG_CH = 32, SPITCH = MT_WIDE + 4;
 constexpr int STG_BYTES = R * STG_CH * SPITCH * 4;
 // stage counts from the shared-memory budget: 3 input stages when that still leaves >= 8 weight stages, else 2.
 // stg: bytes of the epilogue staging rows (0 = the layer stores from registers).  terms = 1: the input and weight stages
@@ -294,7 +300,8 @@ __global__ void conv3x3_pack_wgmma_kernel(const float* __restrict__ w, unsigned 
 
 // NW: accumulator columns per 64-pixel block (FOLD and TERMS = 3: 2 x CoutP, else CoutP or 128 per channel half).
 // FOLD: the packed image has the folded layout (CoutP <= 64).  TERMS: 3 (hi/lo split) or 1 (bf16: hi x hi only).
-template <int NW, bool FOLD, int TPS, int TERMS>
+// MT: pixels per tile row, 128 or 64 (um::tile_width).
+template <int NW, bool FOLD, int TPS, int TERMS, int MT>
 __global__ void __launch_bounds__(um::NTHREADS, 1)
     conv3x3_wgmma_kernel(const float* __restrict__ x, long long x_bs, const unsigned char* __restrict__ wpack,
                          const float* __restrict__ bias_arg, float* __restrict__ out_base, long long out_bs, int Cin, int H, int W,
@@ -312,12 +319,14 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   // stores, 8 = no MMAs, 16 = producers skip loads, conversion and shared-memory stores (they only hand over each stage);
   // the barrier protocol is unchanged, so each phase can be timed by removing it.
   static_assert(TERMS == 1 || TERMS == 3, "one or three products per multiply-add");
+  static_assert(MT == MT_WIDE || MT == MT_NARROW, "128- or 64-pixel tile rows");
   constexpr bool FOLD_ACC = FOLD && TERMS == 3;   // the accumulator holds the [hi*hi | hi*lo] column blocks
   constexpr int P = TERMS == 1 ? 1 : 2;           // planes of the input stage and of a split output
   constexpr int NCOL = FOLD_ACC ? NW / 2 : NW;    // output channels per work item
+  constexpr int MB = MT / 64;                     // m64 blocks per output row
   const int out_mode_k = out_mode_arg & 0xff, lin_prefix_k = out_mode_arg >> 8;
   extern __shared__ __align__(128) unsigned char smem[];
-  const int nslots = n_slots(stride, dil), PW = row_pitch(stride, dil), E = nslots * PW;
+  const int nslots = n_slots(stride, dil), PW = row_pitch(MT, stride, dil), E = nslots * PW;
   const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg, TERMS);
   const int AS = sm.AS, WS = sm.WS;
   const uint32_t s_base = smem_u32(smem);
@@ -349,7 +358,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
     uint32_t a_off[9];
 #pragma unroll
     for (int tap = 0; tap < 9; ++tap)
-      a_off[tap] = (uint32_t)(slot_of(r, tap / 3, stride, dil) * PW + tap_xoff(tap % 3, stride, dil));
+      a_off[tap] = (uint32_t)(slot_of(r, tap / 3, stride, dil) * PW + tap_xoff(MT, tap % 3, stride, dil));
     const uint64_t dh_a = desc_hi(a_lbo, 128u), dh_b = desc_hi(b_lbo, 128u);
     uint32_t as = 0, aph = 0, ws = 0, wph = 0;
     const uint32_t a_lo16 = (uint32_t)sm.a_lo >> 4, a_stage16 = (uint32_t)sm.a_stage >> 4, s_base16 = s_base >> 4;
@@ -364,13 +373,13 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
       }
       rel_w = rel_a = -1;
     };
-    float acc[2][NW / 2];
+    float acc[MB][NW / 2];
     for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
       const Work wk = decode_work(work, sk, nChunks);
       const int cb = wk.cb, ce = wk.ce;
       const uint32_t b_nh16 = (uint32_t)(wk.nh * NCOL);   // first weight row of this channel half (16 B rows)
-      fence_acc(acc[0]);
-      fence_acc(acc[1]);
+#pragma unroll
+      for (int mh = 0; mh < MB; ++mh) fence_acc(acc[mh]);
       if (dbg & 8) {   // profiling: the same barrier traffic without MMAs
         for (int c = cb; c < ce; ++c) {
           mbar_wait(a_full + 8 * as, aph);
@@ -397,7 +406,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           const uint32_t sc = (tap == 0 && c == cb) ? 0u : 1u;
           wgmma_fence();
 #pragma unroll
-          for (int mh = 0; mh < 2; ++mh) {
+          for (int mh = 0; mh < MB; ++mh) {
             const uint32_t a16 = a_st16 + a_off[tap] + (uint32_t)(64 * mh);
             const uint64_t a_hi = dh_a | (uint64_t)a16, a_lo = dh_a | (uint64_t)(a16 + a_lo16);
             if constexpr (TERMS == 1) {
@@ -423,8 +432,8 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         if (++as == (uint32_t)AS) { as = 0; aph ^= 1; }
       }
       wgmma_wait<0>();
-      fence_acc(acc[0]);
-      fence_acc(acc[1]);
+#pragma unroll
+      for (int mh = 0; mh < MB; ++mh) fence_acc(acc[mh]);
       release();
 
       // ---- epilogue from registers: m64nN accumulator fragment of thread (warp wq, lane): rows 16 wq + lane / 4 (+ 8),
@@ -470,7 +479,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
               const float b1 = (bias != nullptr && f + 1 < Cout) ? __ldg(bias + f + 1) : 0.f;
               unsigned char* const row = sst + (P * jj * MT + 16 * wq + (lane >> 2)) * 16 + (lane & 3) * 4;
 #pragma unroll
-              for (int mh = 0; mh < 2; ++mh)
+              for (int mh = 0; mh < MB; ++mh)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   const int i = 4 * j + 2 * h;
@@ -516,7 +525,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
               const float sl = f < lin_prefix ? 1.f : slope;
               float* const row = stg + (8 * jj + 2 * (lane & 3) + e) * SPITCH + 16 * wq + (lane >> 2);
 #pragma unroll
-              for (int mh = 0; mh < 2; ++mh)
+              for (int mh = 0; mh < MB; ++mh)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   const int i = 4 * j + 2 * h + e;
@@ -536,7 +545,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         }
       } else if (y < OH && !(dbg & 4)) {
 #pragma unroll
-        for (int mh = 0; mh < 2; ++mh) {
+        for (int mh = 0; mh < MB; ++mh) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int xx = tx * MT + 64 * mh + 16 * wq + (lane >> 2) + 8 * h;
@@ -868,6 +877,7 @@ static um::SplitK plan_split(int N, int Cin, int H, int W, int Cout, int stride,
   const int ns = cout_pad(Cout) > 128 ? 2 : 1;
   SplitK sk = {1, 0, 0, 0, 0, 0, nullptr, 0u, 0u, 3, ns};
   const int OH = (H - 1) / stride + 1, OW = (W - 1) / stride + 1, nChunks = (Cin + 15) / 16;
+  const int MT = tile_width(OW);   // OW <= 64: one tile column in either geometry, so the plan does not depend on it
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;
   const long long tiles = (long long)N * tilesX * tilesY;
   sk.from = (int)tiles;
@@ -915,6 +925,9 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   using namespace um;
   const int terms = (out_mode & MFN_CONV_BF16) ? 1 : 3;   // products per multiply-add; split operands have 2 / 1 planes
   out_mode &= ~MFN_CONV_BF16;
+  const int grow = ext == 2 ? 8 : 2 * ext;   // ext 1: grid + 1 pixel per side; ext 2: + the six band rows / columns too
+  const int OH = stride == 2 ? (H - 1) / 2 + 1 : H + grow, OW = stride == 2 ? (W - 1) / 2 + 1 : W + grow;
+  const int MT = tile_width(OW);
   SplitDev xs = {0, 0, 0, nullptr, 0, 0};
   CUtensorMap tmx;
   memset(&tmx, 0, sizeof tmx);
@@ -926,7 +939,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
     const int Cg = sa::groups(sio.in_C);
     const cuuint64_t dim[4] = {8, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N * (terms == 1 ? 1 : 2) * Cg};
     const cuuint64_t strides[3] = {16, (cuuint64_t)W * 16, (cuuint64_t)W * H * 16};
-    const cuuint32_t box[4] = {8, (cuuint32_t)row_pitch(1, dil), (cuuint32_t)(dil < R ? n_slots(1, dil) : R), dil < R ? 2u : 1u};
+    const cuuint32_t box[4] = {8, (cuuint32_t)row_pitch(MT, 1, dil), (cuuint32_t)(dil < R ? n_slots(1, dil) : R), dil < R ? 2u : 1u};
     const cuuint32_t es[4] = {1, 1, 1, 1};
     const CUresult r = fn(&tmx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(sio.in), dim, strides, box, es,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -950,10 +963,8 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   if (ext != 0 && !((ext == 1 || ext == 2) && stride == 1 && dil == 1 && out_mode == 0)) return -1;
   if ((out_mode >> 8) != 0 && (out_mode & 0xff) != 0) return -1;   // linear prefix only with plain NCHW output
   const int CoutP = um::cout_pad(Cout), nChunks = (Cin + 15) / 16;
-  const int E = n_slots(stride, dil) * row_pitch(stride, dil);
+  const int E = n_slots(stride, dil) * row_pitch(MT, stride, dil);
   const int as_wide = tuning().conv_as == 2 ? 2 : 3;
-  const int grow = ext == 2 ? 8 : 2 * ext;   // ext 1: grid + 1 pixel per side; ext 2: + the six band rows / columns too
-  const int OH = stride == 2 ? (H - 1) / 2 + 1 : H + grow, OW = stride == 2 ? (W - 1) / 2 + 1 : W + grow;
   // staged epilogue (bulk copies of whole output row segments): plain NCHW output whose rows start 16-byte aligned
   // (split output: every row segment is 16-byte aligned; the register epilogue takes the linear prefix)
   const bool staged = (out_mode & 0xff) == 0 && ext == 0 &&
@@ -962,28 +973,6 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms);
   if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
   if ((long long)H * W >= (1LL << 27)) return -1;   // the producers address a 16-plane chunk with 32-bit element offsets
-  static SmemOptIn opt[8], opt1[8];
-  if (terms == 3) {
-    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9, 3>, sm.total, opt[0]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 9, 3>, sm.total, opt[1]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, true, 3, 3>, sm.total, opt[2]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, true, 3, 3>, sm.total, opt[3]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1, 3>, sm.total, opt[4]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1, 3>, sm.total, opt[5]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1, 3>, sm.total, opt[6]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1, 3>, sm.total, opt[7]);
-    if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(conv3x3_wgmma_kernel): %s", cudaGetErrorString(e));
-  } else {
-    cudaError_t e = ensure_dyn_smem(conv3x3_wgmma_kernel<16, true, 9, 1>, sm.total, opt1[0]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9, 1>, sm.total, opt1[1]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<48, true, 3, 1>, sm.total, opt1[2]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 3, 1>, sm.total, opt1[3]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1, 1>, sm.total, opt1[4]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1, 1>, sm.total, opt1[5]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1, 1>, sm.total, opt1[6]);
-    if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1, 1>, sm.total, opt1[7]);
-    if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(conv3x3_wgmma_kernel): %s", cudaGetErrorString(e));
-  }
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;
   // split-K when the caller lent a workspace (plain grids only): one launch covers the whole tiles (normal epilogue) and the
   // parts of the split tiles (raw sums into the workspace), a second one reduces the split region
@@ -1010,40 +999,70 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const long long numWork = (sk.from + (tiles - sk.from) * sk.k) * ns;
   const int cap = tuning().conv_grid_cap > 0 ? tuning().conv_grid_cap : kNumSMs;
   const unsigned grid = (unsigned)(numWork < cap ? numWork : cap);
+  // variant name (last_kernel): the padded output width, whether the hi / lo weight images are folded, and bf16 for the
+  // one-product variant (whose accumulator is CoutP wide in every layout).  Both tile widths share a name: they compute
+  // the same sums in the same order.
+  const char* name = terms == 3 ? "conv3x3_wgmma_kernel<CoutP=256>" : "conv3x3_wgmma_kernel<CoutP=256,bf16>";
+  // one instantiation set per tile width (mt: std::integral_constant); returns a CUDA error of the shared-memory opt-in
+  auto launch = [&](auto mt) -> cudaError_t {
+    constexpr int M = decltype(mt)::value;
+    static SmemOptIn opt[8], opt1[8];
+    cudaError_t e = cudaSuccess;
+    if (terms == 3) {
+      e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9, 3, M>, sm.total, opt[0]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 9, 3, M>, sm.total, opt[1]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, true, 3, 3, M>, sm.total, opt[2]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, true, 3, 3, M>, sm.total, opt[3]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1, 3, M>, sm.total, opt[4]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1, 3, M>, sm.total, opt[5]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1, 3, M>, sm.total, opt[6]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1, 3, M>, sm.total, opt[7]);
+    } else {
+      e = ensure_dyn_smem(conv3x3_wgmma_kernel<16, true, 9, 1, M>, sm.total, opt1[0]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<32, true, 9, 1, M>, sm.total, opt1[1]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<48, true, 3, 1, M>, sm.total, opt1[2]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<64, true, 3, 1, M>, sm.total, opt1[3]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<80, false, 1, 1, M>, sm.total, opt1[4]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<96, false, 1, 1, M>, sm.total, opt1[5]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<112, false, 1, 1, M>, sm.total, opt1[6]);
+      if (e == cudaSuccess) e = ensure_dyn_smem(conv3x3_wgmma_kernel<128, false, 1, 1, M>, sm.total, opt1[7]);
+    }
+    if (e != cudaSuccess) return e;
 #define MFN_WGMMA_LAUNCH(NW_, FOLD_, TPS_, TERMS_)                                                                      \
-  conv3x3_wgmma_kernel<NW_, FOLD_, TPS_, TERMS_><<<grid, NTHREADS, sm.total, st>>>(                                    \
+  conv3x3_wgmma_kernel<NW_, FOLD_, TPS_, TERMS_, M><<<grid, NTHREADS, sm.total, st>>>(                                 \
       x, x_bs, wpack, bias, out, out_bs, Cin, H, W, OH, OW, Cout, CoutP, nChunks, slope, tilesX, tilesY, (int)numWork, \
       stride, dil, out_mode, ext, sk, xs, tmx, tuning().conv_dbg)
-  // variant name (last_kernel): the padded output width, whether the hi / lo weight images are folded, and bf16 for the
-  // one-product variant (whose accumulator is CoutP wide in every layout)
-  const char* name = "conv3x3_wgmma_kernel<CoutP=256>";
-  if (terms == 3) {
-    switch (CoutP) {
-      case 16: MFN_WGMMA_LAUNCH(32, true, 9, 3); name = "conv3x3_wgmma_kernel<CoutP=16,fold>"; break;
-      case 32: MFN_WGMMA_LAUNCH(64, true, 9, 3); name = "conv3x3_wgmma_kernel<CoutP=32,fold>"; break;
-      case 48: MFN_WGMMA_LAUNCH(96, true, 3, 3); name = "conv3x3_wgmma_kernel<CoutP=48,fold>"; break;
-      case 64: MFN_WGMMA_LAUNCH(128, true, 3, 3); name = "conv3x3_wgmma_kernel<CoutP=64,fold>"; break;
-      case 80: MFN_WGMMA_LAUNCH(80, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=80>"; break;
-      case 96: MFN_WGMMA_LAUNCH(96, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=96>"; break;
-      case 112: MFN_WGMMA_LAUNCH(112, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=112>"; break;
-      case 128: MFN_WGMMA_LAUNCH(128, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=128>"; break;
-      default: MFN_WGMMA_LAUNCH(128, false, 1, 3);   // 256: two 128-channel halves per tile
+    if (terms == 3) {
+      switch (CoutP) {
+        case 16: MFN_WGMMA_LAUNCH(32, true, 9, 3); name = "conv3x3_wgmma_kernel<CoutP=16,fold>"; break;
+        case 32: MFN_WGMMA_LAUNCH(64, true, 9, 3); name = "conv3x3_wgmma_kernel<CoutP=32,fold>"; break;
+        case 48: MFN_WGMMA_LAUNCH(96, true, 3, 3); name = "conv3x3_wgmma_kernel<CoutP=48,fold>"; break;
+        case 64: MFN_WGMMA_LAUNCH(128, true, 3, 3); name = "conv3x3_wgmma_kernel<CoutP=64,fold>"; break;
+        case 80: MFN_WGMMA_LAUNCH(80, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=80>"; break;
+        case 96: MFN_WGMMA_LAUNCH(96, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=96>"; break;
+        case 112: MFN_WGMMA_LAUNCH(112, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=112>"; break;
+        case 128: MFN_WGMMA_LAUNCH(128, false, 1, 3); name = "conv3x3_wgmma_kernel<CoutP=128>"; break;
+        default: MFN_WGMMA_LAUNCH(128, false, 1, 3);   // 256: two 128-channel halves per tile
+      }
+    } else {
+      switch (CoutP) {
+        case 16: MFN_WGMMA_LAUNCH(16, true, 9, 1); name = "conv3x3_wgmma_kernel<CoutP=16,fold,bf16>"; break;
+        case 32: MFN_WGMMA_LAUNCH(32, true, 9, 1); name = "conv3x3_wgmma_kernel<CoutP=32,fold,bf16>"; break;
+        case 48: MFN_WGMMA_LAUNCH(48, true, 3, 1); name = "conv3x3_wgmma_kernel<CoutP=48,fold,bf16>"; break;
+        case 64: MFN_WGMMA_LAUNCH(64, true, 3, 1); name = "conv3x3_wgmma_kernel<CoutP=64,fold,bf16>"; break;
+        case 80: MFN_WGMMA_LAUNCH(80, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=80,bf16>"; break;
+        case 96: MFN_WGMMA_LAUNCH(96, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=96,bf16>"; break;
+        case 112: MFN_WGMMA_LAUNCH(112, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=112,bf16>"; break;
+        case 128: MFN_WGMMA_LAUNCH(128, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=128,bf16>"; break;
+        default: MFN_WGMMA_LAUNCH(128, false, 1, 1);
+      }
     }
-  } else {
-    name = "conv3x3_wgmma_kernel<CoutP=256,bf16>";
-    switch (CoutP) {
-      case 16: MFN_WGMMA_LAUNCH(16, true, 9, 1); name = "conv3x3_wgmma_kernel<CoutP=16,fold,bf16>"; break;
-      case 32: MFN_WGMMA_LAUNCH(32, true, 9, 1); name = "conv3x3_wgmma_kernel<CoutP=32,fold,bf16>"; break;
-      case 48: MFN_WGMMA_LAUNCH(48, true, 3, 1); name = "conv3x3_wgmma_kernel<CoutP=48,fold,bf16>"; break;
-      case 64: MFN_WGMMA_LAUNCH(64, true, 3, 1); name = "conv3x3_wgmma_kernel<CoutP=64,fold,bf16>"; break;
-      case 80: MFN_WGMMA_LAUNCH(80, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=80,bf16>"; break;
-      case 96: MFN_WGMMA_LAUNCH(96, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=96,bf16>"; break;
-      case 112: MFN_WGMMA_LAUNCH(112, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=112,bf16>"; break;
-      case 128: MFN_WGMMA_LAUNCH(128, false, 1, 1); name = "conv3x3_wgmma_kernel<CoutP=128,bf16>"; break;
-      default: MFN_WGMMA_LAUNCH(128, false, 1, 1);
-    }
-  }
 #undef MFN_WGMMA_LAUNCH
+    return cudaSuccess;
+  };
+  const cudaError_t e = MT == MT_NARROW ? launch(std::integral_constant<int, MT_NARROW>{})
+                                        : launch(std::integral_constant<int, MT_WIDE>{});
+  if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(conv3x3_wgmma_kernel): %s", cudaGetErrorString(e));
   const int rc = check_launch(name);
   if (rc != 0 || sk.k <= 1) return rc;
   const long long total = sk.part_stride;

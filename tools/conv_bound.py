@@ -17,7 +17,8 @@ bracketed by CUDA events (median of --reps), in five variants of the profiling k
 The variants give invalid results; replays only time, and the forward that recorded the calls ran before any of them.
 Per launch the table prints the shape, the time, and two lower bounds:
 
-    mma    the MMA slots the kernel issues (128-pixel x 2-row tiles, padded input / output channels, three or two bf16
+    mma    the MMA slots the kernel issues (128-pixel x 2-row tiles, 64-pixel ones where the output is at most 64 pixels
+           wide, padded input / output channels, three or two bf16
            products per fp32 product, whole rounds of one work item per SM) at the 989 TFLOP/s dense-bf16 data-sheet rate
     hbm    input + output + packed weights once over the 3.35 TB/s data-sheet bandwidth
 
@@ -41,7 +42,14 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from maskflownet_b200 import _lib, network, ops  # noqa: E402
 
 PEAK_FLOPS, PEAK_BW, SMS = 989e12, 3.35e12, 132
-MT, R = 128, 2   # pixels per tile row, rows per tile (csrc/conv3x3_wgmma.cu)
+R = 2   # rows per tile (csrc/conv3x3_wgmma.cu)
+
+
+def tile_width(ow: int) -> int:
+    """Pixels per tile row (um::tile_width): one 64-pixel MMA block per row where the output is at most 64 wide."""
+    return 64 if ow <= 64 else 128
+
+
 MODES = (("full", 0), ("-load", 2), ("-input", 16), ("-store", 4), ("-mma", 8))
 
 
@@ -64,6 +72,7 @@ def mma_columns(cout_p: int, terms: int = 3) -> int:
 def bounds(c, terms=3):
     N, Cin, H, W, Cout, stride, dil = c["N"], c["Cin"], c["H"], c["W"], c["Cout"], c["stride"], c["dil"]
     OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
+    MT = tile_width(OW)
     tiles = N * ((OW + MT - 1) // MT) * ((OH + R - 1) // R)
     chunks = (Cin + 15) // 16
     cp = cout_pad(Cin, Cout)
@@ -73,7 +82,7 @@ def bounds(c, terms=3):
     ns = 2 if cp > 128 else 1
     items = tiles * k * ns
     rounds = -(-items // SMS)
-    per_item_flop = 2 * (2 * R * 64) * 16 * mma_columns(cp, terms) // ns * 9 * (-(-chunks // k))
+    per_item_flop = 2 * (R * MT) * 16 * mma_columns(cp, terms) // ns * 9 * (-(-chunks // k))
     mma = rounds * per_item_flop / (PEAK_FLOPS / SMS)
     useful = terms * 2 * N * OH * OW * Cout * Cin * 9 / PEAK_FLOPS
     Fo = Cout // 4 if c["d2s"] else Cout
