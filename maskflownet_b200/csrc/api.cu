@@ -54,6 +54,7 @@ extern "C" int mfn_set_tuning(const char* key, int value) {
   else if (!strcmp(key, "conv_as")) mfn::tuning().conv_as = value;
   else if (!strcmp(key, "conv_splitk")) mfn::tuning().conv_splitk = value;
   else if (!strcmp(key, "conv_narrow")) mfn::tuning().conv_narrow = value;
+  else if (!strcmp(key, "conv_tma_in")) mfn::tuning().conv_tma_in = value;
   else if (!strcmp(key, "corr_rb_twb")) mfn::tuning().corr_rb_twb = value;
   else if (!strcmp(key, "corr_rb_rows")) mfn::tuning().corr_rb_rows = value;
   else if (!strcmp(key, "corr_tma")) mfn::tuning().corr_tma = value;

@@ -27,6 +27,7 @@ struct Tuning {
   int conv_as = 0;            // 2: wide wgmma layers keep 2 input stages (more weight stages); default 3
   int conv_splitk = 1;        // 0: never split K; 1: plan decides (<= 8 parts); k > 1: cap on the number of parts
   int conv_narrow = 1;        // 1: wgmma outputs at most 64 px wide run 64-px tile rows (one M block per row); 0: 128-px rows
+  int conv_tma_in = 1;        // 1: fp32 wgmma inputs that fit the tensor map are staged raw by TMA; 0: per-thread loads
   int corr_rb_twb = 0;        // 2: force 16-pixel strips in the row-block kernel (two CTAs per SM when the tile fits 113 KB)
   int corr_rb_rows = 0;       // > 0: start the row-block kernel's RB search at this value (4 / 2 / 1)
   int corr_tma = 1;           // 1: C <= 32 correlations run on the TMA pipeline kernel (corr_tma.cu) when the shape fits

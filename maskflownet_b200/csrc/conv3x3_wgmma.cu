@@ -40,8 +40,9 @@ constexpr int NTHREADS = 384;    // warps 0..3: row-0 warpgroup, 4..7: row-1 war
 constexpr int NCONS = 8;         // consumer warps: each arrives once on every stage it releases
 constexpr int NPROD = 3;         // producer warps
 constexpr int MAX_AS = 4, MAX_WS = 24;
+constexpr int RS = 2;            // raw fp32 input stages of the TMA-staged input path (SplitDev::in == 2)
 constexpr int BATCH = 6;         // producer items (32 entries x 8 channels) in flight per warp
-constexpr int BAR_BYTES = 1024;  // a_full/a_empty [MAX_AS], w_full/w_empty [MAX_WS]
+constexpr int BAR_BYTES = 1024;  // a_full/a_empty [MAX_AS], w_full/w_empty [MAX_WS], r_full/r_empty [RS]
 
 // Geometry of the converted input tile: `nslots` image rows of PW entries each.
 //   stride 1 (any dilation d): rows y0 - d .. y0 + R - 1 + d (or the 3R rows the taps touch when d >= R); entry p of a row is
@@ -62,6 +63,11 @@ __host__ __device__ inline int tap_xoff(int mt, int kx, int stride, int dil) {
 // first / last row and column and the four corner pixels that the MXNet-1.5 border rule needs.  Maps a virtual
 // coordinate to the real one, or -1 (zero).
 __host__ __device__ inline int band_map(int v, int n) { return v < n ? v : (v == n + 2 ? 0 : (v == n + 5 ? n - 1 : -1)); }
+// TMA-staged fp32 input (stride 1, dilation 1, no ext): one raw stage is the tensor box {MT + 8 pixels from x0 - 4, the
+// nslots rows, 16 channels} of fp32, [channel][row][pixel].  The box starts and ends on 16-byte boundaries of the image row
+// (x0 is a multiple of MT); entry p of converted row s (pixel x0 - 1 + p) reads raw[c][s][p + 3].
+__host__ __device__ inline int raw_pitch(int mt) { return mt + 8; }
+__host__ __device__ inline int raw_stage_bytes(int nslots, int mt) { return 16 * nslots * raw_pitch(mt) * 4; }
 // output channels padded to the next multiple of 16 up to 128 (the MMA widths this file instantiates); wider layers to
 // 256 = 2 x 128
 __host__ __device__ inline int cout_pad(int cout) { return cout <= 128 ? (cout + 15) / 16 * 16 : 256; }
@@ -201,9 +207,10 @@ __device__ __forceinline__ void decode_tile(int tile, int tilesX, int tilesY, co
     n = tile / (tilesX * tilesY);
   }
 }
-// split-activation operands on the device (SplitIO): in = the input tiles come from the tensor map (groups in_g0.. of a
-// buffer of in_Cg groups per plane); out != null = output channels >= the linear prefix go to channel out_c0.. of a split
-// buffer of out_Cg groups
+// split-activation operands on the device (SplitIO): in = 1: the input tiles come from the tensor map (groups in_g0.. of a
+// buffer of in_Cg groups per plane); in = 2: fp32 input whose raw tiles the tensor map {W, H, Cin, N} stages in shared
+// memory for the producers to convert; in = 0: fp32 input the producers load themselves.  out != null = output channels
+// >= the linear prefix go to channel out_c0.. of a split buffer of out_Cg groups
 struct SplitDev {
   int in, in_g0, in_Cg;
   unsigned char* out;
@@ -232,7 +239,7 @@ __device__ __forceinline__ Work decode_work(int w, const SplitK& sk, int nChunks
 }
 
 struct SmemMap {
-  int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, stg_off, total, AS, WS;
+  int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, stg_off, total, AS, WS, raw_off, raw_stage;
 };
 // staged epilogue: per consumer warpgroup STG_CH output channels x MT pixels of fp32, row pitch SPITCH floats (the 4-float
 // pad makes the fragment stores bank-conflict-free and keeps every row 16-byte aligned for the bulk copies; the 64-pixel
@@ -242,23 +249,29 @@ constexpr int STG_BYTES = R * STG_CH * SPITCH * 4;
 // stage counts from the shared-memory budget: 3 input stages when that still leaves >= 8 weight stages, else 2.
 // stg: bytes of the epilogue staging rows (0 = the layer stores from registers).  terms = 1: the input and weight stages
 // hold the hi images alone (half the bytes; w_tile is then the hi tile [2 planes][CoutP][16 B] in shared memory, while
-// the packed image in global memory keeps its 64 CoutP bytes per tap)
-__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0, int terms = 3) {
+// the packed image in global memory keeps its 64 CoutP bytes per tap).  raw: bytes of one raw fp32 input stage of the
+// TMA-staged input path (0: none); its RS raw stages follow the input stages, and the producers, whose conversion from
+// shared memory is short, keep 2 input stages.
+__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0, int terms = 3, int raw = 0) {
   SmemMap m;
   m.a_lo = 2 * E * 16;              // hi image: two 8-channel planes of E entries
   m.a_stage = terms == 1 ? m.a_lo : 2 * m.a_lo;   // hi (+ lo)
   m.w_tile = terms == 1 ? 32 * CoutP : 64 * CoutP;   // [hi (| lo)][2 planes][CoutP][16 B]
-  const int budget = 227 * 1024 - BAR_BYTES - stg;
+  const int budget = 227 * 1024 - BAR_BYTES - stg - (raw ? RS * raw : 0);
   m.w_stage = taps_per_stage(CoutP) * m.w_tile;
   // input stages: narrow layers (several taps per weight stage) take 4 when >= 4 weight stages still fit; wide layers keep
   // the weight ring deep (their weight stages are single taps) and take 3
-  if (taps_per_stage(CoutP) > 1)
+  if (raw)
+    m.AS = 2;
+  else if (taps_per_stage(CoutP) > 1)
     m.AS = (4 * m.a_stage + 4 * m.w_stage <= budget) ? 4 : ((3 * m.a_stage + 3 * m.w_stage <= budget) ? 3 : 2);
   else   // as_wide (tuning "conv_as"): 2 trades an input stage for four more single-tap weight stages
     m.AS = (as_wide >= 3 && 3 * m.a_stage + 8 * m.w_stage <= budget) ? 3 : 2;
   int ws = (budget - m.AS * m.a_stage) / m.w_stage;
   m.WS = ws > MAX_WS ? MAX_WS : ws;
-  m.w_off = m.AS * m.a_stage;
+  m.raw_off = m.AS * m.a_stage;
+  m.raw_stage = raw;
+  m.w_off = m.raw_off + (raw ? RS * raw : 0);
   m.bar_off = m.w_off + m.WS * m.w_stage;
   m.stg_off = m.bar_off + BAR_BYTES;
   m.total = m.stg_off + stg;
@@ -327,11 +340,12 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   const int out_mode_k = out_mode_arg & 0xff, lin_prefix_k = out_mode_arg >> 8;
   extern __shared__ __align__(128) unsigned char smem[];
   const int nslots = n_slots(stride, dil), PW = row_pitch(MT, stride, dil), E = nslots * PW;
-  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg, TERMS);
+  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg, TERMS, xs.in == 2 ? raw_stage_bytes(nslots, MT) : 0);
   const int AS = sm.AS, WS = sm.WS;
   const uint32_t s_base = smem_u32(smem);
   const uint32_t bar0 = s_base + sm.bar_off;
   const uint32_t a_full = bar0, a_empty = bar0 + 8 * MAX_AS, w_full = bar0 + 16 * MAX_AS, w_empty = w_full + 8 * MAX_WS;
+  const uint32_t r_full = w_empty + 8 * MAX_WS, r_empty = r_full + 8 * RS;
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform role (keeps the wgmma path non-divergent)
@@ -339,8 +353,12 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
 
   if (tid == 0) {
     for (int i = 0; i < AS; ++i) {
-      mbar_init(a_full + 8 * i, xs.in ? 1 : NPROD);
+      mbar_init(a_full + 8 * i, xs.in == 1 ? 1 : NPROD);
       mbar_init(a_empty + 8 * i, NCONS);
+    }
+    for (int i = 0; i < RS; ++i) {
+      mbar_init(r_full + 8 * i, 1);
+      mbar_init(r_empty + 8 * i, NPROD);
     }
     for (int i = 0; i < WS; ++i) {
       mbar_init(w_full + 8 * i, 1);
@@ -625,7 +643,7 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
     }
   } else {
     // ============================ input producers (warps 9..11) ============================
-    if (xs.in) {
+    if (xs.in == 1) {
       // split input (split_act.cuh): the buffer already holds the converted entries in the stage layout, so a chunk is a
       // pure tensor copy -- hi and lo each one box {8 channels, PW pixels, nslots rows, 2 groups} (d < R), or one box of
       // R rows per kernel row, group and plane (d >= R) -- issued by one thread.  Out-of-bounds rows / pixels read zero:
@@ -702,6 +720,94 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           *reinterpret_cast<uint4*>(d) = make_uint4(0u, 0u, 0u, 0u);
           if constexpr (P == 2) *reinterpret_cast<uint4*>(d + sm.a_lo) = make_uint4(0u, 0u, 0u, 0u);
         }
+    }
+    if (xs.in == 2) {
+      // TMA-staged fp32 input (stride 1, dilation 1): one thread copies each chunk's raw tile -- the box {RP pixels from
+      // x0 - 4, the 4 rows from y0 - 1, 16 channels} of the tensor map {W, H, Cin, N}, out-of-bounds pixels, rows and
+      // channels read zero: the padding -- into a ring of RS raw stages, RS chunks ahead of the conversion and across tile
+      // boundaries.  The producers convert from shared memory the same entries, in the same layout, as the loads below.
+      // Their per-element work is then a shared-memory load at a fixed offset: no geometry checks and no address chains.
+      constexpr int RP = MT + 8, CP = (R + 2) * RP;   // raw row pitch (raw_pitch(MT)), channel pitch, in floats
+      const uint32_t raw_bytes = (uint32_t)sm.raw_stage, raw_base = s_base + (uint32_t)sm.raw_off;
+      const bool issuer = warp == 9 && lane == 0;
+      int i_work = blockIdx.x, i_c = 0, i_ce = 0, i_x = 0, i_y = 0, i_n = 0;   // issue cursor
+      auto i_tile = [&]() {
+        if (i_work >= numWork) return;
+        const Work wk = decode_work(i_work, sk, nChunks);
+        int tx, ty;
+        decode_tile(wk.tile, tilesX, tilesY, sk, tx, ty, i_n);
+        i_c = wk.cb;
+        i_ce = wk.ce;
+        i_x = tx * MT - 4;   // a 16-byte aligned start: the inner box coordinate of a tensor copy must be
+        i_y = ty * R - 1;
+      };
+      auto issue = [&](uint32_t slot) {   // the cursor's chunk into raw stage `slot`
+        if (i_work >= numWork) return;
+        const uint32_t bar = r_full + 8 * slot;
+        if (dbg & 2) {   // profiling: no global loads, the stage converts whatever it holds
+          mbar_arrive(bar);
+        } else {
+          mbar_arrive_expect_tx(bar, raw_bytes);
+          tma_load_4d(raw_base + slot * raw_bytes, &tmx, i_x, i_y, 16 * i_c, i_n, bar);
+        }
+        if (++i_c >= i_ce) {
+          i_work += gridDim.x;
+          i_tile();
+        }
+      };
+      if (issuer) {
+        i_tile();
+        for (int s = 0; s < RS; ++s) issue((uint32_t)s);
+      }
+      uint32_t as = 0, aph = 0, rs = 0, rph = 0;
+      bool wrapped = false;
+      for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
+        const Work wk = decode_work(work, sk, nChunks);
+        for (int c = wk.cb; c < wk.ce; ++c) {
+          mbar_wait(r_full + 8 * rs, rph);
+          if (wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);   // the MMAs that read this stage have completed
+          const float* raw = reinterpret_cast<const float*>(smem + sm.raw_off + rs * raw_bytes);
+          unsigned char* a_st = smem + as * sm.a_stage;
+#pragma unroll 2
+          for (int t = pw; t < nItems; t += NPROD) {
+            const int kc = one_plane ? 0 : (t & 1);
+            const int e = (one_plane ? t : (t >> 1)) * 32 + lane;
+            if (e >= E) continue;
+            const int slot = e / (MT + 2), pe = e - slot * (MT + 2);   // PW = MT + 2 at stride 1, dilation 1
+            const float* s = raw + 8 * kc * CP + slot * RP + pe + 3;
+            float v[8];
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) v[jj] = s[jj * CP];
+            if constexpr (P == 1) {
+              *reinterpret_cast<uint4*>(a_st + (kc * E + e) * 16) =
+                  make_uint4(bf16_pair(v[0], v[1]), bf16_pair(v[2], v[3]), bf16_pair(v[4], v[5]), bf16_pair(v[6], v[7]));
+            } else {
+              uint4 hi, lo;
+              split_pair(v[0], v[1], hi.x, lo.x);
+              split_pair(v[2], v[3], hi.y, lo.y);
+              split_pair(v[4], v[5], hi.z, lo.z);
+              split_pair(v[6], v[7], hi.w, lo.w);
+              unsigned char* dst = a_st + (kc * E + e) * 16;
+              *reinterpret_cast<uint4*>(dst) = hi;
+              *reinterpret_cast<uint4*>(dst + sm.a_lo) = lo;
+            }
+          }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(a_full + 8 * as);
+            mbar_arrive(r_empty + 8 * rs);   // this warp has read the raw stage
+          }
+          if (issuer) {   // all three have: refill it with the chunk RS ahead
+            mbar_wait(r_empty + 8 * rs, rph);
+            issue(rs);
+          }
+          __syncwarp();
+          if (++as == (uint32_t)AS) { as = 0; aph ^= 1; wrapped = true; }
+          if (++rs == (uint32_t)RS) { rs = 0; rph ^= 1; }
+        }
+      }
+      return;
     }
     // load cursor (runs one batch ahead of the store cursor)
     int l_work = blockIdx.x, l_c = 0, l_kb = 0, l_x0 = 0, l_y0 = 0;
@@ -970,7 +1076,31 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const bool staged = (out_mode & 0xff) == 0 && ext == 0 &&
                       (xs.out != nullptr ? (out_mode >> 8) == 0 : OW % 4 == 0 && out_bs % 4 == 0 && aligned(out, 16)) &&
                       smem_map(E, CoutP, as_wide, STG_BYTES, terms).WS >= 2;
-  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms);
+  // fp32 input staged raw by TMA (tuning "conv_tma_in"): stride 1, dilation 1, no ext, 128-pixel tiles, and a tensor map
+  // the hardware accepts -- a 16-byte aligned base and 16-byte multiples for the row, plane and sample strides (W and x_bs
+  // multiples of 4) -- with room for the raw ring beside at least 3 weight stages.  Everything else keeps the per-thread
+  // loads.  The 64-pixel tiles (levels 4-6: few tiles, many chunks each) measured no faster with the raw ring, whose
+  // two input stages and shallower weight ring lengthen their serial chunk loop.
+  int raw = 0;
+  if (sio.in == nullptr && tuning().conv_tma_in && stride == 1 && dil == 1 && ext == 0 && MT == MT_WIDE && W % 4 == 0 &&
+      x_bs % 4 == 0 && aligned(x, 16)) {
+    raw = raw_stage_bytes(n_slots(1, 1), MT);
+    if (smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms, raw).WS < 3) raw = 0;
+  }
+  if (raw) {
+    EncodeTiledFn fn = encode_tiled_fn();
+    if (fn == nullptr) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
+    const cuuint64_t dim[4] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)Cin, (cuuint64_t)N};
+    const cuuint64_t strides[3] = {(cuuint64_t)W * 4, (cuuint64_t)W * H * 4, (cuuint64_t)x_bs * 4};
+    const cuuint32_t box[4] = {(cuuint32_t)raw_pitch(MT), (cuuint32_t)n_slots(1, 1), 16, 1};
+    const cuuint32_t es[4] = {1, 1, 1, 1};
+    const CUresult r = fn(&tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), dim, strides, box, es,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
+    xs.in = 2;
+  }
+  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms, raw);
   if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
   if ((long long)H * W >= (1LL << 27)) return -1;   // the producers address a 16-plane chunk with 32-bit element offsets
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;
@@ -1000,8 +1130,8 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const int cap = tuning().conv_grid_cap > 0 ? tuning().conv_grid_cap : kNumSMs;
   const unsigned grid = (unsigned)(numWork < cap ? numWork : cap);
   // variant name (last_kernel): the padded output width, whether the hi / lo weight images are folded, and bf16 for the
-  // one-product variant (whose accumulator is CoutP wide in every layout).  Both tile widths share a name: they compute
-  // the same sums in the same order.
+  // one-product variant (whose accumulator is CoutP wide in every layout).  Both tile widths, and both fp32 input paths
+  // (per-thread loads or TMA-staged), share a name: they compute the same sums in the same order.
   const char* name = terms == 3 ? "conv3x3_wgmma_kernel<CoutP=256>" : "conv3x3_wgmma_kernel<CoutP=256,bf16>";
   // one instantiation set per tile width (mt: std::integral_constant); returns a CUDA error of the shared-memory opt-in
   auto launch = [&](auto mt) -> cudaError_t {
