@@ -5,13 +5,15 @@
 //
 // Implicit GEMM without im2col:   D[pixel, f] = sum_{tap, c} X[pixel + tap offset, c] * Wt[tap][c][f]
 //   * a work tile is R = 2 image rows x MT consecutive output pixels x (up to 128) output channels; MT = 128, or 64 where
-//     the output is at most 64 pixels wide (levels 4-6).  PERSISTENT kernel, one CTA per SM, tiles dealt round-robin; the
+//     the output is at most 64 pixels wide (levels 4-6) and at stride 2 (tile_width).  PERSISTENT kernel, one CTA per SM, tiles dealt round-robin; the
 //     producers / weight loader run ahead across tile boundaries.
 //   * K is walked as (16-channel chunk) x (tap).  Per chunk the producer warps convert the input rows the nine taps touch
 //     from fp32 NCHW into split bf16 in the *no-swizzle K-major core-matrix layout*: plane [8-channel group][pixel] with
 //     16 bytes per entry.  In that layout a tap shift is nothing but a different start address (+16 bytes per pixel), so
 //     all nine taps are nine shared-memory descriptors over ONE converted tile: (start, LBO = plane pitch, SBO = 128 B).
-//     Stride 2 de-interleaves even / odd pixels so the same holds (see the geometry helpers).
+//     Stride 2 de-interleaves even / odd pixels so the same holds (see the geometry helpers).  Where a tensor map fits
+//     the fp32 input (stride 1 on 128-pixel tiles, stride 2 on 64-pixel ones, dilation 1), one thread first stages the
+//     raw rows in shared memory with TMA and the producers convert from there (SplitDev::in == 2, raw_pitch).
 //   * weights are pre-packed (mfn_conv3x3_pack_weights) into per-(chunk, tap) images of the same layout and streamed by
 //     one thread with 1-D bulk copies (cp.async.bulk + mbarrier complete_tx) through a deep ring (up to 24 stages).
 //   * two consumer warpgroups, one per output row, each issue m64nNk16 MMAs (bf16 x bf16 -> fp32) for the MT / 64
@@ -32,17 +34,20 @@
 namespace mfn {
 namespace um {
 // pixels per tile row MT (template argument of the kernel): 128 = two 64-row wgmma M blocks per output row; outputs at most
-// 64 pixels wide (levels 4-6) take MT = 64, one M block per row, so that no MMA is issued for pixels right of the image
+// 64 pixels wide (levels 4-6) take MT = 64, one M block per row, so that no MMA is issued for pixels right of the image.
+// Stride 2 takes MT = 64 too while the TMA-staged input is on: its raw ring only fits beside 64-pixel tiles (smem_map).
 constexpr int MT_WIDE = 128, MT_NARROW = 64;
-inline int tile_width(int OW) { return OW <= MT_NARROW && tuning().conv_narrow ? MT_NARROW : MT_WIDE; }
+inline int tile_width(int OW, int stride) {
+  return tuning().conv_narrow && (OW <= MT_NARROW || (stride == 2 && tuning().conv_tma_in)) ? MT_NARROW : MT_WIDE;
+}
 constexpr int R = 2;             // output rows per CTA tile
 constexpr int NTHREADS = 384;    // warps 0..3: row-0 warpgroup, 4..7: row-1 warpgroup, 8: weight loader, 9..11: producers
 constexpr int NCONS = 8;         // consumer warps: each arrives once on every stage it releases
 constexpr int NPROD = 3;         // producer warps
 constexpr int MAX_AS = 4, MAX_WS = 24;
-constexpr int RS = 2;            // raw fp32 input stages of the TMA-staged input path (SplitDev::in == 2)
+constexpr int MAX_RS = 4;        // raw fp32 input stages of the TMA-staged input path (SplitDev::in == 2)
 constexpr int BATCH = 6;         // producer items (32 entries x 8 channels) in flight per warp
-constexpr int BAR_BYTES = 1024;  // a_full/a_empty [MAX_AS], w_full/w_empty [MAX_WS], r_full/r_empty [RS]
+constexpr int BAR_BYTES = 1024;  // a_full/a_empty [MAX_AS], w_full/w_empty [MAX_WS], r_full/r_empty [MAX_RS]
 
 // Geometry of the converted input tile: `nslots` image rows of PW entries each.
 //   stride 1 (any dilation d): rows y0 - d .. y0 + R - 1 + d (or the 3R rows the taps touch when d >= R); entry p of a row is
@@ -63,11 +68,21 @@ __host__ __device__ inline int tap_xoff(int mt, int kx, int stride, int dil) {
 // first / last row and column and the four corner pixels that the MXNet-1.5 border rule needs.  Maps a virtual
 // coordinate to the real one, or -1 (zero).
 __host__ __device__ inline int band_map(int v, int n) { return v < n ? v : (v == n + 2 ? 0 : (v == n + 5 ? n - 1 : -1)); }
-// TMA-staged fp32 input (stride 1, dilation 1, no ext): one raw stage is the tensor box {MT + 8 pixels from x0 - 4, the
-// nslots rows, 16 channels} of fp32, [channel][row][pixel].  The box starts and ends on 16-byte boundaries of the image row
-// (x0 is a multiple of MT); entry p of converted row s (pixel x0 - 1 + p) reads raw[c][s][p + 3].
-__host__ __device__ inline int raw_pitch(int mt) { return mt + 8; }
-__host__ __device__ inline int raw_stage_bytes(int nslots, int mt) { return 16 * nslots * raw_pitch(mt) * 4; }
+// TMA-staged fp32 input (dilation 1, no ext): one raw stage is a tensor box of fp32, [channel][row][pixel], that starts
+// and ends on 16-byte boundaries of the image row (x0, the tile's first output pixel, is a multiple of MT):
+//   stride 1: {MT + 8 pixels from x0 - 4, the nslots rows, 16 channels}; entry p of converted row s (pixel x0 - 1 + p)
+//     reads raw[c][s][p + 3].
+//   stride 2 (MT = 64): {2 MT + 4 pixels from 2 x0 - 4, the 5 rows, 8 channels}, one 8-channel plane of the chunk per
+//     stage; even entry p < MT (pixel 2 (x0 + p)) reads raw[c][s][2 p + 4], odd entry p >= MT (pixel
+//     2 (x0 - 1 + p - MT) + 1) reads raw[c][s][2 (p - MT) + 3].
+__host__ __device__ inline int raw_pitch(int mt, int stride) { return stride == 2 ? 2 * mt + 4 : mt + 8; }
+__host__ __device__ inline int raw_channels(int stride) { return stride == 2 ? 8 : 16; }
+__host__ __device__ inline int raw_stage_bytes(int nslots, int mt, int stride) {
+  return raw_channels(stride) * nslots * raw_pitch(mt, stride) * 4;
+}
+// most raw stages the ring may take: stride 1 keeps the 2 it was measured with; stride 2, whose 8-channel stages hold less
+// (conv1a's 3 channels: 8 KB of image per stage), deepens the ring while >= 3 weight stages still fit (smem_map)
+__host__ __device__ inline int raw_ring_max(int stride) { return stride == 2 ? MAX_RS : 2; }
 // output channels padded to the next multiple of 16 up to 128 (the MMA widths this file instantiates); wider layers to
 // 256 = 2 x 128
 __host__ __device__ inline int cout_pad(int cout) { return cout <= 128 ? (cout + 15) / 16 * 16 : 256; }
@@ -239,7 +254,7 @@ __device__ __forceinline__ Work decode_work(int w, const SplitK& sk, int nChunks
 }
 
 struct SmemMap {
-  int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, stg_off, total, AS, WS, raw_off, raw_stage;
+  int a_lo, a_stage, w_tile, w_stage, w_off, bar_off, stg_off, total, AS, WS, raw_off, raw_stage, RS;
 };
 // staged epilogue: per consumer warpgroup STG_CH output channels x MT pixels of fp32, row pitch SPITCH floats (the 4-float
 // pad makes the fragment stores bank-conflict-free and keeps every row 16-byte aligned for the bulk copies; the 64-pixel
@@ -250,15 +265,24 @@ constexpr int STG_BYTES = R * STG_CH * SPITCH * 4;
 // stg: bytes of the epilogue staging rows (0 = the layer stores from registers).  terms = 1: the input and weight stages
 // hold the hi images alone (half the bytes; w_tile is then the hi tile [2 planes][CoutP][16 B] in shared memory, while
 // the packed image in global memory keeps its 64 CoutP bytes per tap).  raw: bytes of one raw fp32 input stage of the
-// TMA-staged input path (0: none); its RS raw stages follow the input stages, and the producers, whose conversion from
+// TMA-staged input path (0: none); its RS raw stages (the most up to rs_max that leave >= 3 weight stages, at least 2)
+// follow the input stages at a 128-byte boundary (tensor-copy destinations), and the producers, whose conversion from
 // shared memory is short, keep 2 input stages.
-__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0, int terms = 3, int raw = 0) {
+__host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, int stg = 0, int terms = 3, int raw = 0,
+                                            int rs_max = 2) {
   SmemMap m;
   m.a_lo = 2 * E * 16;              // hi image: two 8-channel planes of E entries
   m.a_stage = terms == 1 ? m.a_lo : 2 * m.a_lo;   // hi (+ lo)
   m.w_tile = terms == 1 ? 32 * CoutP : 64 * CoutP;   // [hi (| lo)][2 planes][CoutP][16 B]
-  const int budget = 227 * 1024 - BAR_BYTES - stg - (raw ? RS * raw : 0);
+  int budget = 227 * 1024 - BAR_BYTES - stg;
   m.w_stage = taps_per_stage(CoutP) * m.w_tile;
+  m.RS = 0;
+  if (raw) {
+    const int raw_off = (2 * m.a_stage + 127) / 128 * 128;
+    m.RS = rs_max;
+    while (m.RS > 2 && budget - raw_off - m.RS * raw < 3 * m.w_stage) --m.RS;
+    budget -= m.RS * raw + (raw_off - 2 * m.a_stage);
+  }
   // input stages: narrow layers (several taps per weight stage) take 4 when >= 4 weight stages still fit; wide layers keep
   // the weight ring deep (their weight stages are single taps) and take 3
   if (raw)
@@ -269,9 +293,9 @@ __host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, i
     m.AS = (as_wide >= 3 && 3 * m.a_stage + 8 * m.w_stage <= budget) ? 3 : 2;
   int ws = (budget - m.AS * m.a_stage) / m.w_stage;
   m.WS = ws > MAX_WS ? MAX_WS : ws;
-  m.raw_off = m.AS * m.a_stage;
+  m.raw_off = raw ? (m.AS * m.a_stage + 127) / 128 * 128 : m.AS * m.a_stage;
   m.raw_stage = raw;
-  m.w_off = m.raw_off + (raw ? RS * raw : 0);
+  m.w_off = m.raw_off + m.RS * raw;
   m.bar_off = m.w_off + m.WS * m.w_stage;
   m.stg_off = m.bar_off + BAR_BYTES;
   m.total = m.stg_off + stg;
@@ -340,12 +364,13 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   const int out_mode_k = out_mode_arg & 0xff, lin_prefix_k = out_mode_arg >> 8;
   extern __shared__ __align__(128) unsigned char smem[];
   const int nslots = n_slots(stride, dil), PW = row_pitch(MT, stride, dil), E = nslots * PW;
-  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg, TERMS, xs.in == 2 ? raw_stage_bytes(nslots, MT) : 0);
-  const int AS = sm.AS, WS = sm.WS;
+  const SmemMap sm = smem_map(E, CoutP, sk.as_wide, sk.stg, TERMS, xs.in == 2 ? raw_stage_bytes(nslots, MT, stride) : 0,
+                              raw_ring_max(stride));
+  const int AS = sm.AS, WS = sm.WS, RS = sm.RS;
   const uint32_t s_base = smem_u32(smem);
   const uint32_t bar0 = s_base + sm.bar_off;
   const uint32_t a_full = bar0, a_empty = bar0 + 8 * MAX_AS, w_full = bar0 + 16 * MAX_AS, w_empty = w_full + 8 * MAX_WS;
-  const uint32_t r_full = w_empty + 8 * MAX_WS, r_empty = r_full + 8 * RS;
+  const uint32_t r_full = w_empty + 8 * MAX_WS, r_empty = r_full + 8 * MAX_RS;
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform role (keeps the wgmma path non-divergent)
@@ -722,15 +747,19 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         }
     }
     if (xs.in == 2) {
-      // TMA-staged fp32 input (stride 1, dilation 1): one thread copies each chunk's raw tile -- the box {RP pixels from
-      // x0 - 4, the 4 rows from y0 - 1, 16 channels} of the tensor map {W, H, Cin, N}, out-of-bounds pixels, rows and
-      // channels read zero: the padding -- into a ring of RS raw stages, RS chunks ahead of the conversion and across tile
-      // boundaries.  The producers convert from shared memory the same entries, in the same layout, as the loads below.
-      // Their per-element work is then a shared-memory load at a fixed offset: no geometry checks and no address chains.
-      constexpr int RP = MT + 8, CP = (R + 2) * RP;   // raw row pitch (raw_pitch(MT)), channel pitch, in floats
+      // TMA-staged fp32 input (dilation 1): one thread copies each chunk's raw tile -- at stride 1 the box {MT + 8 pixels
+      // from x0 - 4, the 4 rows from y0 - 1, 16 channels}, at stride 2 one box {2 MT + 4 pixels from 2 x0 - 4, the 5 rows
+      // from 2 y0 - 1, 8 channels} per 8-channel plane (raw_pitch) of the tensor map {W, H, Cin, N}, out-of-bounds pixels,
+      // rows and channels read zero: the padding -- into a ring of RS raw stages, RS stages ahead of the conversion and
+      // across tile boundaries.  The producers convert from shared memory the same entries, in the same layout, as the
+      // loads below.  Their per-element work is then a shared-memory load at a fixed offset: no geometry checks and no
+      // address chains.
+      const bool s2 = stride == 2;
+      const int RP = raw_pitch(MT, stride), CP = nslots * RP;   // raw row and channel pitch, in floats
+      const int RPC = s2 && !one_plane ? 2 : 1;                 // raw stages per chunk (Cin <= 8: plane 1 stays zero)
       const uint32_t raw_bytes = (uint32_t)sm.raw_stage, raw_base = s_base + (uint32_t)sm.raw_off;
       const bool issuer = warp == 9 && lane == 0;
-      int i_work = blockIdx.x, i_c = 0, i_ce = 0, i_x = 0, i_y = 0, i_n = 0;   // issue cursor
+      int i_work = blockIdx.x, i_c = 0, i_h = 0, i_ce = 0, i_x = 0, i_y = 0, i_n = 0;   // issue cursor
       auto i_tile = [&]() {
         if (i_work >= numWork) return;
         const Work wk = decode_work(i_work, sk, nChunks);
@@ -738,18 +767,21 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
         decode_tile(wk.tile, tilesX, tilesY, sk, tx, ty, i_n);
         i_c = wk.cb;
         i_ce = wk.ce;
-        i_x = tx * MT - 4;   // a 16-byte aligned start: the inner box coordinate of a tensor copy must be
-        i_y = ty * R - 1;
+        // a 16-byte aligned start: the inner box coordinate of a tensor copy must be
+        i_x = s2 ? 2 * tx * MT - 4 : tx * MT - 4;
+        i_y = s2 ? 2 * ty * R - 1 : ty * R - 1;
       };
-      auto issue = [&](uint32_t slot) {   // the cursor's chunk into raw stage `slot`
+      auto issue = [&](uint32_t slot) {   // the cursor's chunk (plane i_h at stride 2) into raw stage `slot`
         if (i_work >= numWork) return;
         const uint32_t bar = r_full + 8 * slot;
         if (dbg & 2) {   // profiling: no global loads, the stage converts whatever it holds
           mbar_arrive(bar);
         } else {
           mbar_arrive_expect_tx(bar, raw_bytes);
-          tma_load_4d(raw_base + slot * raw_bytes, &tmx, i_x, i_y, 16 * i_c, i_n, bar);
+          tma_load_4d(raw_base + slot * raw_bytes, &tmx, i_x, i_y, 16 * i_c + 8 * i_h, i_n, bar);
         }
+        if (++i_h < RPC) return;
+        i_h = 0;
         if (++i_c >= i_ce) {
           i_work += gridDim.x;
           i_tile();
@@ -764,47 +796,72 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
       for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
         const Work wk = decode_work(work, sk, nChunks);
         for (int c = wk.cb; c < wk.ce; ++c) {
-          mbar_wait(r_full + 8 * rs, rph);
-          if (wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);   // the MMAs that read this stage have completed
-          const float* raw = reinterpret_cast<const float*>(smem + sm.raw_off + rs * raw_bytes);
           unsigned char* a_st = smem + as * sm.a_stage;
-#pragma unroll 2
-          for (int t = pw; t < nItems; t += NPROD) {
-            const int kc = one_plane ? 0 : (t & 1);
-            const int e = (one_plane ? t : (t >> 1)) * 32 + lane;
-            if (e >= E) continue;
-            const int slot = e / (MT + 2), pe = e - slot * (MT + 2);   // PW = MT + 2 at stride 1, dilation 1
-            const float* s = raw + 8 * kc * CP + slot * RP + pe + 3;
-            float v[8];
+          for (int h = 0; h < RPC; ++h) {
+            mbar_wait(r_full + 8 * rs, rph);
+            if (h == 0 && wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);   // the MMAs that read this stage have completed
+            const float* raw = reinterpret_cast<const float*>(smem + sm.raw_off + rs * raw_bytes);
+            auto put = [&](int kc, int e, const float (&v)[8]) {
+              if constexpr (P == 1) {
+                *reinterpret_cast<uint4*>(a_st + (kc * E + e) * 16) =
+                    make_uint4(bf16_pair(v[0], v[1]), bf16_pair(v[2], v[3]), bf16_pair(v[4], v[5]), bf16_pair(v[6], v[7]));
+              } else {
+                uint4 hi, lo;
+                split_pair(v[0], v[1], hi.x, lo.x);
+                split_pair(v[2], v[3], hi.y, lo.y);
+                split_pair(v[4], v[5], hi.z, lo.z);
+                split_pair(v[6], v[7], hi.w, lo.w);
+                unsigned char* dst = a_st + (kc * E + e) * 16;
+                *reinterpret_cast<uint4*>(dst) = hi;
+                *reinterpret_cast<uint4*>(dst + sm.a_lo) = lo;
+              }
+            };
+            if (s2) {
+              // plane h.  Unit j of row s reads the adjacent pair raw[c][s][2 j + 2 .. 2 j + 3] (one 8-byte load per
+              // channel: consecutive lanes, consecutive words) and writes odd entry MT + j and even entry j - 1.
+              constexpr int U = MT + 1;   // units per row
+              for (int u = pw * 32 + lane; u < (2 * R + 1) * U; u += NPROD * 32) {
+                const int slot = u / U, j = u - slot * U;
+                const float* s = raw + slot * RP + 2 * j + 2;
+                float ve[8], vo[8];
 #pragma unroll
-            for (int jj = 0; jj < 8; ++jj) v[jj] = s[jj * CP];
-            if constexpr (P == 1) {
-              *reinterpret_cast<uint4*>(a_st + (kc * E + e) * 16) =
-                  make_uint4(bf16_pair(v[0], v[1]), bf16_pair(v[2], v[3]), bf16_pair(v[4], v[5]), bf16_pair(v[6], v[7]));
+                for (int jj = 0; jj < 8; ++jj) {
+                  const float2 p2 = *reinterpret_cast<const float2*>(s + jj * CP);
+                  ve[jj] = p2.x;
+                  vo[jj] = p2.y;
+                }
+                put(h, slot * PW + MT + j, vo);
+                if (j > 0) put(h, slot * PW + j - 1, ve);
+              }
             } else {
-              uint4 hi, lo;
-              split_pair(v[0], v[1], hi.x, lo.x);
-              split_pair(v[2], v[3], hi.y, lo.y);
-              split_pair(v[4], v[5], hi.z, lo.z);
-              split_pair(v[6], v[7], hi.w, lo.w);
-              unsigned char* dst = a_st + (kc * E + e) * 16;
-              *reinterpret_cast<uint4*>(dst) = hi;
-              *reinterpret_cast<uint4*>(dst + sm.a_lo) = lo;
+#pragma unroll 2
+              for (int t = pw; t < nItems; t += NPROD) {
+                const int kc = one_plane ? 0 : (t & 1);
+                const int e = (one_plane ? t : (t >> 1)) * 32 + lane;
+                if (e >= E) continue;
+                const int slot = e / (MT + 2), pe = e - slot * (MT + 2);   // PW = MT + 2 at stride 1, dilation 1
+                const float* s = raw + 8 * kc * CP + slot * RP + pe + 3;
+                float v[8];
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) v[jj] = s[jj * CP];
+                put(kc, e, v);
+              }
             }
+            const bool last = h == RPC - 1;
+            if (last) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> tensor core
+            __syncwarp();
+            if (lane == 0) {
+              if (last) mbar_arrive(a_full + 8 * as);
+              mbar_arrive(r_empty + 8 * rs);   // this warp has read the raw stage
+            }
+            if (issuer) {   // all three have: refill it RS stages ahead
+              mbar_wait(r_empty + 8 * rs, rph);
+              issue(rs);
+            }
+            __syncwarp();
+            if (++rs == (uint32_t)RS) { rs = 0; rph ^= 1; }
           }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(a_full + 8 * as);
-            mbar_arrive(r_empty + 8 * rs);   // this warp has read the raw stage
-          }
-          if (issuer) {   // all three have: refill it with the chunk RS ahead
-            mbar_wait(r_empty + 8 * rs, rph);
-            issue(rs);
-          }
-          __syncwarp();
           if (++as == (uint32_t)AS) { as = 0; aph ^= 1; wrapped = true; }
-          if (++rs == (uint32_t)RS) { rs = 0; rph ^= 1; }
         }
       }
       return;
@@ -983,7 +1040,8 @@ static um::SplitK plan_split(int N, int Cin, int H, int W, int Cout, int stride,
   const int ns = cout_pad(Cout) > 128 ? 2 : 1;
   SplitK sk = {1, 0, 0, 0, 0, 0, nullptr, 0u, 0u, 3, ns};
   const int OH = (H - 1) / stride + 1, OW = (W - 1) / stride + 1, nChunks = (Cin + 15) / 16;
-  const int MT = tile_width(OW);   // OW <= 64: one tile column in either geometry, so the plan does not depend on it
+  // the launch's tile width: OW <= 64 is one tile column in either geometry, so only stride 2 with OW > 64 depends on it
+  const int MT = tile_width(OW, stride);
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;
   const long long tiles = (long long)N * tilesX * tilesY;
   sk.from = (int)tiles;
@@ -1033,7 +1091,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   out_mode &= ~MFN_CONV_BF16;
   const int grow = ext == 2 ? 8 : 2 * ext;   // ext 1: grid + 1 pixel per side; ext 2: + the six band rows / columns too
   const int OH = stride == 2 ? (H - 1) / 2 + 1 : H + grow, OW = stride == 2 ? (W - 1) / 2 + 1 : W + grow;
-  const int MT = tile_width(OW);
+  const int MT = tile_width(OW, stride);
   SplitDev xs = {0, 0, 0, nullptr, 0, 0};
   CUtensorMap tmx;
   memset(&tmx, 0, sizeof tmx);
@@ -1076,23 +1134,26 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const bool staged = (out_mode & 0xff) == 0 && ext == 0 &&
                       (xs.out != nullptr ? (out_mode >> 8) == 0 : OW % 4 == 0 && out_bs % 4 == 0 && aligned(out, 16)) &&
                       smem_map(E, CoutP, as_wide, STG_BYTES, terms).WS >= 2;
-  // fp32 input staged raw by TMA (tuning "conv_tma_in"): stride 1, dilation 1, no ext, 128-pixel tiles, and a tensor map
-  // the hardware accepts -- a 16-byte aligned base and 16-byte multiples for the row, plane and sample strides (W and x_bs
-  // multiples of 4) -- with room for the raw ring beside at least 3 weight stages.  Everything else keeps the per-thread
-  // loads.  The 64-pixel tiles (levels 4-6: few tiles, many chunks each) measured no faster with the raw ring, whose
-  // two input stages and shallower weight ring lengthen their serial chunk loop.
+  // fp32 input staged raw by TMA (tuning "conv_tma_in"): dilation 1, no ext, stride 1 on 128-pixel tiles or stride 2 on
+  // the 64-pixel tiles of outputs wider than 64 pixels, and a tensor map the hardware accepts -- a 16-byte aligned base and
+  // 16-byte multiples for the row, plane and sample strides (W and x_bs multiples of 4) -- with room for the raw ring
+  // beside at least 3 weight stages.  Everything else keeps the per-thread loads.  The tiles of outputs at most 64 pixels
+  // wide (levels 4-6: few tiles, many chunks each) measured no faster with the raw ring at stride 1, whose two input
+  // stages and shallower weight ring lengthen their serial chunk loop; their stride-2 layers are not measured with it.
   int raw = 0;
-  if (sio.in == nullptr && tuning().conv_tma_in && stride == 1 && dil == 1 && ext == 0 && MT == MT_WIDE && W % 4 == 0 &&
-      x_bs % 4 == 0 && aligned(x, 16)) {
-    raw = raw_stage_bytes(n_slots(1, 1), MT);
-    if (smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms, raw).WS < 3) raw = 0;
+  const bool raw_geometry = stride == 1 ? dil == 1 && MT == MT_WIDE : MT == MT_NARROW && OW > MT_NARROW;
+  if (sio.in == nullptr && tuning().conv_tma_in && raw_geometry && ext == 0 && W % 4 == 0 && x_bs % 4 == 0 &&
+      aligned(x, 16)) {
+    raw = raw_stage_bytes(n_slots(stride, 1), MT, stride);
+    if (smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms, raw, raw_ring_max(stride)).WS < 3) raw = 0;
   }
   if (raw) {
     EncodeTiledFn fn = encode_tiled_fn();
     if (fn == nullptr) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
     const cuuint64_t dim[4] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)Cin, (cuuint64_t)N};
     const cuuint64_t strides[3] = {(cuuint64_t)W * 4, (cuuint64_t)W * H * 4, (cuuint64_t)x_bs * 4};
-    const cuuint32_t box[4] = {(cuuint32_t)raw_pitch(MT), (cuuint32_t)n_slots(1, 1), 16, 1};
+    const cuuint32_t box[4] = {(cuuint32_t)raw_pitch(MT, stride), (cuuint32_t)n_slots(stride, 1),
+                               (cuuint32_t)raw_channels(stride), 1};
     const cuuint32_t es[4] = {1, 1, 1, 1};
     const CUresult r = fn(&tmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), dim, strides, box, es,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1100,7 +1161,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
     if (r != CUDA_SUCCESS) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
     xs.in = 2;
   }
-  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms, raw);
+  const SmemMap sm = smem_map(E, CoutP, as_wide, staged ? STG_BYTES : 0, terms, raw, raw_ring_max(stride));
   if (sm.WS < 2 || E * 16 > 0x3FFF * 16) return -1;
   if ((long long)H * W >= (1LL << 27)) return -1;   // the producers address a 16-plane chunk with 32-bit element offsets
   const int tilesX = (OW + MT - 1) / MT, tilesY = (OH + R - 1) / R;

@@ -222,10 +222,17 @@ class _FlowNetBase(nn.Module):
         return feats  # [c?1 .. c?6]
 
     def _pyramid_pair(self, im1, im2, names):
-        """Both images through the shared pyramid; inference batches them into one pass (half the launches)."""
+        """Both images through the shared pyramid; inference batches them into one pass (half the launches).  When im1 and
+        im2 are the two adjacent halves of one buffer (ops.preprocess), that buffer is the batch: no copy."""
         if self._fast(im1):
             n = im1.shape[0]
-            f = self._pyramid(torch.cat([im1, im2], dim=0), names)
+            if (im1.is_contiguous() and im2.is_contiguous() and im1.shape == im2.shape and im1.dtype == im2.dtype
+                    and im1.untyped_storage().data_ptr() == im2.untyped_storage().data_ptr()
+                    and im2.storage_offset() == im1.storage_offset() + im1.numel()):
+                x = im1.view(-1).as_strided((2 * im1.numel(),), (1,)).view((2 * n,) + tuple(im1.shape[1:]))
+            else:
+                x = torch.cat([im1, im2], dim=0)
+            f = self._pyramid(x, names)
             return [t[:n] for t in f], [t[n:] for t in f]
         return self._pyramid(im1, names), self._pyramid(im2, names)
 

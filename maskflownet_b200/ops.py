@@ -737,7 +737,9 @@ def padded_size(H: int, W: int, resize=None):
 
 def preprocess(img1: torch.Tensor, img2: torch.Tensor, out_hw=None):
     """/255 (uint8 input) -> centralize -> BilinearResize2D to out_hw: what PipelineFlownet.predict + do_batch_mx do before
-    the network (network/pipeline.py:206-212, 85-87, 117-130).  Returns (im1, im2, rgb_mean (N,C,1,1)).  Forward only."""
+    the network (network/pipeline.py:206-212, 85-87, 117-130).  Returns (im1, im2, rgb_mean (N,C,1,1)).  Forward only.
+    im1 and im2 are the two halves of one (2N, C, OH, OW) buffer, which the network's shared pyramid reads as one batch
+    without a copy."""
     for t, nm in ((img1, "img1"), (img2, "img2")):
         if not (t.is_cuda and t.is_contiguous() and t.dim() == 4 and t.dtype in (torch.uint8, torch.float32)):
             raise MaskflowError(f"preprocess: {nm} must be a contiguous CUDA uint8 / float32 NCHW tensor")
@@ -746,8 +748,8 @@ def preprocess(img1: torch.Tensor, img2: torch.Tensor, out_hw=None):
     _no_grad_path("preprocess", img1, img2)
     N, C, H, W = img1.shape
     OH, OW = (H, W) if out_hw is None else (int(out_hw[0]), int(out_hw[1]))
-    o1 = torch.empty((N, C, OH, OW), device=img1.device, dtype=torch.float32)
-    o2 = torch.empty_like(o1)
+    pair = torch.empty((2 * N, C, OH, OW), device=img1.device, dtype=torch.float32)
+    o1, o2 = pair[:N], pair[N:]
     mean = torch.empty((N, C, 1, 1), device=img1.device, dtype=torch.float32)
     args = (_p(img1), _p(img2), 1 if img1.dtype == torch.uint8 else 0, _p(o1), _p(o2), _p(mean), N, C, H, W, OH, OW)
     if deterministic():

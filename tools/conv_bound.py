@@ -18,7 +18,7 @@ The variants give invalid results; replays only time, and the forward that recor
 Per launch the table prints the shape, the time, and two lower bounds:
 
     mma    the MMA slots the kernel issues (128-pixel x 2-row tiles, 64-pixel ones where the output is at most 64 pixels
-           wide, padded input / output channels, three or two bf16
+           wide and at stride 2, padded input / output channels, three or two bf16
            products per fp32 product, whole rounds of one work item per SM) at the 989 TFLOP/s dense-bf16 data-sheet rate
     hbm    input + output + packed weights once over the 3.35 TB/s data-sheet bandwidth
 
@@ -45,9 +45,10 @@ PEAK_FLOPS, PEAK_BW, SMS = 989e12, 3.35e12, 132
 R = 2   # rows per tile (csrc/conv3x3_wgmma.cu)
 
 
-def tile_width(ow: int) -> int:
-    """Pixels per tile row (um::tile_width): one 64-pixel MMA block per row where the output is at most 64 wide."""
-    return 64 if ow <= 64 else 128
+def tile_width(ow: int, stride: int) -> int:
+    """Pixels per tile row (um::tile_width): one 64-pixel MMA block per row where the output is at most 64 wide, and at
+    stride 2 (the TMA-staged input's tiles)."""
+    return 64 if ow <= 64 or stride == 2 else 128
 
 
 MODES = (("full", 0), ("-load", 2), ("-input", 16), ("-store", 4), ("-mma", 8))
@@ -72,7 +73,7 @@ def mma_columns(cout_p: int, terms: int = 3) -> int:
 def bounds(c, terms=3):
     N, Cin, H, W, Cout, stride, dil = c["N"], c["Cin"], c["H"], c["W"], c["Cout"], c["stride"], c["dil"]
     OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
-    MT = tile_width(OW)
+    MT = tile_width(OW, stride)
     tiles = N * ((OW + MT - 1) // MT) * ((OH + R - 1) // R)
     chunks = (Cin + 15) // 16
     cp = cout_pad(Cin, Cout)
