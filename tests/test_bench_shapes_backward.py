@@ -23,11 +23,18 @@ cannot).  Additions to it, each derived where it is used:
   * deterministic mode (det.cuh): an element that receives n fixed-point contributions is off by n 2^(k+e-62) + u |ref|;
   * the image warp and the EPE read fp32 positions / up-sampled values the reference cannot reproduce bit for bit: their
     rounding (2^-20 (|p| + |d| + 1) px, gamma_5 of the interpolated values) times the slope.
-The image warp's backward is checked on what the cascade's graph asks of it: g_mask_up, and g_im2 where the image
-requires a gradient; its flow gradient is not checked here (an fp32 position a rounding away from an integer may take the
-other cell's slope, which no rounding bound covers).
+The robust EPE of the KITTI / Sintel fine-tuning, e = (|d0| + |d1| + eps)^q with q = 0.4, eps = 1e-8, has a steep
+gradient q s^(q-1) sign(d_c) near d = 0 (s = |d0| + |d1| + eps), so its bound is taken over the box the kernel's fp32 d can
+lie in: each d_c off by delta_c = gamma_6 (max |pred| + |flow_c|), s in [s_lo, s_hi], widened by powf's error.  Where
+|d_c| <= delta_c the sign is open; where s_lo reaches eps the bound is rigorous but says little, and the fraction of such
+gradient elements is reported and asserted small (epe_backward_bounds, test_dataset_shapes_backward.py).
+The image warp's backward is checked on what the cascade's graph asks of it: g_mask_up, g_im2 where the image requires a
+gradient, and g_flow_up where the flow does (the cascade trained end to end).  The flow gradient is the sampler's slope,
+which jumps where the position crosses an integer: an fp32 position within its rounding bound of an integer may take
+either cell's slope, and is accepted against either (image_warp_flow_slopes).
 The cuDNN convolution backward (ops._Conv3x3TrainFn) is not this library's arithmetic: only its wiring is checked (mask from
-the saved y, stride, dilation, padding, bias) against float64 autograd at 2^-12 S.
+the saved y, stride, dilation, padding, bias) against float64 autograd at 2^-12 (S + 2^-8 max S): cuDNN's transform
+algorithms leave rounding noise where the exact gradient is 0, which a wiring error (O(S) everywhere) is far above.
 
 Sensitivity is asserted (each control must fail the bound by CONTROL_MARGIN on one real launch of each kind) and so is
 coverage (launch counts per kind equal the graph's; the deterministic run calls the *_det entry points only).
@@ -46,6 +53,9 @@ from oracle import torch_ref
 from test_bench_shapes import Recorder, _fp32_positions, _images_u8, _named_model, _ratio, _warp_offsets
 
 U = 2.0 ** -24
+# powf is within 4 ulp over its full range (CUDA C Programming Guide, "Mathematical Functions": single-precision maximum
+# ulp errors); one ulp of a normal result is at most 2^-23 of it
+POWF_REL = 4 * 2.0 ** -23
 CONTROL_MARGIN = 3.0
 EPS_WIRING = 2.0 ** -12
 TAPS = tuple((i, j) for i in range(3) for j in range(3))
@@ -162,6 +172,211 @@ def sigmoid_error(v):
     return s, s * (1 - s) * d_exp + 2 * U * s
 
 
+# ---- fused MultiscaleEpe (loss.cu) -----------------------------------------------------------------------------------
+def epe_terms(flow, mask, preds, scales, weights, eps, q, zero=None):
+    """float64 per-sample loss; per scale the up-sampled prediction u and the per-pixel EPE e.  q < 0: the L2 form
+    sqrt(|d|^2 + eps); q >= 0: the robust form (|d0| + |d1| + eps)^q, whose autograd takes sign(0) = 0 as the kernel does.
+    zero = (scale, bool (N, 1, H, W)): pixels where the kernel's d is exactly 0 at that scale (u is the label there)."""
+    f64, m64 = flow.double(), mask.double()
+    loss, parts = 0, []
+    for p, s, w in zip(preds, scales, weights):
+        u = torch_ref.upsample(p, s)
+        if zero is not None and s == zero[0]:
+            u = torch.where(zero[1], f64, u)
+        if q < 0:
+            e = torch.sqrt(((u - f64) ** 2).sum(1, keepdim=True) + eps)
+        else:
+            e = ((u - f64).abs().sum(1, keepdim=True) + eps) ** q
+        loss = loss + w * (e * m64).sum(dim=(1, 2, 3))
+        parts.append((u, e))
+    return loss / m64.sum(dim=(1, 2, 3)), parts
+
+
+def epe_delta(p, flow, s, zero=None):
+    """delta_c = gamma_6 (max |pred| + |flow_c|): how far the kernel's fp32 d = Upsample(s)(pred) - flow (5 roundings of
+    the interpolation, 1 of the difference) can lie from the float64 one; 0 where d is known to be exactly 0."""
+    M = p.abs().amax(dim=(1, 2, 3), keepdim=True).double()
+    delta = gamma(6) * (M + flow.double().abs())
+    if zero is not None and s == zero[0]:
+        delta = delta * ~zero[1]
+    return delta
+
+
+def epe_q_box(d, delta, eps):
+    """The robust EPE's s = |d0| + |d1| + eps (float64, (N, 1, H, W)) and the box [s_lo, s_hi] of the kernel's
+    fl(fl(|d0'| + |d1'|) + eps) when |d_c' - d_c| <= delta_c: the two additions round (gamma_2), and a rounded sum of
+    nonnegative terms and eps cannot fall below eps."""
+    s = d.abs().sum(1, keepdim=True) + eps
+    dd = delta.sum(1, keepdim=True)
+    return s, torch.clamp((s - dd) * (1 - gamma(2)), min=eps), (s + dd) * (1 + gamma(2))
+
+
+def epe_forward_bound(flow, mask, preds, scales, weights, eps, q, zero=None):
+    """(ref, S, L, extra) of epe_forward_kernel + epe_finish_kernel: |loss - ref| <= gamma_L S + extra.
+    Per pixel: Upsample(s) (5 roundings each), d, d^2, sum, + eps, sqrt (5), * w_s, sum over scales (2 per scale); then a
+    thread's ceil(HW / (64 * 256)) pixels, * mask, two reductions of 5 + 8 (block) and 64 (finish), the division:
+    L = 15 * scales + ceil(HW / 16384) + 80.  The up-sampled prediction's rounding: for the L2 form (|de/du| <= 1)
+    gamma_5 max |pred| twice; for the q form e is in [s_lo^q, s_hi^q] widened by powf's error, per pixel."""
+    N, _, H, W = flow.shape
+    ref, parts = epe_terms(flow, mask, [p.double() for p in preds], scales, weights, eps, q, zero)
+    m64, f64 = mask.double(), flow.double()
+    msum = m64.sum(dim=(1, 2, 3))
+    L = 15 * len(preds) + math.ceil(H * W / 16384) + 80
+    S = sum(w * (e * m64).sum(dim=(1, 2, 3)) for (u, e), w in zip(parts, weights)) / msum
+    if q < 0:
+        return ref, S, L, 2 * sum(w * gamma(5) * float(p.abs().max()) for p, w in zip(preds, weights))
+    extra = 0
+    for (u, e), p, s, w in zip(parts, preds, scales, weights):
+        _, s_lo, s_hi = epe_q_box(u - f64, epe_delta(p, flow, s, zero), eps)
+        dev = torch.maximum(s_hi ** q * (1 + POWF_REL) - e, e - s_lo ** q * (1 - POWF_REL))
+        extra = extra + w * (dev * m64).sum(dim=(1, 2, 3))
+    return ref, S, L, extra / msum * (1 + gamma(L))
+
+
+def epe_backward_bounds(flow, mask, msum, preds, scales, weights, eps, q, g, zero=None):
+    """Per scale (ref, S, pos, L, gpix) of epe_backward_kernel: |got - ref| <= gamma_L S + pos, gpix the signed per-pixel
+    gradient w g / msum mask de/du whose transposed Upsample(s) is ref.
+    epe_backward_kernel: per lane ceil(cnt / 32) adds of coef * g (coef: 5 roundings, g = d / e: 4), a 5-level shuffle
+    tree, * (w g / msum) (3).
+    L2 form: the direction d / e of a pixel moves by up to 2 |delta d| / e where delta d, the rounding of the fp32
+    up-sampled prediction and difference, is gamma_6 (max |pred| + |flow|).
+    q form: g_c = q s^(q-1) sign(d_c); over the box, |g_c| lies in q [s_hi^(q-1), s_lo^(q-1)] widened by powf's error;
+    where |d_c| <= delta_c the sign is open (uncertainty q (s^(q-1) + s_lo^(q-1))); where d is exactly 0 (zero) so is g."""
+    N, _, H, W = flow.shape
+    ps = [p.double().requires_grad_() for p in preds]
+    with torch.enable_grad():
+        loss, parts = epe_terms(flow, mask, ps, scales, weights, eps, q, zero)
+        refs = torch.autograd.grad(loss, ps, g.double())
+    kn = (g.double().abs() / msum.double()).view(N, 1, 1, 1)
+    ks = (g.double() / msum.double()).view(N, 1, 1, 1)
+    m64, f64 = mask.double(), flow.double()
+    out = []
+    for p, s, w, ref, (u, e) in zip(preds, scales, weights, refs, parts):
+        u, e = u.detach(), e.detach()
+        Hc, Wc = H // s, W // s
+        L = math.ceil((2 * s) ** 2 / 32) + 5 + 9 + 3
+        d = u - f64
+        if q < 0:
+            S = upsample_T(w * kn * m64 * d.abs() / e, s, Hc, Wc)
+            M = p.abs().amax(dim=(1, 2, 3), keepdim=True).double()
+            pos = upsample_T(w * kn * m64 * 2 * gamma(6) * (M + f64.abs()) / e, s, Hc, Wc)
+            gpix = w * ks * m64 * d / e
+        else:
+            delta = epe_delta(p, flow, s, zero)
+            sv, s_lo, s_hi = epe_q_box(d, delta, eps)
+            k = q * sv ** (q - 1)
+            k_lo, k_hi = q * s_hi ** (q - 1) * (1 - POWF_REL), q * s_lo ** (q - 1) * (1 + POWF_REL)
+            unc = torch.where(d.abs() > delta, torch.maximum(k_hi - k, k - k_lo), k + k_hi)
+            unc = torch.where((d == 0) & (delta == 0), torch.zeros_like(unc), unc)
+            S = upsample_T(w * kn * m64 * k * (d != 0), s, Hc, Wc)
+            pos = upsample_T(w * kn * m64 * unc, s, Hc, Wc) * (1 + gamma(L))
+            gpix = w * ks * m64 * k * torch.sign(d)
+        out.append((ref, S, pos, L, gpix))
+    return out
+
+
+def epe_q_controls(flow, mask, msum, preds, scales, weights, eps, q, g, zero, bounds, loss=None):
+    """Near misses of the robust loss, each judged against the bound of the real launch (err / bound, the launch's max):
+    the L2 form in place of the q form; the mask rounded to {0, 1} (where that moves at least 1 % of its sum, as after
+    the augmentation of a sparse mask); sign(0) = +1 in the q-gradient at the pixels where d is
+    exactly 0 (where zero marks some under a nonzero mask).  With loss: the forward's (bounds = epe_forward_bound), else
+    the backward's (bounds = epe_backward_bounds)."""
+    alts = {"L2 form": (mask, -1.0)}
+    if float((mask.round() - mask).abs().sum()) >= 0.01 * float(mask.sum()):
+        alts["mask rounded"] = (mask.round(), q)
+    res = {}
+    for name, (m_alt, q_alt) in alts.items():
+        if loss is not None:
+            ref, S, L, extra = bounds
+            alt = epe_terms(flow, m_alt, [p.double() for p in preds], scales, weights, eps, q_alt, zero)[0]
+            res[name] = judge_bound(alt, ref, S, L, extra)[0]
+        else:
+            alt = epe_backward_bounds(flow, m_alt, msum, preds, scales, weights, eps, q_alt, g, zero)
+            res[name] = max(judge_bound(ar[0], r, S, L, pos)[0] for ar, (r, S, pos, L, _) in zip(alt, bounds))
+    if loss is None and zero is not None and bool((zero[1] & (mask > 0)).any()):
+        s = zero[0]
+        i = list(scales).index(s)
+        r, S, pos, L, _ = bounds[i]
+        N, _, H, W = flow.shape
+        ks = (g.double() / msum.double()).view(N, 1, 1, 1)
+        plus = weights[i] * ks * mask.double() * q * eps ** (q - 1) * zero[1]
+        res["sign(0) = +1"] = judge_bound(r + upsample_T(plus.expand(-1, 2, -1, -1), s, H // s, W // s), r, S, L, pos)[0]
+    return res
+
+
+# ---- image warp (image_warp_bwd.cu): the sampler's slope ---------------------------------------------------------------
+def _gather0(img, yi, xi):
+    """img[n, c, yi, xi] with 0 outside the plane; yi, xi (N, H, W) integer tensors."""
+    N, C, H, W = img.shape
+    ok = ((yi >= 0) & (yi < H) & (xi >= 0) & (xi < W)).unsqueeze(1)
+    idx = (yi.clamp(0, H - 1) * W + xi.clamp(0, W - 1)).reshape(N, 1, -1).expand(N, C, -1)
+    return torch.gather(img.reshape(N, C, -1), 2, idx).view(N, C, *yi.shape[1:]) * ok
+
+
+def sampler_cell_slopes(img, h, v, y0, x0):
+    """d/dh and d/dv (N, C, H, W) of the zero-padded bilinear sample of img at (h, v), taken in the cell with top-left
+    corner (y0, x0) (the fractions h - y0, v - x0 may lie a little outside [0, 1]); their S (the same sums on |corners|);
+    |Delta| = |a - b - c + d|, the slope of d/dh in the column fraction and of d/dv in the row fraction; sum |corners|."""
+    a, b = _gather0(img, y0, x0), _gather0(img, y0, x0 + 1)
+    c, d = _gather0(img, y0 + 1, x0), _gather0(img, y0 + 1, x0 + 1)
+    ly, lx = (h - y0).unsqueeze(1), (v - x0).unsqueeze(1)
+    sy = (1 - lx) * (c - a) + lx * (d - b)
+    sx = (1 - ly) * (b - a) + ly * (d - c)
+    Sy = (1 - lx).abs() * (a.abs() + c.abs()) + lx.abs() * (b.abs() + d.abs())
+    Sx = (1 - ly).abs() * (a.abs() + b.abs()) + ly.abs() * (c.abs() + d.abs())
+    return sy, sx, Sy, Sx, (a - b - c + d).abs(), a.abs() + b.abs() + c.abs() + d.abs()
+
+
+def image_warp_flow_slopes(img, h, v, dh, dv, g, scale, got):
+    """err / bound of g_flow_up ((N, 2, H, W), (y, x)) of image_warp_concat_bwd_kernel against float64, and of the
+    control that takes every slope from the cell above and to the right.  The kernel's position is the float64 (h, v)
+    within (dh, dv); its slope along y is sum_c g_c d sample_c / dh, in the cell of its fp32 position.
+    Bound: the dwy / dwx sums (4 fmas), the channel chain (Ci), * scale (1): gamma_(Ci+6) S; the corner weights 1 - l
+    and 1 - (1 - l) are off by up to 2u absolutely (2u sum |corners|); and the slope along y is linear in the column
+    fraction with slope Delta (continuous across columns), so a column off by dv moves it by |Delta| dv (the larger
+    |Delta| of the cells the column may lie in), and the same with the axes swapped.  The slope along y jumps where
+    h crosses an integer: where floor(h - dh) != floor(h + dh) the element is accepted against either row cell."""
+    Ci = img.shape[1]
+    L = Ci + 6
+    g, ga = g.double(), g.double().abs()
+    img = img.double()
+    ys = (torch.floor(h - dh).long(), torch.floor(h + dh).long())
+    xs = (torch.floor(v - dv).long(), torch.floor(v + dv).long())
+    cells = {(i, j): sampler_cell_slopes(img, h, v, ys[i], xs[j]) for i in (0, 1) for j in (0, 1)}
+    dmax = torch.stack([c[4] for c in cells.values()]).amax(0)
+    cmax = torch.stack([c[5] for c in cells.values()]).amax(0)
+    pos_y = abs(scale) * (ga * (dmax * dv.unsqueeze(1) + 2 * U * cmax)).sum(1)
+    pos_x = abs(scale) * (ga * (dmax * dh.unsqueeze(1) + 2 * U * cmax)).sum(1)
+
+    # the slope along y in either row cell, each in the column cell of v itself (extrapolating a neighbouring column
+    # cell's interpolant across the integer would not be the float64 value); along x the same with the axes swapped
+    y0, x0 = torch.floor(h).long(), torch.floor(v).long()
+    r, refs = [], []
+    for k, pos_k, cand in ((0, pos_y, [sampler_cell_slopes(img, h, v, yy, x0) for yy in ys]),
+                           (1, pos_x, [sampler_cell_slopes(img, h, v, y0, xx) for xx in xs])):
+        best = None
+        for c in cand:
+            ref = scale * (g * c[k]).sum(1)
+            S = abs(scale) * (ga * c[2 + k]).sum(1)
+            rk = _ratio((got[:, k].double() - ref).abs(), gamma(L) * S + pos_k)
+            best = rk if best is None else torch.minimum(best, rk)
+            refs.append((ref, gamma(L) * S + pos_k))
+        r.append(best)
+    rr = torch.stack(r)
+    i = int(torch.argmax(rr))
+    k, e = divmod(i, rr[0].numel())
+    pick = lambda t: float(t.reshape(-1)[e])  # noqa: E731
+    worst = (f"axis {'yx'[k]} elem {e}: h {pick(h):.9g} v {pick(v):.9g} dh {pick(dh):.3g} dv {pick(dv):.3g} got "
+             f"{float(got[:, k].reshape(-1)[e]):.9g} refs " +
+             ", ".join(f"{pick(a):.9g} (bound {pick(b):.3g})" for a, b in refs[2 * k:2 * k + 2]))
+    nominal = sampler_cell_slopes(img, h, v, y0, x0)
+    shifted = sampler_cell_slopes(img, h, v, y0 - 1, x0 + 1)
+    ctl = max(float(_ratio(scale * ((g * shifted[k]).sum(1) - (g * nominal[k]).sum(1)).abs(),
+                           gamma(L) * abs(scale) * (ga * nominal[2 + k]).sum(1) + pos_k).max())
+              for k, pos_k in ((0, pos_y), (1, pos_x)))
+    return float(rr.max()), ctl, worst
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # CPU: the bound accepts the kernels' summation orders and rejects the controls
 # ------------------------------------------------------------------------------------------------------------------
@@ -257,6 +472,172 @@ def test_bound_accepts_emulated_kernel_order_and_rejects_controls():
     assert bool((torch.floor(h) >= H - 1).any())
 
 
+def _emu_upsample(p, s, H, W):
+    """Upsample(s) of p (N, C, H / s, W / s) in the kernels' fp32 order (upsample_at, sampling.cuh), one rounding per
+    operation."""
+    Hc, Wc = p.shape[2:]
+    y, x = torch.arange(H), torch.arange(W)
+    y0, x0 = y // s, x // s
+    y1, x1 = (y0 + 1).clamp(max=Hc - 1), (x0 + 1).clamp(max=Wc - 1)
+    wy = ((y - y0 * s).float() / s).view(H, 1)
+    wx = ((x - x0 * s).float() / s).view(1, W)
+    a, b = p[:, :, y0][:, :, :, x0], p[:, :, y0][:, :, :, x1]
+    c, d = p[:, :, y1][:, :, :, x0], p[:, :, y1][:, :, :, x1]
+    top, bot = a + (b - a) * wx, c + (d - c) * wx
+    return top + (bot - top) * wy
+
+
+def _emu_lanes(v):
+    """The sum of v (fp32, 1-D) as 32 lanes add it (lane l takes elements l, l + 32, ...) and a xor shuffle tree."""
+    lanes = torch.zeros(32)
+    for k in range(0, v.numel(), 32):
+        blk = v[k:k + 32]
+        lanes[:blk.numel()] = lanes[:blk.numel()] + blk
+    idx = torch.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        lanes = lanes + lanes[idx ^ o]
+    return lanes[0]
+
+
+def _emu_epe(flow, mask, preds, scales, weights, eps, q, gl):
+    """epe_forward_kernel + epe_finish_kernel and epe_backward_kernel (loss.cu) for one sample, H W <= 16384, in fp32."""
+    N, _, H, W = flow.shape
+    assert N == 1 and H * W <= 16384
+    eps32, q32 = torch.tensor(eps, dtype=torch.float32), torch.tensor(q, dtype=torch.float32)
+    ups = [_emu_upsample(p, s, H, W) for p, s in zip(preds, scales)]
+    e = torch.zeros((H, W))
+    kg = []
+    for u, w in zip(ups, weights):
+        d = u[0] - flow[0]
+        sv = d[0].abs() + d[1].abs() + eps32
+        e = e + torch.tensor(w, dtype=torch.float32) * sv ** q32
+        k = q32 * sv ** (q32 - 1)
+        kg.append(torch.stack([torch.where(d[c] > 0, k, torch.where(d[c] < 0, -k, torch.zeros_like(k))) for c in (0, 1)]))
+    # forward: thread t of block b holds pixel 256 b + t; warp trees, the block's warps in order, the blocks in order
+    parts = torch.zeros((2, 64 * 256))
+    parts[0, :H * W], parts[1, :H * W] = (e * mask[0, 0]).reshape(-1), mask[0, 0].reshape(-1)
+    parts = parts.view(2, 64, 8, 32)
+    idx = torch.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        parts = parts + parts[..., idx ^ o]
+    num, den = torch.zeros(()), torch.zeros(())
+    for b in range(64):
+        bn, bd = torch.zeros(()), torch.zeros(())
+        for wp in range(8):
+            bn, bd = bn + parts[0, b, wp, 0], bd + parts[1, b, wp, 0]
+        num, den = num + bn, den + bd
+    loss = (num / den).view(1)
+    # backward: one warp per coarse pixel over the full-resolution pixels that read it
+    grads = []
+    for p, s, w, g in zip(preds, scales, weights, kg):
+        Hc, Wc = p.shape[2:]
+        out = torch.zeros_like(p)
+        kk = torch.tensor(w, dtype=torch.float32) * gl[0] / den
+        for i in range(Hc):
+            for j in range(Wc):
+                ys = torch.arange(max(s * (i - 1), 0), min(s * (i + 1), H))
+                xs = torch.arange(max(s * (j - 1), 0), min(s * (j + 1), W))
+                y0, x0 = ys // s, xs // s
+                y1, x1 = (y0 + 1).clamp(max=Hc - 1), (x0 + 1).clamp(max=Wc - 1)
+                wy, wx = (ys - y0 * s).float() / s, (xs - x0 * s).float() / s
+                cy = torch.where(y0 == i, 1 - wy, torch.zeros_like(wy)) + torch.where(y1 == i, wy, torch.zeros_like(wy))
+                cx = torch.where(x0 == j, 1 - wx, torch.zeros_like(wx)) + torch.where(x1 == j, wx, torch.zeros_like(wx))
+                coef = (cy.view(-1, 1) * cx.view(1, -1)) * mask[0, 0][ys][:, xs]
+                for c in (0, 1):
+                    out[0, c, i, j] = _emu_lanes((coef * g[c][ys][:, xs]).reshape(-1)) * kk
+        grads.append(out)
+    return loss, den.view(1), grads
+
+
+def _emu_image_warp_flow(img, fy, fx, g, scale):
+    """grad_flow_up of image_warp_concat_bwd_kernel (sampler_corners, sample_backward) in fp32, given the kernel's fp32
+    displacements fy, fx (N, H, W)."""
+    N, C, H, W = img.shape
+    yr = torch.arange(H, dtype=torch.float32).view(1, H, 1) + fy
+    xr = torch.arange(W, dtype=torch.float32).view(1, 1, W) + fx
+    y0, x0 = torch.floor(yr), torch.floor(xr)
+    wx0, wy0 = 1 - (xr - x0), 1 - (yr - y0)
+    wx1, wy1 = 1 - wx0, 1 - wy0
+    y0, x0 = y0.long(), x0.long()
+    xin = [(x0 + k >= 0) & (x0 + k <= W - 1) for k in (0, 1)]
+    yin = [(y0 + k >= 0) & (y0 + k <= H - 1) for k in (0, 1)]
+    z = torch.zeros_like(wx0)
+    corners = [(0, 0), (0, 1), (1, 0), (1, 1)]
+    dwx = [torch.where(xin[b] & yin[a], (wy0 if a == 0 else wy1) * (1 if b else -1), z) for a, b in corners]
+    dwy = [torch.where(xin[b] & yin[a], (wx0 if b == 0 else wx1) * (1 if a else -1), z) for a, b in corners]
+    vals = [_gather0(img, y0 + a, x0 + b) for a, b in corners]
+    ax, ay = torch.zeros_like(z), torch.zeros_like(z)
+    for c in range(C):
+        sx, sy = torch.zeros_like(z), torch.zeros_like(z)
+        for t in range(4):
+            sx = sx + dwx[t] * vals[t][:, c]
+            sy = sy + dwy[t] * vals[t][:, c]
+        ax, ay = ax + g[:, c] * sx, ay + g[:, c] * sy
+    return torch.stack([ay * scale, ax * scale], 1)
+
+
+def test_bound_accepts_emulated_q_loss_and_flow_slope_and_rejects_controls():
+    """The robust loss (q = 0.4, eps = 1e-8) and the image warp's flow gradient: the bounds accept the kernels' fp32
+    arithmetic at the edges (d within delta of 0, d exactly 0 so that s = eps, positions one ulp either side of an
+    integer) and reject each near miss by CONTROL_MARGIN."""
+    g = torch.Generator().manual_seed(12)
+    # ---- MultiscaleEpe, q form -------------------------------------------------------------------------------------
+    H, W, scales, weights, q, eps = 32, 48, (8, 4), (0.08, 0.32), 0.4, _f32(1e-8)
+    preds = [torch.randn((1, 2, H // s, W // s), generator=g) * 2 for s in scales]
+    flow = torch.randn((1, 2, H, W), generator=g) * 2
+    flow[..., W // 2:] *= 3                 # larger errors where the mask is below 1/2: rounding it moves the mean
+    mask = torch.rand((1, 1, H, W), generator=g) * 0.5
+    mask[..., :W // 2] += 0.5
+    mask[mask < 0.1] = 0
+    mask[:, :, :6, :] = 1.0
+    u4 = _emu_upsample(preds[1], 4, H, W)
+    zero = torch.zeros((1, 1, H, W), dtype=torch.bool)
+    zero[:, :, 16:28, 8:28] = True                               # d exactly 0 at scale 4: s = eps
+    flow = torch.where(zero, u4, flow)
+    flow[:, :, :6, ::3] = torch.nextafter(u4[:, :, :6, ::3], torch.tensor(float("inf")))   # d one ulp from 0
+    flow[:, :, :6, 1::3] = torch.nextafter(u4[:, :, :6, 1::3], torch.tensor(-float("inf")))
+    gl = torch.tensor([1.0])
+    loss, msum, grads = _emu_epe(flow, mask, preds, scales, weights, eps, q, gl)
+    zero_s = (4, zero)
+    fb = epe_forward_bound(flow, mask, preds, scales, weights, eps, q, zero_s)
+    assert judge_bound(loss, *fb)[0] <= 1.0
+    bb = epe_backward_bounds(flow, mask, msum, preds, scales, weights, eps, q, gl, zero_s)
+    for got, (ref, S, pos, L, _) in zip(grads, bb):
+        assert judge_bound(got, ref, S, L, pos)[0] <= 1.0
+    # the near-zero band really is within delta of 0 there (its sign is open), the patch really has s = eps
+    d4 = torch_ref.upsample(preds[1].double(), 4) - flow.double()
+    near = (d4.abs() <= epe_delta(preds[1], flow, 4))[:, :, :6]
+    assert bool(near[..., 0::3].all() and near[..., 1::3].all())
+    assert bool((_emu_upsample(preds[1], 4, H, W) - flow)[zero.expand(-1, 2, -1, -1)].eq(0).all())
+    fc = epe_q_controls(flow, mask, None, preds, scales, weights, eps, q, None, zero_s, fb, loss=loss)
+    bc = epe_q_controls(flow, mask, msum, preds, scales, weights, eps, q, gl, zero_s, bb)
+    assert set(fc) == {"L2 form", "mask rounded"} and set(bc) == {"L2 form", "mask rounded", "sign(0) = +1"}
+    for name, r in list(fc.items()) + list(bc.items()):
+        assert r >= CONTROL_MARGIN, (name, r)
+
+    # ---- image warp: g_flow_up at fp32 positions on, and one ulp either side of, integers ---------------------------
+    N, C, H, W, scale = 1, 3, 12, 16, 20.0
+    img = torch.randn((N, C, H, W), generator=g)
+    gout = torch.randn((N, C, H, W), generator=g)
+    fy = torch.randn((N, H, W), generator=g) * 3
+    fx = torch.randn((N, H, W), generator=g) * 3
+    ys = torch.arange(H, dtype=torch.float32).view(1, H, 1)
+    xs = torch.arange(W, dtype=torch.float32).view(1, 1, W)
+    ty, tx = torch.round(ys + fy), torch.round(xs + fx)         # the nearest integer positions
+    fy[:, 0::3] = (ty - ys)[:, 0::3]                                # on an integer
+    fy[:, 1::3] = torch.nextafter(ty - ys, torch.tensor(float("inf")))[:, 1::3]        # one ulp either side
+    fy[:, 2::3] = torch.nextafter(ty - ys, torch.tensor(-float("inf")))[:, 2::3]
+    fx[:, :, 0::2] = torch.nextafter(tx - xs, torch.tensor(-float("inf")))[:, :, 0::2]
+    fy[:, 5, :] = 2 - 2.0 ** -22                    # 5 + (2 - 2^-22) rounds to 7 in fp32: the float64 cell is 6
+    got = _emu_image_warp_flow(img, fy, fx, gout, scale)
+    h, v = ys.double() + fy.double(), xs.double() + fx.double()
+    dh, dv = 2.0 ** -20 * (ys.double() + fy.double().abs() + 1), 2.0 ** -20 * (xs.double() + fx.double().abs() + 1)
+    assert bool((torch.floor(h) != torch.floor(ys + fy).double()).any())     # the fp32 position took the other cell
+    r, ctl, _ = image_warp_flow_slopes(img, h, v, dh, dv, gout, scale, got)
+    assert r <= 1.0, r
+    assert ctl >= CONTROL_MARGIN, ctl
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # GPU: the backward recorder
 # ------------------------------------------------------------------------------------------------------------------
@@ -267,6 +648,9 @@ class BackwardRecorder:
     def __init__(self, monkeypatch, run):
         self.run, self.rows, self.failures, self.controls, self.calls = run, [], [], {}, []
         self.capture = None
+        self.exact_zero = None      # (scale, bool (N, 1, H, W)): label pixels where the loss kernel's d is exactly 0
+        # q form, per scale: (scale, elements with pos > gamma_L S, elements with pos >= S > 0 or pos > S = 0, elements)
+        self.epe_vacuous = []
         for cls, fn in ((ops._CorrelationFn, self.correlation), (ops._WarpMaskFn, self.warp_mask),
                         (ops._ImageWarpConcatFn, self.image_warp), (losses._MultiscaleEpeFn, self.epe),
                         (ops._Conv3x3TrainFn, self.conv)):
@@ -522,7 +906,9 @@ class BackwardRecorder:
         torch.cuda.synchronize()
         captured, self.capture = self.capture, None
         gi2 = res[1]
-        gmu = captured[-1] if res[3] is not None else None     # the mask's input of the transposed Upsample(4)
+        # the flow's and the mask's inputs of the transposed Upsample(4), in that order
+        gfu = captured[0] if res[2] is not None else None
+        gmu = captured[-1] if res[3] is not None else None
         i2, fq, mq = ctx.saved_tensors
         scale = ctx.scale
         N, Ci, H, W = i2.shape
@@ -535,7 +921,10 @@ class BackwardRecorder:
                 disp = torch_ref.upsample(fq[n:n + 1].double(), 4) * scale
                 h, v = ys + disp[:, 0], xs + disp[:, 1]
                 # the kernel's positions: fl(p + fl(Upsample(4)(flow) * scale)), off by up to 2^-20 (|p| + |d| + 1) px
+                # and the fp32 Upsample's own rounding, gamma_8 max |flow| (two interpolations), times the scale
+                up_err = gamma(8) * abs(scale) * float(fq[n].abs().max())
                 dh, dv = 2.0 ** -20 * (ys + disp[:, 0].abs() + 1), 2.0 ** -20 * (xs + disp[:, 1].abs() + 1)
+                dh_f, dv_f = dh + up_err, dv + up_err
                 x64 = i2[n:n + 1].double().requires_grad_()
                 grid = torch.stack([v / ((W - 1) / 2) - 1, h / ((H - 1) / 2) - 1], dim=-1)
                 ref = torch.autograd.grad(tF.grid_sample(x64, grid, align_corners=True), x64, g[:, :Ci])[0]
@@ -548,6 +937,15 @@ class BackwardRecorder:
                 if gi2 is not None:
                     r, rus, _ = judge_bound(gi2[n:n + 1], ref, S, cnt + 5, pos)
                     wi["g_im2"] = max(wi.get("g_im2", 0.0), r)
+                if gfu is not None:
+                    with torch.no_grad():
+                        r, ctl, worst = image_warp_flow_slopes(i2[n:n + 1], h, v, dh_f, dv_f, g[:, :Ci], scale,
+                                                               gfu[n:n + 1])
+                    wi["g_flow_up"] = max(wi.get("g_flow_up", 0.0), r)
+                    if r > 1.0:
+                        self.failures.append(f"{self.run}: image warp g_flow_up n={n}: {worst}")
+                    if n == 0 and "image warp" not in self.controls:
+                        self._control("image warp", f"{N}x{Ci}x{H}x{W}", {"cell above right": ctl})
                 # g_mask_up = g * s (1 - s) (3 roundings); s from an fp32 Upsample(4) (gamma_5 max |mask_q|) and __expf
                 m = torch_ref.upsample(mq[n:n + 1].double(), 4)
                 s, es = sigmoid_error(m)
@@ -561,41 +959,21 @@ class BackwardRecorder:
             self._row("image_warp_bwd", k, f"{N}x{Ci}x{H}x{W}", r, 0.0)
         return res
 
-    # ---- MultiscaleEpe ------------------------------------------------------------------------------------------------
-    @staticmethod
-    def _epe_terms(flow, mask, preds, scales, weights, eps):
-        """float64 per-sample loss; per scale the up-sampled prediction u and the per-pixel EPE e."""
-        f64, m64 = flow.double(), mask.double()
-        loss, parts = 0, []
-        for p, s, w in zip(preds, scales, weights):
-            u = torch_ref.upsample(p, s)
-            e = torch.sqrt(((u - f64) ** 2).sum(1, keepdim=True) + eps)
-            loss = loss + w * (e * m64).sum(dim=(1, 2, 3))
-            parts.append((u, e))
-        return loss / m64.sum(dim=(1, 2, 3)), parts
-
+    # ---- MultiscaleEpe: epe_forward_bound, epe_backward_bounds --------------------------------------------------------
     def epe_forward(self, ctx, flow, mask, scales, weights, eps, q, *preds):
         loss = self.orig_epe_fwd(ctx, flow, mask, scales, weights, eps, q, *preds)
         torch.cuda.synchronize()
+        N, _, H, W = flow.shape
         with torch.no_grad():
-            assert q < 0
-            ref, parts = self._epe_terms(flow, mask, [p.double() for p in preds], scales, weights, _f32(eps))
-            m64 = mask.double()
-            N, _, H, W = flow.shape
-            # per pixel: Upsample(s) (5 roundings each), d, d^2, sum, + eps, sqrt (5), * w_s, sum over scales (2 per
-            # scale); then a thread's ceil(HW / (64 * 256)) pixels, * mask, two reductions of 5 + 8 (block) and 64
-            # (finish), the division: L = 15 * scales + ceil(HW / 16384) + 80; the up-sampled prediction's rounding
-            # gamma_5 max |pred| moves e by as much
-            L = 15 * len(preds) + math.ceil(H * W / 16384) + 80
-            S = sum(w * (e * m64).sum(dim=(1, 2, 3)) for (u, e), w in zip(parts, weights)) / m64.sum(dim=(1, 2, 3))
-            extra = sum(w * gamma(5) * float(p.abs().max()) for p, w in zip(preds, weights))
-            r, rus, _ = judge_bound(loss, ref, S, L, extra * 2)
-        self._row("epe_fwd", f"{len(preds)} scales", f"{N}x{H}x{W}", r, rus)
+            bounds = epe_forward_bound(flow, mask, preds, scales, weights, _f32(eps), q, self.exact_zero)
+            r, rus, _ = judge_bound(loss, *bounds)
+            if q >= 0:
+                for kind, ratio in epe_q_controls(flow, mask, None, preds, scales, weights, _f32(eps), q, None,
+                                                  self.exact_zero, bounds, loss=loss).items():
+                    self._control(f"epe {kind}", f"fwd {N}x{H}x{W}", {"fwd": ratio})
+        self._row("epe_fwd", f"{len(preds)} scales" + (f" q={q:g}" if q >= 0 else ""), f"{N}x{H}x{W}", r, rus)
         return loss
 
-    # epe_backward_kernel: per lane ceil(cnt / 32) adds of coef * g (coef: 5 roundings, g = d / e: 4), a 5-level
-    # shuffle tree, * (w g / msum) (3).  The direction d / e of a pixel moves by up to 2 |delta d| / e where delta d, the
-    # rounding of the fp32 up-sampled prediction and difference, is gamma_6 (max |pred| + |flow|)
     def epe(self, orig, ctx, g):
         res = orig(ctx, g)
         torch.cuda.synchronize()
@@ -604,28 +982,24 @@ class BackwardRecorder:
         grads = res[6:]
         N, _, H, W = flow.shape
         with torch.no_grad():
-            ps = [p.double().requires_grad_() for p in preds]
-            with torch.enable_grad():
-                loss, parts = self._epe_terms(flow, mask, ps, scales, weights, _f32(eps))
-                refs = torch.autograd.grad(loss, ps, g.double())
-            kn = (g.double().abs() / msum.double()).view(N, 1, 1, 1)
-            m64, f64 = mask.double(), flow.double()
-            for s_i, (p, s, w, got, ref) in enumerate(zip(preds, scales, weights, grads, refs)):
-                u, e = (t.detach() for t in parts[s_i])
+            bounds = epe_backward_bounds(flow, mask, msum, preds, scales, weights, _f32(eps), q, g, self.exact_zero)
+            for s, got, (ref, S, pos, L, gpix) in zip(scales, grads, bounds):
                 Hc, Wc = H // s, W // s
-                dirn = (u - f64).abs() / e
-                S = upsample_T(w * kn * m64 * dirn, s, Hc, Wc)
-                M = p.abs().amax(dim=(1, 2, 3), keepdim=True).double()
-                pos = upsample_T(w * kn * m64 * 2 * gamma(6) * (M + f64.abs()) / e, s, Hc, Wc)
-                L = math.ceil((2 * s) ** 2 / 32) + 5 + 9 + 3
                 r, rus, _ = judge_bound(got, ref, S, L, pos)
-                self._row("epe_bwd", f"x{s}", f"{N}x2x{Hc}x{Wc}", r, rus)
+                self._row("epe_bwd", f"x{s}" + (f" q={q:g}" if q >= 0 else ""), f"{N}x2x{Hc}x{Wc}", r, rus)
+                if q >= 0:     # elements whose bound the box of the fp32 d dominates / leaves no larger than S
+                    self.epe_vacuous.append((s, int((pos > gamma(L) * S).sum()), int(((pos >= S) & (pos > 0)).sum()),
+                                             pos.numel()))
                 if s == max(scales) and "epe x%d" % s not in self.controls:
-                    gd = w * kn * m64 * (u - f64) / e
+                    gd = gpix.clone()
                     gd[:, :, s * (Hc - 1):] = 0
                     gd[:, :, :, s * (Wc - 1):] = 0
                     self._control(f"epe x{s}", f"{N}x2x{Hc}x{Wc}",
                                   {"clamped": judge_bound(upsample_T(gd, s, Hc, Wc), ref, S, L, pos)[0]})
+            if q >= 0:
+                for kind, ratio in epe_q_controls(flow, mask, msum, preds, scales, weights, _f32(eps), q, g,
+                                                  self.exact_zero, bounds).items():
+                    self._control(f"epe {kind}", f"bwd {N}x{H}x{W}", {"bwd": ratio})
         return res
 
     # ---- cuDNN convolution backward: wiring only ----------------------------------------------------------------------
@@ -644,16 +1018,26 @@ class BackwardRecorder:
                     return torch.autograd.grad(tF.conv2d(xr, wr, stride=s, padding=d, dilation=d), (xr, wr), gv)
             rx, rw = grads(x.double(), weight.double(), gm)
             sx, sw = grads(x.double().abs(), weight.double().abs(), gm.abs())
-            worst = 0.0
+
+            def wiring_bound(S):
+                # cuDNN's transform-based algorithms (Winograd, FFT) do not keep an exact zero exact: a weight tap that
+                # only meets zero data (the outer displacement planes of a 5-row level-6 correlation) comes back as
+                # rounding noise of the whole sum, so the bound has a floor at 2^-8 of the tensor's largest S
+                return EPS_WIRING * (S + 2.0 ** -8 * S.max())
+            worst, zero_err = 0.0, 0.0
             for got, ref, S in ((gx, rx, sx), (gw, rw, sw), (gb, gm.sum(dim=(0, 2, 3)), gm.abs().sum(dim=(0, 2, 3)))):
                 if got is not None:
-                    worst = max(worst, float(_ratio((got.double() - ref).abs(), EPS_WIRING * S).max()))
+                    err = (got.double() - ref).abs()
+                    worst = max(worst, float(_ratio(err, wiring_bound(S)).max()))
+                    if bool((S == 0).any()) and float(S.max()) > 0:
+                        zero_err = max(zero_err, float(err[S == 0].max() / S.max()))
             if dil > 1 and "conv wiring" not in self.controls and gx is not None:
                 cx, _ = grads(x.double(), weight.double(), gm, d=1) if stride == 1 else (None, None)
                 if cx is not None:
                     self._control("conv wiring", f"d={dil} {tuple(x.shape)}",
-                                  {"dilation 1": float(_ratio((cx - rx).abs(), EPS_WIRING * sx).max())})
-        self._row("conv_bwd", f"d={dil} s={stride}", "x".join(map(str, x.shape)), worst, 0.0)
+                                  {"dilation 1": float(_ratio((cx - rx).abs(), wiring_bound(sx)).max())})
+        # err_us of this row: the largest error where S = 0, relative to the largest S
+        self._row("conv_bwd", f"d={dil} s={stride}", "x".join(map(str, x.shape)), worst, zero_err)
         return res
 
     def report(self):
@@ -665,6 +1049,9 @@ class BackwardRecorder:
                 where, rs = entry[-2], entry[-1]
                 print(f"{self.run:13s} control {kind:14s} on {where}: " +
                       ", ".join(f"{k} err/bound={v:.3g}" for k, v in rs.items()))
+        for s, n_dom, n_vac, n in self.epe_vacuous:
+            print(f"{self.run:13s} epe_bwd x{s} q form, of {n} elements: pos > gamma_L S at {n_dom} ({n_dom / n:.2e}), "
+                  f"pos >= S at {n_vac} ({n_vac / n:.2e})")
 
 
 RUNS = {   # run: (model class, batch, H, W, image seed, label seed, masked rows from the bottom, deterministic)
@@ -730,6 +1117,7 @@ def test_every_backward_launch_of_the_benchmarked_step_against_float64(run, monk
     if cascade:
         assert any(r["op"] == "warp_bwd" and r["name"].startswith("F=196 up=1") for r in bwd.rows)
         assert any(r["op"] == "image_warp_bwd" for r in bwd.rows)
+        assert any(r["op"] == "image_warp_bwd" and r["name"] == "g_flow_up" for r in bwd.rows)
     if det:
         assert bwd.calls.count("mfn_warp_mask_backward_det") == 4
         atomic = {"mfn_warp_mask_backward", "mfn_deformable_conv_backward", "mfn_bilinear_sampler_backward",
@@ -737,7 +1125,8 @@ def test_every_backward_launch_of_the_benchmarked_step_against_float64(run, monk
         assert not atomic & set(bwd.calls), sorted(atomic & set(bwd.calls))
 
     # sensitivity: every control fails the bound by CONTROL_MARGIN on its launch
-    want = {"corr md=4", "corr leaky", "upsample x2", "warp", "epe x64", "conv wiring"} | ({"corr md=2"} if cascade else set())
+    want = {"corr md=4", "corr leaky", "upsample x2", "warp", "epe x64", "conv wiring"} | \
+        ({"corr md=2", "image warp"} if cascade else set())
     assert want <= set(bwd.controls), sorted(bwd.controls)
     for kind, lst in bwd.controls.items():
         for entry in lst:

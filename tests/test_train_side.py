@@ -260,6 +260,8 @@ def _cuda(a):
     (True, True, 2, (64, 96), (48, 80)),
     (True, False, 4, (96, 128), (64, 112)),
     (False, True, 2, (384, 512), (320, 448)),          # FlyingChairs shapes of main.py (orig 384x512 -> target 320x448)
+    (True, False, 2, (370, 1224), (320, 896)),         # KITTI crops, a per-pixel (sparse) mask
+    (True, True, 2, (436, 1024), (384, 768)),          # Sintel / Things3D crops
 ])
 def test_geometry_augment_parity(uint8, bcast, N, orig, target):
     from maskflownet_b200 import augment
@@ -523,7 +525,7 @@ class _TinyNet(torch.nn.Module):
         return preds, [torch.sigmoid(tF.avg_pool2d(y[:, 2:3], 4))], None
 
 
-def _cpu_pipeline(monkeypatch):
+def _cpu_pipeline(monkeypatch, **kw):
     from maskflownet_b200 import network, ops, pipeline
     from oracle import cref, prepost_ref, torch_ref
     t = torch.from_numpy
@@ -534,7 +536,7 @@ def _cpu_pipeline(monkeypatch):
         prepost_ref.postprocess(p.numpy(), H, W, flip_channels, is_flow)))
     monkeypatch.setattr(ops, "grid_generator_warp", lambda f: t(cref.grid_generator_warp(f.numpy())))
     monkeypatch.setattr(ops, "bilinear_sampler", lambda d, g: t(cref.bilinear_sampler(d.numpy(), g.numpy())))
-    return pipeline.PipelineFlownet(device="cpu", lr_schedule=[(2, 1e-4), (5, 5e-5)])
+    return pipeline.PipelineFlownet(device="cpu", lr_schedule=[(2, 1e-4), (5, 5e-5)], **kw)
 
 
 def test_pipeline_host_plumbing_on_cpu(monkeypatch):
@@ -574,6 +576,36 @@ def test_pipeline_host_plumbing_on_cpu(monkeypatch):
     assert np.allclose(res[0][0], flow[0].permute(1, 2, 0).flip(-1).numpy()) and warp.shape == (1, 3, Hs, Ws)
     with pytest.raises(Exception):
         pipe.fix_head()                      # only the cascade has a head to freeze
+
+
+@pytest.mark.parametrize("q", [None, 0.4])
+def test_pipeline_passes_the_robust_loss_settings_to_multiscale_epe_on_cpu(monkeypatch, q):
+    """The KITTI and Sintel fine-tuning configs set q: 0.4; the reference's pipeline hands it to MultiscaleEpe with
+    eps = 1e-8 (network/pipeline.py).  train_batch must call losses.multiscale_epe so, with the pipeline's strides and
+    weights, and train on what it returns."""
+    from maskflownet_b200 import losses
+    pipe = _cpu_pipeline(monkeypatch, q=q)
+    seen = []
+    real = losses.multiscale_epe
+
+    def spy(flow, mask, preds, **kw):
+        seen.append(kw)
+        return real(flow, mask, preds, **kw)
+    monkeypatch.setattr(losses, "multiscale_epe", spy)
+    rng = np.random.default_rng(2)
+    n, H, W = 2, 128, 192
+
+    def geo(i1, i2, fl, mk):
+        return i1.float() / 255, i2.float() / 255, fl.clone(), (mk.float() / 255).expand(n, 1, H, W).contiguous()
+    img1 = rng.integers(0, 256, (n, 3, H, W), dtype=np.uint8)
+    img2 = rng.integers(0, 256, (n, 3, H, W), dtype=np.uint8)
+    label = (rng.standard_normal((n, 2, H, W)) * 2).astype(np.float32)
+    w0 = pipe.network.conv.weight.detach().clone()
+    out = pipe.train_batch(img1, img2, label, geo, lambda a, b: (a, b))
+    assert len(seen) == 1
+    assert seen[0]["q"] == q and seen[0]["eps"] == 1e-8
+    assert list(seen[0]["scales"]) == [64, 32, 16, 8, 4] and list(seen[0]["weights"]) == list(losses.WEIGHTS)
+    assert np.isfinite(out["epe"]) and not torch.equal(pipe.network.conv.weight, w0)
 
 
 def test_pipeline_load_head_and_fix_head_on_cpu(tmp_path):
