@@ -352,6 +352,24 @@ MFN_API int mfn_flow_to_color(const float* flow_xy, unsigned char* rgb, float* r
                               float max_radius, int bgr, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Forward-backward consistency check (Sundaram, Brox and Keutzer, ECCV 2010): which pixels of each image of a pair have
+ * no consistent match in the other.
+ *   flow_fw, flow_bw (N,H,W,2) float32, (x,y) in pixels: the flows image 1 -> image 2 and image 2 -> image 1, in the
+ *   layout mfn_postprocess_forward writes; 8-byte aligned.
+ *   occ_fw, occ_bw (N,H,W) uint8 out, 1 = occluded: the pixels of image 1 (occ_fw) / image 2 (occ_bw) that fail the test.
+ * Per pixel (n,y,x) of the forward direction, (u,v) = flow_fw[n,y,x], target (qx,qy) = (x+u, y+v) in float32:
+ *   outside 0 <= qx <= W-1, 0 <= qy <= H-1 (NaN included) -> 1; else (bu,bv) = flow_bw sampled bilinearly at (qx,qy)
+ *   (corners floor(q) and min(floor(q)+1, extent-1), weights q - floor(q)) and
+ *   occ = !((u+bu)^2 + (v+bv)^2 <= rhs && rhs finite), rhs = alpha (u^2 + v^2 + bu^2 + bv^2) + beta: NaN or inf
+ *   anywhere gives 1.
+ * The backward direction is the same with the roles swapped.  alpha = 0.01, beta = 0.5 are the paper's constants.
+ * One launch covers both directions; no atomics (deterministic), no allocation, capture-safe.  A null pointer, an extent
+ * below 1, a misaligned flow, or a negative or non-finite alpha / beta returns MFN_ERR_INVALID_ARG.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API int mfn_flow_consistency(const float* flow_fw, const float* flow_bw, unsigned char* occ_fw, unsigned char* occ_bw,
+                                 int N, int H, int W, float alpha, float beta, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Deterministic mode: bit-reproducible variants of the entry points whose default kernels accumulate with fp32 atomics
  * (the scatter of a bilinear sample's gradient to its four corners, per-CTA weight partials, per-slice plane sums).  Same
  * arguments and results as the counterpart named without _det, plus a caller-owned workspace `det_ws` of `det_ws_bytes`

@@ -39,6 +39,7 @@ SIGNATURES = {
     "mfn_preprocess_forward": [_f, _f, _i, _f, _f, _f, _i, _i, _i, _i, _i, _i, _f],
     "mfn_postprocess_forward": [_f, _f, _i, _i, _i, _i, _i, _i, _i, _i, _f],
     "mfn_flow_to_color": [_f, _f, _f, _i, _i, _i, _fl, _i, _f],
+    "mfn_flow_consistency": [_f, _f, _f, _f, _i, _i, _i, _fl, _fl, _f],
     "mfn_warp_mask_backward_det": [_f] * 14 + [_i] * 5 + [_fl, _fl, _fl, _i, _f, _ll, _f],
     "mfn_deformable_conv_backward_det": [_f] * 8 + [_i] * 6 + [_f, _ll, _f],
     "mfn_bilinear_sampler_backward_det": [_f] * 5 + [_i] * 6 + [_f, _ll, _f],

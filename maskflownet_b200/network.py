@@ -42,6 +42,11 @@ def _conv(cin, cout, k=3, s=1, p=1, d=1):
     return nn.Conv2d(cin, cout, k, s, p, d)
 
 
+def _swap_halves(t: torch.Tensor, n: int) -> torch.Tensor:
+    """[t[n:]; t[:n]] of a (2n, ...) batch, in a new contiguous tensor: the second images of the reversed pairs."""
+    return torch.cat([t[n:], t[:n]], dim=0)
+
+
 def msra_prelu_init_(module: nn.Module, slope: float = SLOPE, seed: Optional[int] = None) -> None:
     """MSRAPrelu(factor_type='avg', slope) for weights, zeros for biases -- the reference's initialiser
     (network/pipeline.py:26)."""
@@ -221,20 +226,37 @@ class _FlowNetBase(nn.Module):
             feats.append(x)
         return feats  # [c?1 .. c?6]
 
-    def _pyramid_pair(self, im1, im2, names):
+    @staticmethod
+    def _joined(im1, im2):
+        """[im1; im2] as one (2N, ...) batch: a view when im1 and im2 are the two adjacent halves of one buffer
+        (ops.preprocess), else a copy."""
+        n = im1.shape[0]
+        if (im1.is_contiguous() and im2.is_contiguous() and im1.shape == im2.shape and im1.dtype == im2.dtype
+                and im1.untyped_storage().data_ptr() == im2.untyped_storage().data_ptr()
+                and im2.storage_offset() == im1.storage_offset() + im1.numel()):
+            return im1.view(-1).as_strided((2 * im1.numel(),), (1,)).view((2 * n,) + tuple(im1.shape[1:]))
+        return torch.cat([im1, im2], dim=0)
+
+    def _pyramid_pair(self, im1, im2, names, bidirectional=False):
         """Both images through the shared pyramid; inference batches them into one pass (half the launches).  When im1 and
-        im2 are the two adjacent halves of one buffer (ops.preprocess), that buffer is the batch: no copy."""
+        im2 are the two adjacent halves of one buffer (ops.preprocess), that buffer is the batch: no copy.
+        bidirectional (inference only): the pairs (im1 -> im2) then (im2 -> im1) from the same pass -- c1 is the whole
+        2N batch [f(im1); f(im2)] and c2 its halves swapped, [f(im2); f(im1)], one copy per level from level 2 on (no
+        consumer reads level 1 of c2, which is None)."""
         if self._fast(im1):
             n = im1.shape[0]
-            if (im1.is_contiguous() and im2.is_contiguous() and im1.shape == im2.shape and im1.dtype == im2.dtype
-                    and im1.untyped_storage().data_ptr() == im2.untyped_storage().data_ptr()
-                    and im2.storage_offset() == im1.storage_offset() + im1.numel()):
-                x = im1.view(-1).as_strided((2 * im1.numel(),), (1,)).view((2 * n,) + tuple(im1.shape[1:]))
-            else:
-                x = torch.cat([im1, im2], dim=0)
-            f = self._pyramid(x, names)
+            f = self._pyramid(self._joined(im1, im2), names)
+            if bidirectional:
+                return f, [None] + [_swap_halves(t, n) for t in f[1:]]
             return [t[:n] for t in f], [t[n:] for t in f]
         return self._pyramid(im1, names), self._pyramid(im2, names)
+
+    def _check_bidirectional(self, im1, im2):
+        if not self._fast(im1):
+            raise ops.MaskflowError("bidirectional=True is an inference feature: it needs CUDA inputs, use_tc_conv and no "
+                                    "autograd recording (call it under torch.no_grad())")
+        if im1.shape != im2.shape:
+            raise ops.MaskflowError(f"bidirectional: im1 {tuple(im1.shape)} and im2 {tuple(im2.shape)} differ")
 
     def _dense(self, lvl, x):
         """x = concat(leaky(conv_i(x)), x) five times (network/MaskFlownet.py:219-223 ...).  Inference: see _dense_split."""
@@ -377,10 +399,20 @@ class MaskFlownetS(_FlowNetBase):
             c += e.shape[1]
         return self._dense(lvl, buf)
 
-    def forward(self, im1: torch.Tensor, im2: torch.Tensor, want_cascade_inputs: bool = False):
+    def forward(self, im1: torch.Tensor, im2: torch.Tensor, want_cascade_inputs: bool = False,
+                bidirectional: bool = False):
         """Returns (predictions [flow6..flow2, each * scale], [sigmoid(mask2)], srcs or None) like the reference
-        (network/MaskFlownet.py:302-315).  srcs (needed only by the cascade) is built when want_cascade_inputs."""
-        c1, c2 = self._pyramid_pair(im1, im2, "abc")
+        (network/MaskFlownet.py:302-315).  srcs (needed only by the cascade) is built when want_cascade_inputs.
+        bidirectional (inference only): im1 and im2 hold N images each and the outputs hold 2N pairs, (im1 -> im2) then
+        (im2 -> im1), from one pyramid pass over [im1; im2] (_pyramid_pair)."""
+        if bidirectional:
+            self._check_bidirectional(im1, im2)
+            n = im1.shape[0]
+            im1 = self._joined(im1, im2)
+            im2 = _swap_halves(im1, n) if want_cascade_inputs else None
+            c1, c2 = self._pyramid_pair(im1[:n], im1[n:], "abc", bidirectional=True)
+        else:
+            c1, c2 = self._pyramid_pair(im1, im2, "abc")
         x = self._corr_block(6, c1[5], c2[5], [])   # correlation + dense block
         flow, mask = self._heads(6, x, True)
         flows = [flow]
@@ -448,8 +480,12 @@ class MaskFlownet(_FlowNetBase):
     def _corr(self, a, b):
         return ops.correlation(a, b, pad_size=self.md, max_displacement=self.md, leaky_slope=SLOPE)
 
-    def forward(self, im1, im2):
-        _, _, srcs = self.MaskFlownet_S(im1, im2, want_cascade_inputs=True)
+    def forward(self, im1, im2, bidirectional: bool = False):
+        """As MaskFlownetS.forward; bidirectional: 2N pairs, (im1 -> im2) then (im2 -> im1), the head's pyramid computed
+        once, the dual pyramid and decoder at batch 2N."""
+        if bidirectional:
+            self._check_bidirectional(im1, im2)
+        _, _, srcs = self.MaskFlownet_S(im1, im2, want_cascade_inputs=True, bidirectional=bidirectional)
         c1, c2, flows_s, c30, c40 = srcs
         c3 = self._pyramid(c30, "xyz")
         c4 = self._pyramid(c40, "xyz")
@@ -511,6 +547,29 @@ def predict(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, resize=None)
     mask = ops.postprocess(occ[0], H, W, flip_channels=False, is_flow=False) if occ and occ[0].shape[1] == 1 and \
         occ[0].shape[2] * 4 == a.shape[2] else None
     return flow, mask
+
+
+@torch.no_grad()
+def predict_bidirectional(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, resize=None, alpha: float = 0.01,
+                          beta: float = 0.5):
+    """Flow in both directions and forward-backward occlusion masks of uint8 (or [0,1] float) pairs (N,3,H,W) of any size.
+
+    The mask `predict` returns is not a visibility map: for the cascade it is the y-component of the flow (the reference's
+    "visual" output), for MaskFlownet-S the sigmoid of the learned warp mask.  This function gives one: a pixel is
+    occluded (1) where its flow has no consistent match in the other direction's flow (ops.flow_consistency, Sundaram
+    et al. 2010, constants alpha and beta).
+
+    One ops.preprocess, one bidirectional forward (the pair's feature pyramid computed once for both directions), one
+    ops.postprocess over the 2N finest flows, one ops.flow_consistency.  Returns (flow_fw, flow_bw, occ_fw, occ_bw) at the
+    input size: flows (N,H,W,2) in (x,y) pixels, img1 -> img2 and img2 -> img1; masks (N,H,W) uint8, of img1's and of
+    img2's pixels."""
+    N, _, H, W = img1.shape
+    a, b, _ = ops.preprocess(img1, img2, ops.padded_size(H, W, resize))
+    preds = net(a, b, bidirectional=True)[0]
+    flows = ops.postprocess(preds[-1], H, W, flip_channels=True, is_flow=True)
+    flow_fw, flow_bw = flows[:N], flows[N:]
+    occ_fw, occ_bw = ops.flow_consistency(flow_fw, flow_bw, alpha, beta)
+    return flow_fw, flow_bw, occ_fw, occ_bw
 
 
 def precision_key(net: nn.Module) -> Tuple[str, ...]:

@@ -791,3 +791,31 @@ def flow_to_color(flow_xy: torch.Tensor, max_radius: Optional[float] = None, bgr
     _call("mfn_flow_to_color", f.device, _p(f4), _p(rgb), _p(rad_max), N, H, W,
           float(max_radius) if max_radius is not None else 0.0, 1 if bgr else 0)
     return (rgb, rad_max) if f.dim() == 4 else (rgb[0], rad_max[0])
+
+
+def flow_consistency(flow_fw: torch.Tensor, flow_bw: torch.Tensor, alpha: float = 0.01, beta: float = 0.5):
+    """Forward-backward consistency check (Sundaram, Brox and Keutzer, ECCV 2010) of the flows image 1 -> image 2
+    (flow_fw) and image 2 -> image 1 (flow_bw), (x,y) in pixels, the layout postprocess returns: (N,H,W,2) ->
+    (occ_fw, occ_bw) uint8 (N,H,W), 1 where a pixel of image 1 (occ_fw) / image 2 (occ_bw) has no consistent match in the
+    other image: its target leaves the frame, or |w + w_other(target)|^2 > alpha (|w|^2 + |w_other(target)|^2) + beta
+    (NaN or inf anywhere: 1).  An (H,W,2) pair gives (H,W) masks.  Defaults: the paper's constants.  Forward only (include/maskflow_b200.h)."""
+    for t, nm in ((flow_fw, "flow_fw"), (flow_bw, "flow_bw")):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise MaskflowError(f"flow_consistency: {nm} must be a CUDA tensor; the hot path has no CPU implementation")
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise MaskflowError(f"flow_consistency: {nm} must be a contiguous float32 tensor")
+        if t.dim() not in (3, 4) or t.shape[-1] != 2:
+            raise MaskflowError(f"flow_consistency: expected an (N,H,W,2) or (H,W,2) {nm}, got {tuple(t.shape)}")
+    if flow_fw.shape != flow_bw.shape or flow_fw.device != flow_bw.device:
+        raise MaskflowError(f"flow_consistency: flow_fw {tuple(flow_fw.shape)} and flow_bw {tuple(flow_bw.shape)} differ")
+    inf = float("inf")
+    if not (0.0 <= float(alpha) < inf and 0.0 <= float(beta) < inf):
+        raise MaskflowError(f"flow_consistency: alpha and beta must be finite and non-negative, got {alpha}, {beta}")
+    _no_grad_path("flow_consistency", flow_fw, flow_bw)
+    fw = flow_fw if flow_fw.dim() == 4 else flow_fw.unsqueeze(0)
+    bw = flow_bw if flow_bw.dim() == 4 else flow_bw.unsqueeze(0)
+    N, H, W, _ = fw.shape
+    occ_fw = torch.empty((N, H, W), device=fw.device, dtype=torch.uint8)
+    occ_bw = torch.empty((N, H, W), device=fw.device, dtype=torch.uint8)
+    _call("mfn_flow_consistency", fw.device, _p(fw), _p(bw), _p(occ_fw), _p(occ_bw), N, H, W, float(alpha), float(beta))
+    return (occ_fw, occ_bw) if flow_fw.dim() == 4 else (occ_fw[0], occ_bw[0])

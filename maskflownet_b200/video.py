@@ -8,6 +8,10 @@ images are F[:B] and their second images F[1:], both contiguous views.  Between 
 and the next B frames go into F[1:].  The graph holds the whole chain:
     HWC -> NCHW  ->  ops.preprocess (/255, centralise, resize to padded_size)  ->  network  ->  ops.postprocess
     (Upsample(4), resize back, (x,y) NHWC)  ->  ops.flow_to_color
+With bidirectional=True the network's bidirectional forward (one feature pyramid for both directions of each pair) gives
+2B flows, postprocess takes them all, the forward flows are coloured and ops.flow_consistency gives both occlusion masks:
+    preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  flow_to_color (forward flows)
+    ->  flow_consistency
 Copies follow network.PipelinedFlowPredictor's slot scheme: pinned host staging, H2D on one copy stream, D2H of the colours
 (and flows) on another, `depth` slots, so the copies of neighbouring batches run under the replay of this one.
 """
@@ -34,11 +38,19 @@ class VideoFlowPredictor:
     cv2 frames to pipe.predict); every frame must have the first one's size.  batch: pairs per graph replay; the last,
     partial batch repeats the last frame in its unused slots and yields only its real pairs.  resize: the network input
     size (H', W'), default the next multiples of 64.  max_radius / bgr: as ops.flow_to_color; a fixed max_radius keeps the
-    colours of successive frames comparable.  Weights are read through the packed images cached in the model: call
-    invalidate() after changing parameters.  Graphs are kept per frame size and network.precision_key of the model."""
+    colours of successive frames comparable.
+
+    bidirectional: each pair is also predicted backwards, (t+1 -> t), from the same feature pyramid, and each result
+    appends the forward-backward occlusion masks (H,W) uint8 (ops.flow_consistency with alpha, beta): occ_fw marks the
+    pixels of frame t with no consistent match in frame t+1, occ_bw those of frame t+1 with none in frame t.  Results are
+    (colour, occ_fw, occ_bw), or with want_flow (colour, flow, flow_bw, occ_fw, occ_bw); the masks and the backward flow
+    take the same slots and copy streams as the colours.
+
+    Weights are read through the packed images cached in the model: call invalidate() after changing parameters.  Graphs are kept per frame size and network.precision_key of the model."""
 
     def __init__(self, net: nn.Module, batch: int = 8, resize=None, max_radius=None, bgr: bool = False,
-                 want_flow: bool = False, depth: int = 2):
+                 want_flow: bool = False, depth: int = 2, bidirectional: bool = False, alpha: float = 0.01,
+                 beta: float = 0.5):
         if batch < 1 or depth < 1:
             raise MaskflowError(f"VideoFlowPredictor: batch and depth must be >= 1 (got {batch}, {depth})")
         if max_radius is not None and not (0.0 < float(max_radius) < float("inf")):
@@ -46,6 +58,9 @@ class VideoFlowPredictor:
         self.net, self.batch, self.depth = net, int(batch), int(depth)
         self.resize = None if resize is None else (int(resize[0]), int(resize[1]))
         self.max_radius, self.bgr, self.want_flow = max_radius, bool(bgr), bool(want_flow)
+        if bidirectional and not (0.0 <= float(alpha) < float("inf") and 0.0 <= float(beta) < float("inf")):
+            raise MaskflowError(f"VideoFlowPredictor: alpha and beta must be finite and non-negative, got {alpha}, {beta}")
+        self.bidirectional, self.alpha, self.beta = bool(bidirectional), float(alpha), float(beta)
         self._states = {}
         self._streams = None
 
@@ -54,12 +69,25 @@ class VideoFlowPredictor:
 
     # ---- one graph per frame size ------------------------------------------------------------------------------
     def _chain(self, F: torch.Tensor, H: int, W: int):
+        """The captured chain: {"rgb", "flow"}, and with bidirectional also {"flow_bw", "occ_fw", "occ_bw"}."""
         B = self.batch
         x = F.permute(0, 3, 1, 2).contiguous()
         a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
-        flow = ops.postprocess(self.net(a, b)[0][-1], H, W, flip_channels=True, is_flow=True)
+        if not self.bidirectional:
+            flow = ops.postprocess(self.net(a, b)[0][-1], H, W, flip_channels=True, is_flow=True)
+            rgb, _ = ops.flow_to_color(flow, self.max_radius, self.bgr)
+            return {"rgb": rgb, "flow": flow}
+        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
+        flow, flow_bw = flows[:B], flows[B:]
         rgb, _ = ops.flow_to_color(flow, self.max_radius, self.bgr)
-        return rgb, flow
+        occ_fw, occ_bw = ops.flow_consistency(flow, flow_bw, self.alpha, self.beta)
+        return {"rgb": rgb, "flow": flow, "flow_bw": flow_bw, "occ_fw": occ_fw, "occ_bw": occ_bw}
+
+    def _outputs(self):
+        """The chain outputs that leave the GPU, in the order of a result."""
+        if not self.bidirectional:
+            return ("rgb", "flow") if self.want_flow else ("rgb",)
+        return ("rgb", "flow", "flow_bw", "occ_fw", "occ_bw") if self.want_flow else ("rgb", "occ_fw", "occ_bw")
 
     def _state(self, H: int, W: int, dev: torch.device):
         key = (H, W, network.precision_key(self.net))
@@ -77,19 +105,18 @@ class VideoFlowPredictor:
         cur.wait_stream(side)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            rgb, flow = self._chain(F, H, W)
+            out = self._chain(F, H, W)
         slots = []
         for _ in range(self.depth):
             s = {"in": torch.empty((B + 1, H, W, 3), dtype=torch.uint8, device=dev),
                  "in_host": torch.empty((B + 1, H, W, 3), dtype=torch.uint8, pin_memory=True),
-                 "rgb": torch.empty_like(rgb), "rgb_host": torch.empty(rgb.shape, dtype=torch.uint8, pin_memory=True),
                  "ev_h2d": torch.cuda.Event(), "ev_in_free": torch.cuda.Event(), "ev_out": torch.cuda.Event(),
                  "ev_out_free": torch.cuda.Event(), "used": False}
-            if self.want_flow:
-                s["flow"] = torch.empty_like(flow)
-                s["flow_host"] = torch.empty(flow.shape, dtype=torch.float32, pin_memory=True)
+            for name in self._outputs():
+                s[name] = torch.empty_like(out[name])
+                s[name + "_host"] = torch.empty(out[name].shape, dtype=out[name].dtype, pin_memory=True)
             slots.append(s)
-        st = self._states[key] = {"graph": graph, "F": F, "rgb": rgb, "flow": flow, "slots": slots, "i": 0}
+        st = self._states[key] = {"graph": graph, "F": F, "out": out, "slots": slots, "i": 0}
         return st
 
     # ---- one batch ---------------------------------------------------------------------------------------------
@@ -122,24 +149,23 @@ class VideoFlowPredictor:
         st["graph"].replay()
         if s["used"]:
             cur.wait_event(s["ev_out_free"])
-        s["rgb"].copy_(st["rgb"])
-        if self.want_flow:
-            s["flow"].copy_(st["flow"])
+        for name in self._outputs():
+            s[name].copy_(st["out"][name])
         s["ev_out"].record(cur)
         with torch.cuda.stream(d2h):
             d2h.wait_event(s["ev_out"])
-            s["rgb_host"].copy_(s["rgb"], non_blocking=True)
-            if self.want_flow:
-                s["flow_host"].copy_(s["flow"], non_blocking=True)
+            for name in self._outputs():
+                s[name + "_host"].copy_(s[name], non_blocking=True)
             s["ev_out_free"].record(d2h)
         s["used"] = True
         return s
 
     def _collect(self, s, b: int) -> Iterator:
         s["ev_out_free"].synchronize()
+        names = self._outputs()
         for j in range(b):
-            rgb = s["rgb_host"][j].numpy().copy()
-            yield (rgb, s["flow_host"][j].numpy().copy()) if self.want_flow else rgb
+            res = tuple(s[name + "_host"][j].numpy().copy() for name in names)
+            yield res if len(res) > 1 else res[0]
 
     @staticmethod
     def _frame(fr, hw) -> torch.Tensor:

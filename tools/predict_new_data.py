@@ -2,7 +2,7 @@
 
     python tools/predict_new_data.py out.png --image_1 a.png --image_2 b.png -c weights.params [-n MaskFlownet_S]
     python tools/predict_new_data.py out.avi --video_filepath in.mp4 -c weights.params [--batch 8] [--resize 448,1024]
-                                     [--max_radius 20]
+                                     [--max_radius 20] [--occlusion occ.avi]
 
 An image pair gives one PNG.  A video gives a video of the input's frame rate with one colour frame per consecutive frame
 pair (so one frame fewer than the input), streamed through network.VideoFlowPredictor: each frame is uploaded once and
@@ -16,6 +16,10 @@ coloured on the GPU.  Frames go to the network in the channel order cv2 reads th
   * videos are written with cv2.VideoWriter (MJPG for .avi, mp4v otherwise) instead of moviepy; there is no audio.
   * --max_radius (new) fixes the colour scale across frames; by default every frame is normalised by its own largest
     flow, as flow_vis does.
+  * --occlusion PATH (new) also writes the forward-backward occlusion mask of each pair's first image (255 = occluded:
+    no consistent match in the second image, ops.flow_consistency): an 8-bit image for a pair, a greyscale video of one
+    frame per pair for a video.  The pair is then predicted in both directions from one feature pyramid
+    (network.predict_bidirectional); the flow written is the forward one of that run.
 """
 from __future__ import annotations
 
@@ -50,9 +54,10 @@ def _imread(cv2, path):
 
 @torch.no_grad()
 def predict_files(model: torch.nn.Module, flow_filepath: str, image_1=None, image_2=None, video_filepath=None, batch=8,
-                  resize=None, max_radius=None) -> int:
+                  resize=None, max_radius=None, occlusion_filepath=None) -> int:
     """Writes the colour-coded flow of an image pair (one image) or of a video (one frame per consecutive pair) to
-    flow_filepath; returns the number of images written."""
+    flow_filepath, and with occlusion_filepath the occlusion masks of the pairs' first images there (255 = occluded);
+    returns the number of flow images written."""
     import cv2
 
     if video_filepath is None:
@@ -63,7 +68,12 @@ def predict_files(model: torch.nn.Module, flow_filepath: str, image_1=None, imag
             raise ValueError(f"the images differ in size: {a.shape} vs {b.shape}")
         dev = next(model.parameters()).device
         to_dev = lambda im: torch.from_numpy(im).permute(2, 0, 1)[None].contiguous().to(dev)  # noqa: E731
-        flow, _ = network.predict(model, to_dev(a), to_dev(b), resize)
+        if occlusion_filepath is None:
+            flow, _ = network.predict(model, to_dev(a), to_dev(b), resize)
+        else:
+            flow, _, occ, _ = network.predict_bidirectional(model, to_dev(a), to_dev(b), resize)
+            if not cv2.imwrite(occlusion_filepath, (occ[0] * 255).cpu().numpy()):
+                raise OSError(f"cannot write {occlusion_filepath}")
         rgb, _ = ops.flow_to_color(flow[0], max_radius, bgr=True)
         if not cv2.imwrite(flow_filepath, rgb.cpu().numpy()):
             raise OSError(f"cannot write {flow_filepath}")
@@ -84,20 +94,32 @@ def predict_files(model: torch.nn.Module, flow_filepath: str, image_1=None, imag
         finally:
             cap.release()
 
-    pred = VideoFlowPredictor(model, batch=batch, resize=resize, max_radius=max_radius, bgr=True)
-    fourcc = cv2.VideoWriter_fourcc(*("MJPG" if flow_filepath.lower().endswith(".avi") else "mp4v"))
-    writer, n = None, 0
+    bidirectional = occlusion_filepath is not None
+    pred = VideoFlowPredictor(model, batch=batch, resize=resize, max_radius=max_radius, bgr=True,
+                              bidirectional=bidirectional)
+
+    def open_writer(path, shape):
+        fourcc = cv2.VideoWriter_fourcc(*("MJPG" if path.lower().endswith(".avi") else "mp4v"))
+        w = cv2.VideoWriter(path, fourcc, fps if fps > 0 else 25.0, (shape[1], shape[0]))
+        if not w.isOpened():
+            raise OSError(f"cannot write {path}")
+        return w
+
+    writers, n = [], 0
     try:
-        for rgb in pred.run(frames()):
-            if writer is None:
-                writer = cv2.VideoWriter(flow_filepath, fourcc, fps if fps > 0 else 25.0, (rgb.shape[1], rgb.shape[0]))
-                if not writer.isOpened():
-                    raise OSError(f"cannot write {flow_filepath}")
-            writer.write(rgb)
+        for res in pred.run(frames()):
+            rgb = res[0] if bidirectional else res
+            if not writers:
+                writers.append(open_writer(flow_filepath, rgb.shape))
+                if bidirectional:
+                    writers.append(open_writer(occlusion_filepath, rgb.shape))
+            writers[0].write(rgb)
+            if bidirectional:   # grey frames through the colour writer: 255 = occluded in all three channels
+                writers[1].write(cv2.cvtColor(res[1] * 255, cv2.COLOR_GRAY2BGR))
             n += 1
     finally:
-        if writer is not None:
-            writer.release()
+        for w in writers:
+            w.release()
     return n
 
 
@@ -115,14 +137,18 @@ def main(argv=None):
                     help="fixed flow magnitude (pixels) of the colour wheel's rim; default: each frame's largest flow")
     ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
                     help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
+    ap.add_argument("--occlusion", default=None, metavar="PATH",
+                    help="also write the forward-backward occlusion mask of each pair (255 = occluded) to PATH: an image "
+                         "for an image pair, a video for a video")
     a = ap.parse_args(argv)
     if a.video_filepath is None and (a.image_1 is None or a.image_2 is None):
         ap.error("give --image_1 and --image_2, or --video_filepath")
     resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
     model = load_model(a.network, a.checkpoint)
     model.inference_precision = a.precision
-    n = predict_files(model, a.flow_filepath, a.image_1, a.image_2, a.video_filepath, a.batch, resize, a.max_radius)
-    print(f"wrote {n} image(s) to {a.flow_filepath}")
+    n = predict_files(model, a.flow_filepath, a.image_1, a.image_2, a.video_filepath, a.batch, resize, a.max_radius,
+                      a.occlusion)
+    print(f"wrote {n} image(s) to {a.flow_filepath}" + (f" and their occlusion masks to {a.occlusion}" if a.occlusion else ""))
 
 
 if __name__ == "__main__":
