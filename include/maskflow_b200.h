@@ -464,6 +464,39 @@ MFN_API int mfn_multiscale_epe_backward(const float* flow, const float* mask, co
                                         const float* weights, int num_scales, float eps, float q, const float* grad_loss,
                                         const float* mask_sum, float* const* grad_preds, int N, int H, int W, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Unsupervised losses on unlabelled frame pairs (UnFlow, Meister, Hur and Roth, AAAI 2018): an occlusion-masked census
+ * distance between image 1 and image 2 warped by the flow, and a second-order, edge-aware flow smoothness.
+ * All tensors float32 NCHW (occ uint8), device pointers, 4-byte aligned.
+ *
+ * Census.  img1, img2w (N,3,H,W) RGB in [0,1]; occ (N,H,W) uint8, nonzero = occluded (left out).
+ *   I = 255 (0.2989 R + 0.5870 G + 0.1140 B).  Interior pixels p: 3 <= x <= W-4, 3 <= y <= H-4.  Over the 48 offsets o
+ *   of {-3..3}^2 without (0,0):  t(I,p,o) = D / sqrt(0.81 + D^2), D = I(p+o) - I(p);  s = t(I1,p,o) - t(I2w,p,o);
+ *   d(p) = sum_o s^2 / (0.1 + s^2);  rho(d) = (d^2 + 1e-6)^0.45;  v(p) = 1 - occ(p) on interior pixels, 0 elsewhere.
+ *   forward:  loss[n] = sum_p v rho(d) / max(vsum[n], 1), vsum[n] = sum_p v (N floats each);
+ *             coef (N,H,W) = v rho'(d), the per-pixel factor the backward reads;
+ *             ws: 8*N*ceil(H/8)*ceil(W/32) bytes of caller-owned scratch (per-tile partial sums, added in a fixed order).
+ *   backward: g_img2w (N,3,H,W) = d( sum_n g_loss[n] loss[n] ) / d img2w, every element written (a gather).  img1 gets
+ *             no gradient.
+ * Smoothness.  flow (N,2,H,W) (either channel order: both are summed alike), img (N,3,H,W) the image whose edges weight it.
+ *   d2x F_c(p) = F_c(x-1) - 2 F_c(x) + F_c(x+1) on 1 <= x <= W-2, wx(p) = exp(-10 (1/3) sum_k |img_k(x+1) - img_k(x-1)| / 2),
+ *   the same in y.  forward: loss[n] = sum_{c,p} wx |d2x F_c| / (2 H (W-2)) + sum_{c,p} wy |d2y F_c| / (2 (H-2) W)
+ *   (a direction with no pixels adds 0); ws: 8*N*ceil(H*W/256) bytes.
+ *   backward: g_flow (N,2,H,W) = d( sum_n g_loss[n] loss[n] ) / d flow, with d|z|/dz = sign(z) (0 at 0); a 3-tap gather
+ *   per direction, every element written.  img gets no gradient.
+ * Shapes below 7 (census) or 3 (smoothness) in a dimension are legal: no interior pixels, loss 0, gradient 0.  No atomics:
+ * results are bit-reproducible.  A null pointer, an extent below 1, a misaligned pointer, N > 65535, 3*H*W >= 2^31 or a
+ * too small workspace returns MFN_ERR_INVALID_ARG.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API int mfn_census_loss_forward(const float* img1, const float* img2w, const unsigned char* occ, float* coef, float* vsum,
+                                    float* loss, void* ws, long long ws_bytes, int N, int H, int W, void* stream);
+MFN_API int mfn_census_loss_backward(const float* img1, const float* img2w, const float* coef, const float* vsum,
+                                     const float* g_loss, float* g_img2w, int N, int H, int W, void* stream);
+MFN_API int mfn_smoothness_loss_forward(const float* flow, const float* img, float* loss, void* ws, long long ws_bytes, int N,
+                                        int H, int W, void* stream);
+MFN_API int mfn_smoothness_loss_backward(const float* flow, const float* img, const float* g_loss, float* g_flow, int N,
+                                         int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,10 @@ SIGNATURES = {
     "mfn_color_augment_forward": [_f, _f, _f, _f, _f, _fl, _ll, _f, _f, _f, _ll, _i, _i, _i, _i, _f],
     "mfn_multiscale_epe_forward": [_f, _f, _f, _f, _f, _i, _fl, _fl, _f, _f, _f, _ll, _i, _i, _i, _f],
     "mfn_multiscale_epe_backward": [_f, _f, _f, _f, _f, _i, _fl, _fl, _f, _f, _f, _i, _i, _i, _f],
+    "mfn_census_loss_forward": [_f] * 7 + [_ll, _i, _i, _i, _f],
+    "mfn_census_loss_backward": [_f] * 6 + [_i, _i, _i, _f],
+    "mfn_smoothness_loss_forward": [_f] * 4 + [_ll, _i, _i, _i, _f],
+    "mfn_smoothness_loss_backward": [_f] * 4 + [_i, _i, _i, _f],
     "mfn_set_tuning": [ctypes.c_char_p, _i],
     "mfn_conv3x3_pack_weights": [_f, _f, _i, _i, _f],
     "mfn_conv3x3_forward": [_f, _ll, _f, _f, _f, _ll, _i, _i, _i, _i, _i, _i, _fl, _f],

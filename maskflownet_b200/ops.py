@@ -819,3 +819,85 @@ def flow_consistency(flow_fw: torch.Tensor, flow_bw: torch.Tensor, alpha: float 
     occ_bw = torch.empty((N, H, W), device=fw.device, dtype=torch.uint8)
     _call("mfn_flow_consistency", fw.device, _p(fw), _p(bw), _p(occ_fw), _p(occ_bw), N, H, W, float(alpha), float(beta))
     return (occ_fw, occ_bw) if flow_fw.dim() == 4 else (occ_fw[0], occ_bw[0])
+
+
+# ----------------------------------------------------------------------------------------------------------
+# Unsupervised losses (csrc/unsup_loss.cu): census photometric loss and second-order smoothness
+# ----------------------------------------------------------------------------------------------------------
+def unsup_workspace_bytes(loss: str, N: int, H: int, W: int) -> int:
+    """Bytes of the `ws` scratch of mfn_census_loss_forward ("census") / mfn_smoothness_loss_forward ("smoothness")
+    (include/maskflow_b200.h, "Unsupervised losses")."""
+    if loss == "census":
+        return 8 * N * (-(-H // 8)) * (-(-W // 32))
+    if loss == "smoothness":
+        return 8 * N * (-(-H * W // 256))
+    raise MaskflowError(f"unsup_workspace_bytes: unknown loss {loss!r}")
+
+
+def _census_forward(img1, img2w, occ):
+    """(loss (N,), vsum (N,), coef (N,H,W)) of mfn_census_loss_forward."""
+    N, _, H, W = img1.shape
+    dev = img1.device
+    loss = torch.empty(N, device=dev, dtype=torch.float32)
+    vsum = torch.empty(N, device=dev, dtype=torch.float32)
+    coef = torch.empty((N, H, W), device=dev, dtype=torch.float32)
+    nb = unsup_workspace_bytes("census", N, H, W)
+    ws = torch.empty(nb // 4, device=dev, dtype=torch.float32)
+    _call("mfn_census_loss_forward", dev, _p(img1), _p(img2w), _p(occ), _p(coef), _p(vsum), _p(loss), _p(ws), nb, N, H, W)
+    return loss, vsum, coef
+
+
+def _census_backward(img1, img2w, coef, vsum, g):
+    N, _, H, W = img1.shape
+    gi = torch.empty_like(img2w)
+    _call("mfn_census_loss_backward", img1.device, _p(img1), _p(img2w), _p(coef), _p(vsum), _p(g), _p(gi), N, H, W)
+    return gi
+
+
+def _smoothness_forward(flow, img):
+    N, _, H, W = flow.shape
+    loss = torch.empty(N, device=flow.device, dtype=torch.float32)
+    nb = unsup_workspace_bytes("smoothness", N, H, W)
+    ws = torch.empty(nb // 4, device=flow.device, dtype=torch.float32)
+    _call("mfn_smoothness_loss_forward", flow.device, _p(flow), _p(img), _p(loss), _p(ws), nb, N, H, W)
+    return loss
+
+
+def _smoothness_backward(flow, img, g):
+    N, _, H, W = flow.shape
+    gf = torch.empty_like(flow)
+    _call("mfn_smoothness_loss_backward", flow.device, _p(flow), _p(img), _p(g), _p(gf), N, H, W)
+    return gf
+
+
+class CensusLossFn(torch.autograd.Function):
+    """mfn_census_loss_forward / _backward: per-sample census loss (N,) of (img1, img2_warped, occ); the gradient
+    reaches img2_warped only (img1 and occ are data).  Inputs are checked by losses.census_loss."""
+
+    @staticmethod
+    def forward(ctx, img1, img2w, occ):
+        loss, vsum, coef = _census_forward(img1, img2w, occ)
+        ctx.save_for_backward(img1, img2w, coef, vsum)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        img1, img2w, coef, vsum = ctx.saved_tensors
+        return None, _census_backward(img1, img2w, coef, vsum, g.contiguous().float()), None
+
+
+class SmoothnessLossFn(torch.autograd.Function):
+    """mfn_smoothness_loss_forward / _backward: per-sample smoothness (N,) of flow weighted by the edges of img; the
+    gradient reaches the flow only.  Inputs are checked by losses.smoothness_loss."""
+
+    @staticmethod
+    def forward(ctx, flow, img):
+        ctx.save_for_backward(flow, img)
+        return _smoothness_forward(flow, img)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        flow, img = ctx.saved_tensors
+        return _smoothness_backward(flow, img, g.contiguous().float()), None

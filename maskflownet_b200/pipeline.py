@@ -4,6 +4,8 @@ drives -- same method names, argument meaning and return values -- composed from
     train_batch   pipeline.py:89-115   /255, geo_aug, color_aug (augment.py), centralize, network (tensor-core forward under
                                        autograd), labels.flip, MultiscaleEpe (fused), backward, ONE gradient all-reduce,
                                        Adam step rescaled by 1/batch_size (Trainer.step(batch_size)), EPE metric
+    train_batch_unsupervised           (not in the reference) the same step on unlabelled pairs: network at batch 2n on
+                                       both directions, losses.unsupervised_loss (census + smoothness, occlusion-masked)
     do_batch_mx   pipeline.py:117-132  centralize + BilinearResize2D to multiples of 64 (ops.preprocess) + network
     do_batch      pipeline.py:134-147  Upsample(4), resize back + per-channel rescale, Reconstruction2DSmooth, masked EPE
     validate      pipeline.py:149-187  dataset loop -> mean EPE, or the KITTI outlier ratio (return_type != 'epe')
@@ -27,6 +29,7 @@ from . import losses, network, ops, params as mparams
 from ._lib import MaskflowError
 
 STRIDES = (64, 32, 16, 8, 4)
+SMOOTH_WEIGHT = 3.0     # train_batch_unsupervised's weight of the smoothness term (README, "Unsupervised fine-tuning")
 
 
 def _to_device(x, device, dtype=None) -> torch.Tensor:
@@ -52,7 +55,7 @@ class PipelineFlownet:
 
     def __init__(self, device=None, network_class: str = "MaskFlownet_S", lr_schedule: Optional[Sequence[Tuple[int, float]]] = None,
                  multiscale_weights: Sequence[float] = losses.WEIGHTS, q: Optional[float] = None, learning_rate: float = 1e-4,
-                 deterministic: bool = False, precision: str = "fp32"):
+                 deterministic: bool = False, precision: str = "fp32", smooth_weight: float = SMOOTH_WEIGHT):
         if precision not in network.PRECISIONS:
             raise MaskflowError(f"PipelineFlownet: precision must be one of {network.PRECISIONS}, got {precision!r}")
         self.precision = precision
@@ -73,6 +76,7 @@ class PipelineFlownet:
         self.multiscale_weights = w if len(w) == 5 else list(losses.WEIGHTS)              # pipeline.py:39-41
         self.q = q
         self.lr_schedule = list(lr_schedule) if lr_schedule is not None else []
+        self.smooth_weight = float(smooth_weight)
         self._bucket: Optional[mdist.GradBucket] = None
 
     # ---- deterministic mode -------------------------------------------------------------------------------------
@@ -168,10 +172,7 @@ class PipelineFlownet:
             mask = np.full((n, 1, 1, 1), 255, dtype=np.uint8)
         img1, img2, mask = _to_device(img1, dev), _to_device(img2, dev), _to_device(mask, dev)
         label = _to_device(label, dev, torch.float32)
-        self.network.train()
-        if self._bucket is None:
-            self._bucket = mdist.GradBucket(self.network.parameters())
-        self._bucket.zero_()
+        self._begin_step()
         with torch.no_grad():                                   # the augmentation is data preparation (forward only)
             img1, img2, label, mask = geo_aug(img1, img2, label, mask)        # uint8 in: `/ 255` is folded into the kernel
             img1, img2 = color_aug(img1, img2)
@@ -179,13 +180,56 @@ class PipelineFlownet:
             label = label.flip(1).contiguous()
         pred, occ_masks, _ = self.network(img1, img2)
         per_sample = self.loss(pred, occ_masks, label, mask)
+        self._finish_step(per_sample, n, global_batch)
+        with torch.no_grad():
+            epe = epe_loss_with_mask(ops.upsample(pred[-1].detach(), self.scale), label, mask)
+        return {"epe": float(epe.mean().item())}
+
+    def _begin_step(self) -> None:
+        self.network.train()
+        if self._bucket is None:
+            self._bucket = mdist.GradBucket(self.network.parameters())
+        self._bucket.zero_()
+
+    def _finish_step(self, per_sample: torch.Tensor, n: int, global_batch: Optional[int]) -> None:
+        """Backward of the summed per-sample losses, ONE gradient all-reduce scaled by 1/global_batch (default: n * world
+        size), Adam step: the tail every training step shares."""
         per_sample.sum().backward()                             # per-sample losses are summed (pipeline.py:112-113)
         world = torch.distributed.get_world_size() if torch.distributed.is_initialized() else 1
         self._bucket.allreduce_(global_batch=n * world if global_batch is None else global_batch)
         self.trainer.step()                                     # trainer.step(batch_size): the 1/batch rescale is in the bucket
+
+    def train_batch_unsupervised(self, img1, img2, color_aug=None, global_batch: Optional[int] = None) -> Dict[str, float]:
+        """One unsupervised optimisation step on this rank's shard of unlabelled pairs (losses.unsupervised_loss: census
+        photometric loss masked by the forward-backward check, plus smooth_weight times the second-order smoothness).
+        img1 / img2 (n,3,H,W) uint8, H and W multiples of 64.  The network runs once at batch 2n on [img1; img2] ->
+        [img2; img1]; color_aug (an augment.ColorAugmentation for batch n) changes only the network input, the losses see
+        the original images.  global_batch: pairs over ALL ranks (default n * world size); each pair contributes both
+        directions' losses.  Returns the means over this rank's 2n directed pairs: {"loss", "photo", "smooth",
+        "occluded"} (occluded: share of pixels left out of the census term)."""
+        with self._determinism():
+            return self._train_batch_unsupervised(img1, img2, color_aug, global_batch)
+
+    def _train_batch_unsupervised(self, img1, img2, color_aug, global_batch) -> Dict[str, float]:
+        img1, img2 = _to_device(img1, self.device), _to_device(img2, self.device)
+        if img1.dtype != torch.uint8 or img2.dtype != torch.uint8 or img1.dim() != 4 or img1.shape[1] != 3 \
+                or img1.shape != img2.shape:
+            raise MaskflowError(f"train_batch_unsupervised: expected two uint8 (n,3,H,W) batches of one shape, got "
+                                f"{tuple(img1.shape)} {img1.dtype} and {tuple(img2.shape)} {img2.dtype}")
+        n, _, H, W = img1.shape
+        if H % 64 or W % 64:
+            raise MaskflowError(f"train_batch_unsupervised: H and W must be multiples of 64, got {H}x{W}")
+        self._begin_step()
         with torch.no_grad():
-            epe = epe_loss_with_mask(ops.upsample(pred[-1].detach(), self.scale), label, mask)
-        return {"epe": float(epe.mean().item())}
+            a, b = img1.float() / 255.0, img2.float() / 255.0
+            x1, x2 = (a, b) if color_aug is None else color_aug(a, b)
+            x1, x2, _ = self.centralize(torch.cat([x1, x2]), torch.cat([x2, x1]))
+        pred, _, _ = self.network(x1, x2)
+        flow = ops.upsample(pred[-1], self.scale)
+        out = losses.unsupervised_loss(a, b, flow[:n], flow[n:], self.smooth_weight)
+        self._finish_step(out.loss, n, global_batch)
+        means = torch.stack([t.detach().mean() for t in out]).tolist()
+        return dict(zip(("loss", "occluded", "photo", "smooth"), means))
 
     # ---- inference ---------------------------------------------------------------------------------------------
     @torch.no_grad()
