@@ -370,6 +370,32 @@ MFN_API int mfn_flow_consistency(const float* flow_fw, const float* flow_bw, uns
                                  int N, int H, int W, float alpha, float beta, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Frame interpolation from bidirectional flow: occlusion-weighted forward splatting of both images of each pair.
+ *   img0, img1 (N,H,W,3) uint8 (any channel order); flow_fw (img0 -> img1), flow_bw (img1 -> img0) (N,H,W,2) float32,
+ *   (x,y) pixels, 8-byte aligned; occ_fw, occ_bw (N,H,W) uint8 (mfn_flow_consistency's masks, nonzero = occluded);
+ *   times_host: a HOST array of T times, each in (0,1); occ_weight in [0,1].  out (N,T,H,W,3) uint8.
+ * For time t, every pixel p = (x,y) of img0 is a source with uv = flow_fw[p], target q = (fmaf(t,u,x), fmaf(t,v,y)) in
+ * float32 and weight w = (1-t) (occ_fw[p] ? occ_weight : 1); every pixel of img1 likewise with flow_bw, occ_bw, target
+ * fmaf(1-t, u, x) and weight t (occ_bw[p] ? occ_weight : 1) (1-t in float32).  A non-finite q, or one outside
+ * [-1,W] x [-1,H], contributes nothing.  Otherwise each corner c of floor(q), floor(q)+1 inside [0,W-1] x [0,H-1] receives
+ * b w I(p) in each colour sum and b w in the weight sum, b = (1-|qx-cx|)(1-|qy-cy|); corners outside are dropped.
+ * Output pixel o: weight sum W_o >= 2^-20: rint(acc_c / W_o) (ties to even), clamped to [0,255]; otherwise (a hole)
+ * rint((1-t) img0[o] + t img1[o]).
+ * The sums are 64-bit fixed point added with integer atomics (scales 2^(61 - k) for the weight and 2^(53 - k) for the
+ * colours, k = bit length of 2HW), so the result does not depend on the order of the atomics: bit-reproducible.  Per time
+ * step: a cudaMemsetAsync of the workspace, a splat launch and a normalise launch; t goes by value, so the call is
+ * capture-safe for any T.  ws: caller-owned, mfn_interpolate_frames_workspace_bytes(N,H,W) = 32 N H W bytes (one step's
+ * accumulators), 16-byte aligned.  A null pointer, an extent or T below 1, a time outside (0,1) or non-finite, occ_weight
+ * outside [0,1], a misaligned flow or workspace, or a short workspace returns MFN_ERR_INVALID_ARG; H*W >= 2^31 or
+ * N > 65535 returns MFN_ERR_ALIGNMENT.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API long long mfn_interpolate_frames_workspace_bytes(int N, int H, int W);
+MFN_API int mfn_interpolate_frames(const unsigned char* img0, const unsigned char* img1, const float* flow_fw,
+                                   const float* flow_bw, const unsigned char* occ_fw, const unsigned char* occ_bw,
+                                   unsigned char* out, void* ws, long long ws_bytes, int N, int H, int W,
+                                   const float* times_host, int T, float occ_weight, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Deterministic mode: bit-reproducible variants of the entry points whose default kernels accumulate with fp32 atomics
  * (the scatter of a bilinear sample's gradient to its four corners, per-CTA weight partials, per-slice plane sums).  Same
  * arguments and results as the counterpart named without _det, plus a caller-owned workspace `det_ws` of `det_ws_bytes`

@@ -40,6 +40,8 @@ SIGNATURES = {
     "mfn_postprocess_forward": [_f, _f, _i, _i, _i, _i, _i, _i, _i, _i, _f],
     "mfn_flow_to_color": [_f, _f, _f, _i, _i, _i, _fl, _i, _f],
     "mfn_flow_consistency": [_f, _f, _f, _f, _i, _i, _i, _fl, _fl, _f],
+    "mfn_interpolate_frames_workspace_bytes": [_i, _i, _i],
+    "mfn_interpolate_frames": [_f] * 8 + [_ll, _i, _i, _i, _f, _i, _fl, _f],
     "mfn_warp_mask_backward_det": [_f] * 14 + [_i] * 5 + [_fl, _fl, _fl, _i, _f, _ll, _f],
     "mfn_deformable_conv_backward_det": [_f] * 8 + [_i] * 6 + [_f, _ll, _f],
     "mfn_bilinear_sampler_backward_det": [_f] * 5 + [_i] * 6 + [_f, _ll, _f],
@@ -62,6 +64,8 @@ SIGNATURES = {
     "mfn_split_pack": [_f, _ll, _i, _i, _i, _i, _f, _i, _i, _f],
     "mfn_bf16_pack": [_f, _ll, _i, _i, _i, _i, _f, _i, _i, _f],
 }
+# entries of SIGNATURES that do not return an int status
+RESTYPES = {"mfn_interpolate_frames_workspace_bytes": _ll}
 
 
 class MaskflowError(RuntimeError):
@@ -102,7 +106,7 @@ def lib() -> ctypes.CDLL:
         for name, argtypes in SIGNATURES.items():
             fn = getattr(L, name)
             fn.argtypes = argtypes
-            fn.restype = ctypes.c_int
+            fn.restype = RESTYPES.get(name, ctypes.c_int)
         _lib = L
         # experiment hook: MFN_TUNING="key=value,key=value" applies mfn_set_tuning at load time
         for item in filter(None, os.environ.get("MFN_TUNING", "").split(",")):

@@ -58,18 +58,26 @@ struct FixedScale {
 // above +inf, so an unsigned max over it is a max that keeps NaN.
 __device__ __forceinline__ unsigned det_abs_bits(float v) { return __float_as_uint(v) & 0x7fffffffu; }
 
+// the finite scale 2^s for an exponent known in advance (-126 <= s <= 126), e.g. from a static bound on the contributions
+__device__ __forceinline__ FixedScale det_fixed_scale(int s) {
+  FixedScale f;
+  f.up = __int_as_float((s + 127) << 23);
+  f.down = __longlong_as_double((long long)(1023 - s) << 52);
+  f.finite = true;
+  return f;
+}
+
 // nb = 1: B = bound[0]; nb = 2: B = bound[0] * bound[1] (in double, so that the product itself cannot overflow)
 __device__ __forceinline__ FixedScale det_scale(const unsigned* __restrict__ bound, int nb, int fanin_bits) {
   double b = (double)__uint_as_float(bound[0]);
   if (nb == 2) b *= (double)__uint_as_float(bound[1]);
-  FixedScale f;
-  f.finite = b <= 3.4028234663852886e38;   // FLT_MAX; false for NaN and inf
+  const bool finite = b <= 3.4028234663852886e38;   // FLT_MAX; false for NaN and inf
   int e = 0;
-  if (f.finite && b > 0.0) frexp(b, &e);
+  if (finite && b > 0.0) frexp(b, &e);
   int s = 61 - fanin_bits - e;
   if (s > 126) s = 126;                    // s >= 61 - 40 - 128 for every shape the entry points accept
-  f.up = __int_as_float((s + 127) << 23);
-  f.down = __longlong_as_double((long long)(1023 - s) << 52);
+  FixedScale f = det_fixed_scale(s);
+  f.finite = finite;
   return f;
 }
 

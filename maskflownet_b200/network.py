@@ -572,6 +572,22 @@ def predict_bidirectional(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor
     return flow_fw, flow_bw, occ_fw, occ_bw
 
 
+@torch.no_grad()
+def interpolate_frames(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, times, resize=None, alpha: float = 0.01,
+                       beta: float = 0.5, occ_weight: float = 0.01) -> torch.Tensor:
+    """In-between frames of uint8 pairs (N,3,H,W) of any size at the given times in (0,1) (0 = img1): predict_bidirectional
+    (flows both ways and the occlusion masks, constants alpha, beta), then ops.interpolate_frames (occlusion-weighted
+    forward splatting, occluded pixels weighted by occ_weight) on NHWC views of the images.  Returns (N,T,H,W,3) uint8, in
+    the channel order of the inputs."""
+    if img1.dtype != torch.uint8 or img2.dtype != torch.uint8:
+        raise ops.MaskflowError(f"interpolate_frames: the images must be uint8, got {img1.dtype} and {img2.dtype}")
+    ts = ops._interp_times(times, "interpolate_frames")
+    flow_fw, flow_bw, occ_fw, occ_bw = predict_bidirectional(net, img1, img2, resize, alpha, beta)
+    a = img1.permute(0, 2, 3, 1).contiguous()
+    b = img2.permute(0, 2, 3, 1).contiguous()
+    return ops.interpolate_frames(a, b, flow_fw, flow_bw, occ_fw, occ_bw, ts, occ_weight)
+
+
 def precision_key(net: nn.Module) -> Tuple[str, ...]:
     """The inference_precision of every flow network inside `net` (the cascade's head may be set on its own): what a
     captured graph depends on besides the input shape."""

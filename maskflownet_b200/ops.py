@@ -821,6 +821,65 @@ def flow_consistency(flow_fw: torch.Tensor, flow_bw: torch.Tensor, alpha: float 
     return (occ_fw, occ_bw) if flow_fw.dim() == 4 else (occ_fw[0], occ_bw[0])
 
 
+def _interp_times(times, who: str):
+    """times -> a tuple of floats, each in (0,1)."""
+    try:
+        ts = tuple(float(t) for t in times)
+    except TypeError:               # a single time
+        ts = (float(times),)
+    if not ts:
+        raise MaskflowError(f"{who}: at least one time is required")
+    for t in ts:
+        if not 0.0 < t < 1.0:
+            raise MaskflowError(f"{who}: every time must lie in (0,1), got {t}")
+    return ts
+
+
+def interpolate_frames(img0: torch.Tensor, img1: torch.Tensor, flow_fw: torch.Tensor, flow_bw: torch.Tensor,
+                       occ_fw: torch.Tensor, occ_bw: torch.Tensor, times, occ_weight: float = 0.01) -> torch.Tensor:
+    """In-between frames of image pairs by occlusion-weighted forward splatting of both images along their flows
+    (include/maskflow_b200.h, mfn_interpolate_frames).  img0, img1 (N,H,W,3) uint8, any channel order (the layout of the
+    video predictor's frame buffer); flow_fw (img0 -> img1) and flow_bw (img1 -> img0) (N,H,W,2) float32 (x,y) pixels, the
+    layout postprocess and network.predict_bidirectional return; occ_fw, occ_bw (N,H,W) uint8 from flow_consistency.
+    times: one time or a sequence, each in (0,1) (0 = img0).  At time t each pixel of img0 moves by t * flow_fw with weight
+    (1 - t), each of img1 by (1 - t) * flow_bw with weight t, occluded ones weighted by occ_weight (in [0,1]); pixels no
+    source reaches take the blend (1 - t) img0 + t img1.  Returns (N,T,H,W,3) uint8; (H,W,...) inputs give (T,H,W,3).
+    Bit-reproducible.  Forward only."""
+    ts = _interp_times(times, "interpolate_frames")
+    if not (0.0 <= float(occ_weight) <= 1.0):
+        raise MaskflowError(f"interpolate_frames: occ_weight must lie in [0,1], got {occ_weight}")
+    args = ((img0, "img0", torch.uint8, 3), (img1, "img1", torch.uint8, 3), (flow_fw, "flow_fw", torch.float32, 2),
+            (flow_bw, "flow_bw", torch.float32, 2), (occ_fw, "occ_fw", torch.uint8, None), (occ_bw, "occ_bw", torch.uint8, None))
+    batched = isinstance(img0, torch.Tensor) and img0.dim() == 4
+    lead = None
+    for t, nm, dtype, last in args:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise MaskflowError(f"interpolate_frames: {nm} must be a CUDA tensor; the hot path has no CPU implementation")
+        if t.dtype != dtype or not t.is_contiguous():
+            raise MaskflowError(f"interpolate_frames: {nm} must be a contiguous {dtype} tensor")
+        dims = (4 if batched else 3) - (last is None)
+        if t.dim() != dims or (last is not None and t.shape[-1] != last):
+            want = ("(N,H,W" if batched else "(H,W") + (f",{last})" if last is not None else ")")
+            raise MaskflowError(f"interpolate_frames: expected {nm} of shape {want}, got {tuple(t.shape)}")
+        ld = tuple(t.shape[:dims if last is None else dims - 1])
+        if lead is None:
+            lead, dev = ld, t.device
+        elif ld != lead or t.device != dev:
+            raise MaskflowError(f"interpolate_frames: {nm} {tuple(t.shape)} on {t.device} does not match img0 "
+                                f"{tuple(img0.shape)} on {img0.device}")
+    _no_grad_path("interpolate_frames", flow_fw, flow_bw)
+    if not batched:
+        img0, img1, flow_fw, flow_bw, occ_fw, occ_bw = (t.unsqueeze(0) for t in (img0, img1, flow_fw, flow_bw, occ_fw, occ_bw))
+    N, H, W, _ = img0.shape
+    out = torch.empty((N, len(ts), H, W, 3), device=dev, dtype=torch.uint8)
+    nb = int(_lib.lib().mfn_interpolate_frames_workspace_bytes(N, H, W))
+    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    times_host = (ctypes.c_float * len(ts))(*ts)
+    _call("mfn_interpolate_frames", dev, _p(img0), _p(img1), _p(flow_fw), _p(flow_bw), _p(occ_fw), _p(occ_bw), _p(out),
+          _p(ws), nb, N, H, W, ctypes.cast(times_host, ctypes.c_void_p), len(ts), float(occ_weight))
+    return out if batched else out[0]
+
+
 # ----------------------------------------------------------------------------------------------------------
 # Unsupervised losses (csrc/unsup_loss.cu): census photometric loss and second-order smoothness
 # ----------------------------------------------------------------------------------------------------------

@@ -12,6 +12,10 @@ With bidirectional=True the network's bidirectional forward (one feature pyramid
 2B flows, postprocess takes them all, the forward flows are coloured and ops.flow_consistency gives both occlusion masks:
     preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  flow_to_color (forward flows)
     ->  flow_consistency
+With interpolate=T the chain continues into ops.interpolate_frames, which reads the frame buffer's two views directly, and
+the colour coding is skipped:
+    preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  flow_consistency
+    ->  interpolate_frames(F[:B], F[1:], ...) at the times k / (T+1), k = 1..T
 Copies follow network.PipelinedFlowPredictor's slot scheme: pinned host staging, H2D on one copy stream, D2H of the colours
 (and flows) on another, `depth` slots, so the copies of neighbouring batches run under the replay of this one.
 """
@@ -46,11 +50,16 @@ class VideoFlowPredictor:
     (colour, occ_fw, occ_bw), or with want_flow (colour, flow, flow_bw, occ_fw, occ_bw); the masks and the backward flow
     take the same slots and copy streams as the colours.
 
+    interpolate: T >= 1 in-between frames per pair instead of the colour image, at the uniform times k / (T+1), k = 1..T
+    (ops.interpolate_frames, occluded pixels weighted by occ_weight); implies bidirectional.  Results are the (T,H,W,3)
+    uint8 stack of pair (t, t+1), in the channel order of the frames, or with want_flow (frames, flow, flow_bw, occ_fw,
+    occ_bw).  interpolate=0 (default): no interpolation.
+
     Weights are read through the packed images cached in the model: call invalidate() after changing parameters.  Graphs are kept per frame size and network.precision_key of the model."""
 
     def __init__(self, net: nn.Module, batch: int = 8, resize=None, max_radius=None, bgr: bool = False,
                  want_flow: bool = False, depth: int = 2, bidirectional: bool = False, alpha: float = 0.01,
-                 beta: float = 0.5):
+                 beta: float = 0.5, interpolate: int = 0, occ_weight: float = 0.01):
         if batch < 1 or depth < 1:
             raise MaskflowError(f"VideoFlowPredictor: batch and depth must be >= 1 (got {batch}, {depth})")
         if max_radius is not None and not (0.0 < float(max_radius) < float("inf")):
@@ -58,9 +67,15 @@ class VideoFlowPredictor:
         self.net, self.batch, self.depth = net, int(batch), int(depth)
         self.resize = None if resize is None else (int(resize[0]), int(resize[1]))
         self.max_radius, self.bgr, self.want_flow = max_radius, bool(bgr), bool(want_flow)
+        if not isinstance(interpolate, int) or isinstance(interpolate, bool) or interpolate < 0:
+            raise MaskflowError(f"VideoFlowPredictor: interpolate must be a non-negative integer, got {interpolate!r}")
+        if interpolate and not 0.0 <= float(occ_weight) <= 1.0:
+            raise MaskflowError(f"VideoFlowPredictor: occ_weight must lie in [0,1], got {occ_weight}")
+        bidirectional = bool(bidirectional) or interpolate > 0
         if bidirectional and not (0.0 <= float(alpha) < float("inf") and 0.0 <= float(beta) < float("inf")):
             raise MaskflowError(f"VideoFlowPredictor: alpha and beta must be finite and non-negative, got {alpha}, {beta}")
-        self.bidirectional, self.alpha, self.beta = bool(bidirectional), float(alpha), float(beta)
+        self.bidirectional, self.alpha, self.beta = bidirectional, float(alpha), float(beta)
+        self.interpolate, self.occ_weight = int(interpolate), float(occ_weight)
         self._states = {}
         self._streams = None
 
@@ -69,7 +84,8 @@ class VideoFlowPredictor:
 
     # ---- one graph per frame size ------------------------------------------------------------------------------
     def _chain(self, F: torch.Tensor, H: int, W: int):
-        """The captured chain: {"rgb", "flow"}, and with bidirectional also {"flow_bw", "occ_fw", "occ_bw"}."""
+        """The captured chain: {"rgb", "flow"}, and with bidirectional also {"flow_bw", "occ_fw", "occ_bw"}; with
+        interpolate {"frames", "flow", "flow_bw", "occ_fw", "occ_bw"}."""
         B = self.batch
         x = F.permute(0, 3, 1, 2).contiguous()
         a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
@@ -79,12 +95,19 @@ class VideoFlowPredictor:
             return {"rgb": rgb, "flow": flow}
         flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
         flow, flow_bw = flows[:B], flows[B:]
+        if self.interpolate:
+            occ_fw, occ_bw = ops.flow_consistency(flow, flow_bw, self.alpha, self.beta)
+            times = [k / (self.interpolate + 1) for k in range(1, self.interpolate + 1)]
+            frames = ops.interpolate_frames(F[:B], F[1:], flow, flow_bw, occ_fw, occ_bw, times, self.occ_weight)
+            return {"frames": frames, "flow": flow, "flow_bw": flow_bw, "occ_fw": occ_fw, "occ_bw": occ_bw}
         rgb, _ = ops.flow_to_color(flow, self.max_radius, self.bgr)
         occ_fw, occ_bw = ops.flow_consistency(flow, flow_bw, self.alpha, self.beta)
         return {"rgb": rgb, "flow": flow, "flow_bw": flow_bw, "occ_fw": occ_fw, "occ_bw": occ_bw}
 
     def _outputs(self):
         """The chain outputs that leave the GPU, in the order of a result."""
+        if self.interpolate:
+            return ("frames", "flow", "flow_bw", "occ_fw", "occ_bw") if self.want_flow else ("frames",)
         if not self.bidirectional:
             return ("rgb", "flow") if self.want_flow else ("rgb",)
         return ("rgb", "flow", "flow_bw", "occ_fw", "occ_bw") if self.want_flow else ("rgb", "occ_fw", "occ_bw")

@@ -45,6 +45,39 @@ def load_model(name: str, checkpoint: str, device="cuda") -> torch.nn.Module:
     return model.to(device).eval()
 
 
+def open_video(path: str):
+    """(cv2.VideoCapture, frame rate) of a video file; the rate is 0 when the container does not give one."""
+    import cv2
+
+    cap = cv2.VideoCapture(path)
+    if not cap.isOpened():
+        raise FileNotFoundError(f"cannot open video {path}")
+    return cap, cap.get(cv2.CAP_PROP_FPS)
+
+
+def video_frames(cap):
+    """The frames of an open cv2.VideoCapture (H,W,3) uint8 B,G,R, in order; releases it at the end."""
+    try:
+        while True:
+            ok, frame = cap.read()
+            if not ok:
+                return
+            yield frame
+    finally:
+        cap.release()
+
+
+def open_video_writer(path: str, fps: float, shape):
+    """cv2.VideoWriter of (H,W,...) frames at `fps` (25 when fps is not positive): MJPG for .avi, mp4v otherwise."""
+    import cv2
+
+    fourcc = cv2.VideoWriter_fourcc(*("MJPG" if path.lower().endswith(".avi") else "mp4v"))
+    w = cv2.VideoWriter(path, fourcc, fps if fps > 0 else 25.0, (shape[1], shape[0]))
+    if not w.isOpened():
+        raise OSError(f"cannot write {path}")
+    return w
+
+
 def _imread(cv2, path):
     img = cv2.imread(path)
     if img is None:
@@ -79,40 +112,19 @@ def predict_files(model: torch.nn.Module, flow_filepath: str, image_1=None, imag
             raise OSError(f"cannot write {flow_filepath}")
         return 1
 
-    cap = cv2.VideoCapture(video_filepath)
-    if not cap.isOpened():
-        raise FileNotFoundError(f"cannot open video {video_filepath}")
-    fps = cap.get(cv2.CAP_PROP_FPS)
-
-    def frames():
-        try:
-            while True:
-                ok, frame = cap.read()
-                if not ok:
-                    return
-                yield frame
-        finally:
-            cap.release()
-
+    cap, fps = open_video(video_filepath)
     bidirectional = occlusion_filepath is not None
     pred = VideoFlowPredictor(model, batch=batch, resize=resize, max_radius=max_radius, bgr=True,
                               bidirectional=bidirectional)
 
-    def open_writer(path, shape):
-        fourcc = cv2.VideoWriter_fourcc(*("MJPG" if path.lower().endswith(".avi") else "mp4v"))
-        w = cv2.VideoWriter(path, fourcc, fps if fps > 0 else 25.0, (shape[1], shape[0]))
-        if not w.isOpened():
-            raise OSError(f"cannot write {path}")
-        return w
-
     writers, n = [], 0
     try:
-        for res in pred.run(frames()):
+        for res in pred.run(video_frames(cap)):
             rgb = res[0] if bidirectional else res
             if not writers:
-                writers.append(open_writer(flow_filepath, rgb.shape))
+                writers.append(open_video_writer(flow_filepath, fps, rgb.shape))
                 if bidirectional:
-                    writers.append(open_writer(occlusion_filepath, rgb.shape))
+                    writers.append(open_video_writer(occlusion_filepath, fps, rgb.shape))
             writers[0].write(rgb)
             if bidirectional:   # grey frames through the colour writer: 255 = occluded in all three channels
                 writers[1].write(cv2.cvtColor(res[1] * 255, cv2.COLOR_GRAY2BGR))
