@@ -370,6 +370,70 @@ MFN_API int mfn_flow_consistency(const float* flow_fw, const float* flow_bw, uns
                                  int N, int H, int W, float alpha, float beta, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Dense point tracking (Sundaram, Brox and Keutzer, ECCV 2010): tracks chained along the forward flow, stopped by the
+ * forward-backward check or at motion boundaries, and reseeded on a grid where textured cells are uncovered.
+ * Frames 0..T-1 of H x W; flow_fw of frame k -> k+1 and flow_bw of k+1 -> k are (H,W,2) float32 (x,y) pixels (the layout
+ * mfn_postprocess_forward writes), 8-byte aligned.  The tracker holds K slots, the first M of them for the queries.  Each
+ * slot holds at most one track: pos (K,2) float32 (x,y), 8-byte aligned, and a status byte per slot and frame:
+ *   0 EMPTY     no track in this slot in this frame
+ *   1 TRACKED   a track continued into this frame
+ *   2 BORN      a track started in this frame (seed or query)
+ *   3 LEFT      the track's last frame was the previous one: its target was non-finite or left the frame
+ *   4 OCCLUDED  the same, ended by the forward-backward check
+ *   5 BOUNDARY  the same, ended by the motion-boundary test
+ * A stopped slot's position is NaN in that frame, and the slot may be seeded again from the next frame on.  Every live
+ * (TRACKED or BORN) position lies inside [0,W-1] x [0,H-1].
+ *
+ * mfn_track_advance: frame k -> k+1 for every slot.  A slot that is not live in frame k becomes EMPTY.  A live slot at p:
+ *   1. w = flow_fw sampled bilinearly at p: corners x0 = floor(px), x1 = min(x0+1, W-1), the same in y, weights
+ *      p - floor(p) (mfn_flow_consistency's rule).
+ *   2. q = p + w in float32.  Non-finite or outside [0,W-1] x [0,H-1]: LEFT.
+ *   3. b = flow_bw sampled at q with the same rule.  OCCLUDED unless |w+b|^2 <= alpha (|w|^2 + |b|^2) + beta with that
+ *      right-hand side finite.
+ *   4. At the pixel nearest p (rint, ties to even, clamped to the frame), central differences of flow_fw with the
+ *      neighbours clamped to the frame, divided by their index distance (0 where the extent is 1); g = the sum of their
+ *      four squares.  BOUNDARY unless g <= alpha_b |w|^2 + beta_b.
+ *   5. Otherwise TRACKED at q.
+ *   The first test that fires wins.  Then `cells` (Gy,Gx) uint8 is zeroed and each TRACKED slot sets the cell
+ *   (floor(qx) / h, floor(qy) / h) if it lies inside the grid.  alpha = 0.01, beta = 0.5 as mfn_flow_consistency;
+ *   alpha_b = 0.01, beta_b = 0.002 the paper's motion-boundary constants.
+ * Grid: spacing h >= 1, Gx = W / h, Gy = H / h cells (integer division); cell (i,j) covers [ih,(i+1)h) x [jh,(j+1)h) and
+ *   its seed point is (ih + h/2, jh + h/2), h/2 in integers.
+ * mfn_track_texture: for each of F frames (F,H,W,3) uint8 and each seed point, lambda2 (F,Gy,Gx) float64, the smaller
+ *   eigenvalue of the structure tensor: grey I = R+G+B (any channel order), gx = I(x+1,y) - I(x-1,y), gy likewise,
+ *   coordinates clamped to the frame; (a,b,c) = the sums of (gx^2, gx gy, gy^2) over the 5x5 window around the seed point
+ *   (window coordinates clamped), exact in int32; lambda2 = max(0, (a+c)/2 - sqrt(((a-c)/2)^2 + b^2)) in float64, every
+ *   intermediate exact and the square root correctly rounded, so the value is reproducible bit for bit anywhere.
+ *   lambda_max (F) float64: each frame's largest lambda2 (0 without seed points).
+ * mfn_track_seed: the births of the frame f = *frame, after its advance (or after a reset, for frame 0); then *frame = f+1.
+ *   - Query births: queries (M,3) float32 rows (t, x, y).  Query i with t == f is BORN at (x,y) in slot i if (x,y) lies
+ *     inside [0,W-1] x [0,H-1] (and covers its cell like a TRACKED slot); otherwise LEFT, with a NaN position.
+ *   - Covered cells: `cells` as the advance left it, plus the query births.
+ *   - Candidates: the uncovered cells with lambda2 > 0 and lambda2 >= tau lambda_max (the product in float64 from the
+ *     float32 tau).  A flat frame seeds nothing.
+ *   - Assignment: the n-th candidate in row-major cell order is BORN at its seed point in the n-th free slot in slot order;
+ *     the free slots are the slots M..K-1 that are EMPTY after the advance.  *dropped = the candidates left without a slot.
+ *   - out_pos (K,2), out_status (K), optional (both null or neither): a copy of the frame's state.
+ *   ws: caller-owned, mfn_track_seed_workspace_bytes(K) = 4 K bytes, 4-byte aligned.
+ * A video starts from pos = NaN, status = EMPTY, *frame = 0: mfn_track_texture of frame 0 and mfn_track_seed.  Each next
+ * frame is mfn_track_advance and mfn_track_seed; mfn_track_texture may cover many frames in one call.  No float atomics
+ * (deterministic), no allocation, no host synchronisation, launch configurations depend on the extents only: a sequence
+ * of calls is capture-safe and replayable.  A null pointer, an extent below 1, spacing below 1, a negative or non-finite
+ * constant, a misaligned pointer, M outside [0,K] or a short workspace returns MFN_ERR_INVALID_ARG; H*W >= 2^31 or
+ * F > 65535 returns MFN_ERR_ALIGNMENT.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API int mfn_track_texture(const unsigned char* frames, double* lambda2, double* lambda_max, int F, int H, int W,
+                              int spacing, void* stream);
+MFN_API int mfn_track_advance(const float* flow_fw, const float* flow_bw, float* pos, unsigned char* status,
+                              unsigned char* cells, int K, int H, int W, int spacing, float alpha, float beta, float alpha_b,
+                              float beta_b, void* stream);
+MFN_API long long mfn_track_seed_workspace_bytes(int K);
+MFN_API int mfn_track_seed(const double* lambda2, const double* lambda_max, const float* queries, int M, float* pos,
+                           unsigned char* status, unsigned char* cells, int* frame, int* dropped, void* ws,
+                           long long ws_bytes, float* out_pos, unsigned char* out_status, int K, int H, int W, int spacing,
+                           float tau, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Frame interpolation from bidirectional flow: occlusion-weighted forward splatting of both images of each pair.
  *   img0, img1 (N,H,W,3) uint8 (any channel order); flow_fw (img0 -> img1), flow_bw (img1 -> img0) (N,H,W,2) float32,
  *   (x,y) pixels, 8-byte aligned; occ_fw, occ_bw (N,H,W) uint8 (mfn_flow_consistency's masks, nonzero = occluded);

@@ -40,6 +40,10 @@ SIGNATURES = {
     "mfn_postprocess_forward": [_f, _f, _i, _i, _i, _i, _i, _i, _i, _i, _f],
     "mfn_flow_to_color": [_f, _f, _f, _i, _i, _i, _fl, _i, _f],
     "mfn_flow_consistency": [_f, _f, _f, _f, _i, _i, _i, _fl, _fl, _f],
+    "mfn_track_texture": [_f, _f, _f, _i, _i, _i, _i, _f],
+    "mfn_track_advance": [_f] * 5 + [_i] * 4 + [_fl] * 4 + [_f],
+    "mfn_track_seed_workspace_bytes": [_i],
+    "mfn_track_seed": [_f, _f, _f, _i, _f, _f, _f, _f, _f, _f, _ll, _f, _f, _i, _i, _i, _i, _fl, _f],
     "mfn_interpolate_frames_workspace_bytes": [_i, _i, _i],
     "mfn_interpolate_frames": [_f] * 8 + [_ll, _i, _i, _i, _f, _i, _fl, _f],
     "mfn_warp_mask_backward_det": [_f] * 14 + [_i] * 5 + [_fl, _fl, _fl, _i, _f, _ll, _f],
@@ -65,7 +69,7 @@ SIGNATURES = {
     "mfn_bf16_pack": [_f, _ll, _i, _i, _i, _i, _f, _i, _i, _f],
 }
 # entries of SIGNATURES that do not return an int status
-RESTYPES = {"mfn_interpolate_frames_workspace_bytes": _ll}
+RESTYPES = {"mfn_interpolate_frames_workspace_bytes": _ll, "mfn_track_seed_workspace_bytes": _ll}
 
 
 class MaskflowError(RuntimeError):

@@ -14,34 +14,9 @@
 
 #include "common.cuh"
 #endif
+#include "flowcheck.cuh"   // fb_occluded
 
 namespace mfn {
-
-__device__ __forceinline__ float fb_lerp(float p, float q, float w) { return p * (1.f - w) + q * w; }
-
-// 1 where the pixel (x, y) with flow uv has no consistent match in `other` (the H x W flow plane of the other direction):
-// its target (x+u, y+v) lies outside [0, W-1] x [0, H-1] (NaN included), or the other flow sampled bilinearly there,
-// (bu, bv), fails |uv + (bu,bv)|^2 <= alpha (|uv|^2 + |(bu,bv)|^2) + beta with a finite right-hand side: NaN or inf
-// anywhere fails (an inf corner reaches the sample as inf, or as NaN where its weight is 0: both give 1).  Inside the
-// frame the four corners are x0 = floor(qx), x1 = min(x0 + 1, W - 1), and the same in y, so every read is inside the
-// plane.
-__device__ __forceinline__ unsigned char fb_occluded(const float2* __restrict__ other, int H, int W, int x, int y,
-                                                     float2 uv, float alpha, float beta) {
-  const float qx = (float)x + uv.x, qy = (float)y + uv.y;
-  if (!(qx >= 0.f && qx <= (float)(W - 1) && qy >= 0.f && qy <= (float)(H - 1))) return 1;
-  const int x0 = (int)floorf(qx), y0 = (int)floorf(qy);
-  const int x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
-  const float wx = qx - (float)x0, wy = qy - (float)y0;
-  const float2 a = __ldg(other + (size_t)y0 * W + x0), b = __ldg(other + (size_t)y0 * W + x1);
-  const float2 c = __ldg(other + (size_t)y1 * W + x0), d = __ldg(other + (size_t)y1 * W + x1);
-  const float bu = fb_lerp(fb_lerp(a.x, b.x, wx), fb_lerp(c.x, d.x, wx), wy);
-  const float bv = fb_lerp(fb_lerp(a.y, b.y, wx), fb_lerp(c.y, d.y, wx), wy);
-  const float su = uv.x + bu, sv = uv.y + bv;
-  const float d2 = su * su + sv * sv;
-  const float m2 = uv.x * uv.x + uv.y * uv.y + bu * bu + bv * bv;
-  const float rhs = alpha * m2 + beta;
-  return d2 <= rhs && rhs <= 3.402823466e38f ? 0 : 1;   // rhs <= FLT_MAX: finite
-}
 
 // grid (ceil(HW / blockDim), N, 2): z = 0 writes occ_fw from flow_fw against flow_bw, z = 1 the reverse.
 __global__ void __launch_bounds__(256)

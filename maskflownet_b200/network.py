@@ -588,6 +588,38 @@ def interpolate_frames(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, t
     return ops.interpolate_frames(a, b, flow_fw, flow_bw, occ_fw, occ_bw, ts, occ_weight)
 
 
+@torch.no_grad()
+def track_video(net: nn.Module, frames: torch.Tensor, batch: int = 8, resize=None, spacing: int = 8, tau: float = 0.001,
+                alpha: float = 0.01, beta: float = 0.5, boundary=(0.01, 0.002), max_tracks=None, queries=None):
+    """Dense point tracks through a clip of uint8 frames (T,H,W,3) on the device, any channel order (ops.TrackState
+    for the arguments; include/maskflow_b200.h, "Dense point tracking").  Frame 0 is seeded; then the pairs go through
+    predict_bidirectional `batch` at a time (the last batch padded with the last frame, as video.VideoTracker does), the
+    texture of each batch's frames in one ops.track_texture, and per pair ops.track_advance and ops.track_seed.  This is
+    the eager chain VideoTracker captures.  Returns (xy (T,K,2) float32, status (T,K) uint8, dropped (T,) int32) on the
+    device: every slot's position and status in every frame, and the seeding candidates left without a slot."""
+    if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+        raise ops.MaskflowError("track_video: frames must be a (T,H,W,3) uint8 tensor")
+    if batch < 1:
+        raise ops.MaskflowError(f"track_video: batch must be >= 1, got {batch}")
+    T, H, W, _ = frames.shape
+    st = ops.TrackState(H, W, spacing, tau, alpha, beta, boundary, max_tracks, queries, device=frames.device)
+    xy = torch.empty((T, st.K, 2), dtype=torch.float32, device=frames.device)
+    status = torch.empty((T, st.K), dtype=torch.uint8, device=frames.device)
+    dropped = torch.empty((T,), dtype=torch.int32, device=frames.device)
+    ops.track_start(st, frames[0].contiguous(), xy[0], status[0], dropped[0:1])
+    P = T - 1
+    for k0 in range(0, P, batch):
+        F = frames[[min(k0 + j, P) for j in range(batch + 1)]]
+        x = F.permute(0, 3, 1, 2).contiguous()
+        flow_fw, flow_bw, _, _ = predict_bidirectional(net, x[:batch], x[1:], resize, alpha, beta)
+        lam, lmax = ops.track_texture(F, spacing)
+        for j in range(min(batch, P - k0)):
+            k = k0 + j + 1
+            ops.track_advance(st, flow_fw[j], flow_bw[j])
+            ops.track_seed(st, lam[j + 1], lmax[j + 1:j + 2], xy[k], status[k], dropped[k:k + 1])
+    return xy, status, dropped
+
+
 def precision_key(net: nn.Module) -> Tuple[str, ...]:
     """The inference_precision of every flow network inside `net` (the cascade's head may be set on its own): what a
     captured graph depends on besides the input shape."""

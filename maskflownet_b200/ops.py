@@ -881,6 +881,167 @@ def interpolate_frames(img0: torch.Tensor, img1: torch.Tensor, flow_fw: torch.Te
 
 
 # ----------------------------------------------------------------------------------------------------------
+# Dense point tracking (csrc/track.cu)
+# ----------------------------------------------------------------------------------------------------------
+TRACK_EMPTY, TRACK_TRACKED, TRACK_BORN, TRACK_LEFT, TRACK_OCCLUDED, TRACK_BOUNDARY = range(6)
+
+
+def _finite_nonneg(v) -> bool:
+    try:
+        return 0.0 <= float(v) < float("inf")
+    except (TypeError, ValueError):
+        return False
+
+
+class TrackState:
+    """Device-side state of the dense point tracker (include/maskflow_b200.h, "Dense point tracking") for H x W frames.
+
+    pos (K,2) float32 (x,y) and status (K,) uint8 (TRACK_EMPTY ... TRACK_BOUNDARY) of the slots in the current frame;
+    cells (Gy,Gx) uint8, the cells its live tracks cover; frame (1,) int32, the index of the next frame to seed; dropped
+    (1,) int32, the candidates of the last seeded frame left without a slot; and the seed kernel's workspace.  Slots
+    0..M-1 belong to `queries`, M rows (t, x, y) with t an integer frame index; max_tracks dense slots follow (default
+    2 Gx Gy, Gx = W // spacing, Gy = H // spacing).  tau: the texture threshold relative to the frame's largest; alpha,
+    beta: the forward-backward check; boundary: (alpha_b, beta_b) of the motion-boundary test.  Everything is allocated
+    here once: the track_* ops write into it and allocate nothing else for the state, so a sequence of them can be
+    captured in a CUDA graph.  reset() returns it to the start of a video."""
+
+    def __init__(self, H: int, W: int, spacing: int = 8, tau: float = 0.001, alpha: float = 0.01, beta: float = 0.5,
+                 boundary=(0.01, 0.002), max_tracks: Optional[int] = None, queries=None, device=None):
+        if not (isinstance(spacing, int) and not isinstance(spacing, bool) and spacing >= 1):
+            raise MaskflowError(f"TrackState: spacing must be an integer >= 1, got {spacing!r}")
+        if int(H) < 1 or int(W) < 1 or int(H) * int(W) >= 1 << 31:
+            raise MaskflowError(f"TrackState: frame size {H}x{W} outside 1 <= H, W and H*W < 2^31")
+        try:
+            ab, bb = boundary
+        except (TypeError, ValueError):
+            raise MaskflowError(f"TrackState: boundary must be a pair (alpha_b, beta_b), got {boundary!r}") from None
+        for v, nm in ((tau, "tau"), (alpha, "alpha"), (beta, "beta"), (ab, "boundary alpha_b"), (bb, "boundary beta_b")):
+            if not _finite_nonneg(v):
+                raise MaskflowError(f"TrackState: {nm} must be finite and non-negative, got {v!r}")
+        q = torch.zeros((0, 3), dtype=torch.float32) if queries is None else torch.as_tensor(queries).detach()
+        if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_complex:
+            raise MaskflowError(f"TrackState: queries must be (M,3) rows (t, x, y), got {tuple(q.shape)}")
+        q = q.to("cpu", torch.float64)
+        t = q[:, 0]
+        if q.shape[0] and not bool(((t >= 0) & (t < 1 << 24) & (t == torch.floor(t))).all()):
+            raise MaskflowError("TrackState: every query's t must be an integer frame index in [0, 2^24)")
+        self.H, self.W, self.spacing = int(H), int(W), int(spacing)
+        self.Gx, self.Gy = self.W // self.spacing, self.H // self.spacing
+        self.tau, self.alpha, self.beta = float(tau), float(alpha), float(beta)
+        self.boundary = (float(ab), float(bb))
+        self.M = int(q.shape[0])
+        dense = 2 * self.Gx * self.Gy if max_tracks is None else max_tracks
+        if not (isinstance(dense, int) and not isinstance(dense, bool) and dense >= 0):
+            raise MaskflowError(f"TrackState: max_tracks must be a non-negative integer, got {max_tracks!r}")
+        self.K = self.M + dense
+        if self.K < 1 or self.K >= 1 << 31:
+            raise MaskflowError(f"TrackState: {self.K} slots ({self.M} queries, {dense} dense): need 1 <= K < 2^31")
+        dev = torch.device("cuda") if device is None else torch.device(device)
+        self.pos = torch.empty((self.K, 2), dtype=torch.float32, device=dev)
+        self.device = dev = self.pos.device          # with its index: tensors are compared against it
+        self.queries = q.to(dev, torch.float32).contiguous()
+        self.status = torch.empty((self.K,), dtype=torch.uint8, device=dev)
+        self.cells = torch.zeros((self.Gy, self.Gx), dtype=torch.uint8, device=dev)
+        self.frame = torch.empty((1,), dtype=torch.int32, device=dev)
+        self.dropped = torch.empty((1,), dtype=torch.int32, device=dev)
+        self.ws_bytes = int(_lib.lib().mfn_track_seed_workspace_bytes(self.K))
+        self.ws = torch.empty((self.ws_bytes,), dtype=torch.uint8, device=dev)
+        self.reset()
+
+    def reset(self) -> None:
+        """The start of a video: no tracks (NaN positions, EMPTY, no covered cell), frame 0 next."""
+        self.pos.fill_(float("nan"))
+        self.status.zero_()
+        self.cells.zero_()
+        self.frame.zero_()
+        self.dropped.zero_()
+
+
+def _track_tensor(t, nm: str, dtype, shape, who: str) -> torch.Tensor:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise MaskflowError(f"{who}: {nm} must be a CUDA tensor; the hot path has no CPU implementation")
+    if t.dtype != dtype or not t.is_contiguous():
+        raise MaskflowError(f"{who}: {nm} must be a contiguous {dtype} tensor")
+    if tuple(t.shape) != tuple(shape):
+        raise MaskflowError(f"{who}: expected {nm} of shape {tuple(shape)}, got {tuple(t.shape)}")
+    return t
+
+
+def track_texture(frames: torch.Tensor, spacing: int = 8):
+    """Seed-point texture of uint8 frames (F,H,W,3) (or one (H,W,3) frame), any channel order: the smaller eigenvalue of
+    the 5x5 structure tensor of R+G+B at each seed point (i h + h/2, j h + h/2), h = spacing, exact in float64
+    (include/maskflow_b200.h, mfn_track_texture).  Returns (lambda2 (F,Gy,Gx) float64, lambda_max (F,) float64, each
+    frame's largest); an (H,W,3) frame gives (Gy,Gx) and (1,)."""
+    if not isinstance(frames, torch.Tensor) or frames.dim() not in (3, 4):
+        raise MaskflowError("track_texture: frames must be an (F,H,W,3) or (H,W,3) uint8 CUDA tensor")
+    f4 = frames if frames.dim() == 4 else frames.unsqueeze(0)
+    F, H, W = (int(s) for s in f4.shape[:3])
+    _track_tensor(f4, "frames", torch.uint8, (F, H, W, 3), "track_texture")
+    if not (isinstance(spacing, int) and spacing >= 1):
+        raise MaskflowError(f"track_texture: spacing must be an integer >= 1, got {spacing!r}")
+    lam = torch.empty((F, H // spacing, W // spacing), dtype=torch.float64, device=f4.device)
+    lmax = torch.empty((F,), dtype=torch.float64, device=f4.device)
+    _call("mfn_track_texture", f4.device, _p(f4), _p(lam), _p(lmax), F, H, W, int(spacing))
+    return (lam, lmax) if frames.dim() == 4 else (lam[0], lmax)
+
+
+def track_advance(state: TrackState, flow_fw: torch.Tensor, flow_bw: torch.Tensor) -> None:
+    """Moves every track of `state` from frame k to k+1 along flow_fw (k -> k+1) and flow_bw (k+1 -> k), (H,W,2) float32
+    (x,y) pixels: TRACKED at p + flow_fw(p), or stopped LEFT, OCCLUDED (forward-backward check) or BOUNDARY (flow
+    gradient), and marks the cells the tracks cover (include/maskflow_b200.h, mfn_track_advance).  Forward only."""
+    shape = (state.H, state.W, 2)
+    _track_tensor(flow_fw, "flow_fw", torch.float32, shape, "track_advance")
+    _track_tensor(flow_bw, "flow_bw", torch.float32, shape, "track_advance")
+    if flow_fw.device != state.device or flow_bw.device != state.device:
+        raise MaskflowError(f"track_advance: the flows must be on the state's device {state.device}")
+    _no_grad_path("track_advance", flow_fw, flow_bw)
+    ab, bb = state.boundary
+    _call("mfn_track_advance", state.device, _p(flow_fw), _p(flow_bw), _p(state.pos), _p(state.status), _p(state.cells),
+          state.K, state.H, state.W, state.spacing, state.alpha, state.beta, ab, bb)
+
+
+def track_seed(state: TrackState, lambda2: torch.Tensor, lambda_max: torch.Tensor, out_xy=None, out_status=None,
+               out_dropped=None):
+    """The births of the frame `state.frame` (on the device): query births, then new tracks at the seed points of the
+    uncovered cells with lambda2 > 0 and lambda2 >= tau lambda_max, in row-major cell order, into the free dense slots in
+    slot order (include/maskflow_b200.h, mfn_track_seed).  lambda2 (Gy,Gx) and lambda_max (1,) float64 of that frame, as
+    track_texture returns them.  Returns the frame's (xy (K,2) float32, status (K,) uint8, dropped (1,) int32), written
+    into out_xy, out_status and out_dropped when given (dropped defaults to state.dropped)."""
+    _track_tensor(lambda2, "lambda2", torch.float64, (state.Gy, state.Gx), "track_seed")
+    _track_tensor(lambda_max, "lambda_max", torch.float64, (1,), "track_seed")
+    xy = torch.empty((state.K, 2), dtype=torch.float32, device=state.device) if out_xy is None else out_xy
+    st = torch.empty((state.K,), dtype=torch.uint8, device=state.device) if out_status is None else out_status
+    dropped = state.dropped if out_dropped is None else out_dropped
+    _track_tensor(xy, "out_xy", torch.float32, (state.K, 2), "track_seed")
+    _track_tensor(st, "out_status", torch.uint8, (state.K,), "track_seed")
+    _track_tensor(dropped, "out_dropped", torch.int32, (1,), "track_seed")
+    for t in (lambda2, lambda_max, xy, st, dropped):
+        if t.device != state.device:
+            raise MaskflowError(f"track_seed: every tensor must be on the state's device {state.device}")
+    _call("mfn_track_seed", state.device, _p(lambda2), _p(lambda_max), _p(state.queries) if state.M else None, state.M,
+          _p(state.pos), _p(state.status), _p(state.cells), _p(state.frame), _p(dropped), _p(state.ws), state.ws_bytes,
+          _p(xy), _p(st), state.K, state.H, state.W, state.spacing, state.tau)
+    return xy, st, dropped
+
+
+def track_start(state: TrackState, frame: torch.Tensor, out_xy=None, out_status=None, out_dropped=None):
+    """Frame 0 of a video: state.reset(), then the seeds (and the queries born) in `frame` (H,W,3) uint8.  Returns
+    track_seed's (xy, status, dropped)."""
+    state.reset()
+    lam, lmax = track_texture(frame, state.spacing)
+    return track_seed(state, lam, lmax, out_xy, out_status, out_dropped)
+
+
+def track_step(state: TrackState, flow_fw: torch.Tensor, flow_bw: torch.Tensor, frame: torch.Tensor, out_xy=None,
+               out_status=None, out_dropped=None):
+    """One frame k -> k+1: track_advance along the pair's flows, then track_seed in frame k+1 (H,W,3) uint8.  Returns
+    track_seed's (xy, status, dropped)."""
+    track_advance(state, flow_fw, flow_bw)
+    lam, lmax = track_texture(frame, state.spacing)
+    return track_seed(state, lam, lmax, out_xy, out_status, out_dropped)
+
+
+# ----------------------------------------------------------------------------------------------------------
 # Unsupervised losses (csrc/unsup_loss.cu): census photometric loss and second-order smoothness
 # ----------------------------------------------------------------------------------------------------------
 def unsup_workspace_bytes(loss: str, N: int, H: int, W: int) -> int:

@@ -16,13 +16,18 @@ With interpolate=T the chain continues into ops.interpolate_frames, which reads 
 the colour coding is skipped:
     preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  flow_consistency
     ->  interpolate_frames(F[:B], F[1:], ...) at the times k / (T+1), k = 1..T
+VideoTracker extends the bidirectional chain with dense point tracking (ops.track_*) and yields one TrackFrame per
+video frame:
+    preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  track_texture(F)
+    ->  per pair: track_advance, track_seed
 Copies follow network.PipelinedFlowPredictor's slot scheme: pinned host staging, H2D on one copy stream, D2H of the colours
 (and flows) on another, `depth` slots, so the copies of neighbouring batches run under the replay of this one.
 """
 from __future__ import annotations
 
 import collections
-from typing import Iterable, Iterator
+import itertools
+from typing import Iterable, Iterator, NamedTuple
 
 import numpy as np
 import torch
@@ -165,6 +170,7 @@ class VideoFlowPredictor:
         F = st["F"]
         if first:
             F.copy_(s["in"])
+            self._start(st)
         else:
             F[0].copy_(F[B])
             F[1:].copy_(s["in"][:B])
@@ -182,6 +188,9 @@ class VideoFlowPredictor:
             s["ev_out_free"].record(d2h)
         s["used"] = True
         return s
+
+    def _start(self, st) -> None:
+        """Runs on the compute stream once per video, after frame 0 is in the frame buffer and before the first replay."""
 
     def _collect(self, s, b: int) -> Iterator:
         s["ev_out_free"].synchronize()
@@ -230,3 +239,179 @@ class VideoFlowPredictor:
                 pending.append((self._submit(st, buf, first_batch), pairs))
         while pending:
             yield from self._collect(*pending.popleft())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Dense point tracking
+# ---------------------------------------------------------------------------------------------------------------------
+class TrackFrame(NamedTuple):
+    """The tracks of one video frame.  ids (n,) int64, xy (n,2) float32 (x,y) pixels and born (n,) bool: the tracks alive
+    in this frame (born: started in it); ended_ids (m,) int64 and ended_reason (m,) uint8 (ops.TRACK_LEFT,
+    TRACK_OCCLUDED or TRACK_BOUNDARY): the tracks whose last frame was the previous one.  Query i has id i and is reported
+    as ended with TRACK_LEFT in its frame if its point lies outside the frame; dense tracks count on from the number of
+    queries, in order of birth frame, then slot."""
+    ids: np.ndarray
+    xy: np.ndarray
+    born: np.ndarray
+    ended_ids: np.ndarray
+    ended_reason: np.ndarray
+
+
+class _TrackIds:
+    """Host bookkeeping: slot -> track id, from each frame's slot positions and status bytes."""
+
+    def __init__(self, M: int):
+        self.M, self.next, self.slot = M, M, None
+
+    def frame(self, xy: np.ndarray, status: np.ndarray) -> TrackFrame:
+        if self.slot is None:
+            self.slot = np.full(len(status), -1, np.int64)
+            self.slot[:self.M] = np.arange(self.M)
+        born = status == ops.TRACK_BORN
+        new = np.flatnonzero(born[self.M:]) + self.M
+        self.slot[new] = np.arange(self.next, self.next + len(new))
+        self.next += len(new)
+        alive = born | (status == ops.TRACK_TRACKED)
+        ended = status >= ops.TRACK_LEFT
+        res = TrackFrame(self.slot[alive], xy[alive], born[alive], self.slot[ended], status[ended])
+        ended[:self.M] = False
+        self.slot[ended] = -1                 # a dense slot may be seeded again from the next frame on
+        return res
+
+
+def track_frames(xy, status, num_queries: int = 0) -> Iterator[TrackFrame]:
+    """TrackFrames from per-frame slot arrays, xy (T,K,2) and status (T,K) (network.track_video's first two results,
+    on the host), num_queries = M."""
+    ids = _TrackIds(int(num_queries))
+    for k in range(len(status)):
+        yield ids.frame(np.asarray(xy[k]), np.asarray(status[k]))
+
+
+def collect_tracks(frames: Iterable[TrackFrame]):
+    """Ragged arrays of the tracks in a sequence of TrackFrames (frame 0 first), indexed by track id: "start" (n,) int64,
+    the first frame (-1 for an id never seen); "length" (n,) int64, the frames it was alive in; "offset" (n,) int64 into
+    "xy" (sum(length), 2) float32, its positions frame by frame; "reason" (n,) uint8, how it ended (0 = still alive in the
+    last frame).  A query whose point lay outside its frame has length 0, its frame as start and reason TRACK_LEFT."""
+    ids, ts, xys, eids, ets, ereasons = [], [], [], [], [], []
+    for t, fr in enumerate(frames):
+        ids.append(np.asarray(fr.ids, np.int64))
+        ts.append(np.full(len(fr.ids), t, np.int64))
+        xys.append(np.asarray(fr.xy, np.float32).reshape(-1, 2))
+        eids.append(np.asarray(fr.ended_ids, np.int64))
+        ets.append(np.full(len(fr.ended_ids), t, np.int64))
+        ereasons.append(np.asarray(fr.ended_reason, np.uint8))
+    cat = lambda a, dt: np.concatenate(a) if a else np.zeros(0, dt)   # noqa: E731
+    ids, ts, eids, ets, ereasons = cat(ids, np.int64), cat(ts, np.int64), cat(eids, np.int64), cat(ets, np.int64), \
+        cat(ereasons, np.uint8)
+    xy = np.concatenate(xys) if xys else np.zeros((0, 2), np.float32)
+    n = int(max(ids.max(initial=-1), eids.max(initial=-1))) + 1
+    order = np.argsort(ids, kind="stable")
+    length = np.bincount(ids, minlength=n).astype(np.int64)
+    offset = np.cumsum(length) - length
+    start = np.full(n, -1, np.int64)
+    has = length > 0
+    start[has] = ts[order][offset[has]]
+    reason = np.zeros(n, np.uint8)
+    reason[eids] = ereasons
+    unborn = np.zeros(n, bool)
+    unborn[eids] = True
+    unborn &= ~has
+    start[eids[unborn[eids]]] = ets[unborn[eids]]
+    return {"start": start, "length": length, "offset": offset, "xy": xy[order], "reason": reason}
+
+
+class VideoTracker(VideoFlowPredictor):
+    """Dense point tracks through a video, streamed: run(frames) yields one TrackFrame per video frame, frame 0 included.
+
+    The pairs go through VideoFlowPredictor's bidirectional machinery (frame buffer, pinned slots, copy streams, one CUDA
+    graph per frame size and network.precision_key), and the graph continues after postprocess with the tracking steps
+    of network.track_video: one ops.track_texture over the batch's B+1 frames, then per pair ops.track_advance and
+    ops.track_seed.  The tracker's state (ops.TrackState: spacing, tau, alpha, beta, boundary, max_tracks, queries) lives
+    on the device; run() resets it and seeds frame 0 before its first replay.  Only the slot positions and status bytes
+    cross PCIe (9 bytes per slot and frame); track ids are assigned on the host.  The padded tail of a partial batch is
+    discarded.  frames: host uint8 (H,W,3) arrays or tensors, any channel order.  collect_tracks turns the TrackFrames
+    into ragged arrays."""
+
+    def __init__(self, net: nn.Module, batch: int = 8, resize=None, spacing: int = 8, tau: float = 0.001,
+                 alpha: float = 0.01, beta: float = 0.5, boundary=(0.01, 0.002), max_tracks=None, queries=None,
+                 depth: int = 2):
+        super().__init__(net, batch=batch, resize=resize, depth=depth, bidirectional=True, alpha=alpha, beta=beta)
+        self.track_args = dict(spacing=spacing, tau=tau, alpha=alpha, beta=beta, boundary=boundary, max_tracks=max_tracks,
+                               queries=None if queries is None else np.asarray(queries, np.float64))
+        if not (isinstance(spacing, int) and not isinstance(spacing, bool) and spacing >= 1):
+            raise MaskflowError(f"VideoTracker: spacing must be an integer >= 1, got {spacing!r}")
+        q = self.track_args["queries"]
+        if q is not None and (q.ndim != 2 or q.shape[1] != 3):
+            raise MaskflowError(f"VideoTracker: queries must be (M,3) rows (t, x, y), got {q.shape}")
+        self.num_queries = 0 if q is None else int(q.shape[0])
+        self._tracks = {}
+        self._first = None
+
+    def invalidate(self) -> None:
+        super().invalidate()
+        self._tracks.clear()
+
+    def _track(self, H: int, W: int, dev: torch.device):
+        """The device state of H x W videos and the buffers of frame 0's result."""
+        e = self._tracks.get((H, W))
+        if e is None:
+            st = ops.TrackState(H, W, **self.track_args, device=dev)
+            e = self._tracks[(H, W)] = {
+                "state": st, "xy0": torch.empty((st.K, 2), dtype=torch.float32, device=dev),
+                "status0": torch.empty((st.K,), dtype=torch.uint8, device=dev),
+                "dropped0": torch.empty((1,), dtype=torch.int32, device=dev),
+                "xy0_host": torch.empty((st.K, 2), dtype=torch.float32, pin_memory=True),
+                "status0_host": torch.empty((st.K,), dtype=torch.uint8, pin_memory=True), "ev0": torch.cuda.Event()}
+        return e
+
+    def _chain(self, F: torch.Tensor, H: int, W: int):
+        B = self.batch
+        st = self._track(H, W, F.device)["state"]
+        x = F.permute(0, 3, 1, 2).contiguous()
+        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
+        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
+        lam, lmax = ops.track_texture(F, st.spacing)
+        xy = torch.empty((B, st.K, 2), dtype=torch.float32, device=F.device)
+        status = torch.empty((B, st.K), dtype=torch.uint8, device=F.device)
+        dropped = torch.empty((B,), dtype=torch.int32, device=F.device)
+        for j in range(B):
+            ops.track_advance(st, flows[j], flows[B + j])
+            ops.track_seed(st, lam[j + 1], lmax[j + 1:j + 2], xy[j], status[j], dropped[j:j + 1])
+        return {"xy": xy, "status": status, "dropped": dropped}
+
+    def _outputs(self):
+        return ("xy", "status")
+
+    def _start(self, st) -> None:
+        F = st["F"]
+        e = self._track(F.shape[1], F.shape[2], F.device)
+        ops.track_start(e["state"], F[0], e["xy0"], e["status0"], e["dropped0"])
+        e["xy0_host"].copy_(e["xy0"], non_blocking=True)
+        e["status0_host"].copy_(e["status0"], non_blocking=True)
+        e["ev0"].record()
+        self._first = e
+
+    def _collect(self, s, b: int) -> Iterator:
+        if self._first is not None:
+            e, self._first = self._first, None
+            e["ev0"].synchronize()
+            yield e["xy0_host"].numpy().copy(), e["status0_host"].numpy().copy()
+        yield from super()._collect(s, b)
+
+    @torch.no_grad()
+    def run(self, frames: Iterable) -> Iterator[TrackFrame]:
+        ids = _TrackIds(self.num_queries)
+        it = iter(frames)
+        head = [fr for fr in (next(it, None), next(it, None)) if fr is not None]
+        if not head:
+            return
+        if len(head) == 1:                   # one frame: no pair, only its seeds
+            fr = self._frame(head[0], None)
+            dev = next(self.net.parameters()).device
+            with torch.cuda.device(dev):
+                e = self._track(int(fr.shape[0]), int(fr.shape[1]), dev)
+                ops.track_start(e["state"], fr.to(dev).contiguous(), e["xy0"], e["status0"], e["dropped0"])
+                yield ids.frame(e["xy0"].cpu().numpy(), e["status0"].cpu().numpy())
+            return
+        for xy, status in super().run(itertools.chain(head, it)):
+            yield ids.frame(xy, status)
