@@ -460,6 +460,45 @@ MFN_API int mfn_interpolate_frames(const unsigned char* img0, const unsigned cha
                                    const float* times_host, int T, float occ_weight, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Video stabilisation: the camera's motion between two frames as a robust affine fit to the flow, and a warp of uint8
+ * frames by per-frame affine maps.
+ *
+ * mfn_affine_motion: flow (N,H,W,2) float32 (x,y) pixels (the layout mfn_postprocess_forward writes), 8-byte aligned.
+ *   Pixel p = (x,y) has target q = p + flow[p] in float64; it is valid when q lies inside [0,W-1] x [0,H-1] (a non-finite
+ *   component is never inside).  Coordinates are normalised for the fit: p^ = (p - c) / s, q^ = (q - c) / s with
+ *   c = ((W-1)/2, (H-1)/2) and s = max(W,H)/2.  Iteration k solves the weighted least squares
+ *     M = sum w phi phi^T,  b_x = sum w phi q^_x,  b_y = sum w phi q^_y,  phi = (x^, y^, 1)   (12 float64 sums)
+ *   by the adjugate of the symmetric M over det(M), and maps the solution back to pixels, A = [L | c + s t - L c] for
+ *   q^ = L p^ + t.  Weights: invalid pixels 0; iteration 0: 1 (plain least squares); iteration k >= 1: the Cauchy weight
+ *   w = 1 / (1 + r^2 / sigma_k^2), r^2 = |A_{k-1} p - q|^2 in pixels under the previous iteration's A (all float64),
+ *   sigma_k = sigma 2^max(0, 4-k) (8 sigma, 4 sigma, 2 sigma, sigma, sigma, ...).
+ *   A solve is well conditioned when the total weight M[2][2] >= 3 and det(M) > 1e-9 (tr(M)/3)^3; otherwise it writes
+ *   the identity, which the next iteration's weights then use.
+ *   affine (N,2,3) float64, 8-byte aligned: the last iteration's A, A [x,y,1]^T ~ p + flow[p].  ok (N) uint8: 1 when the
+ *   last solve was well conditioned.  residual (N,H,W) float32, optional (null: not written), 4-byte aligned:
+ *   float(sqrt(r^2)) under the final A, NaN on invalid pixels.
+ *   Each iteration is two launches: per-CTA float64 partials (each thread's pixels summed in a fixed order, the CTA's
+ *   threads by a fixed tree; the number of CTAs per sample depends on H and W only) and one CTA per sample that adds them
+ *   in a fixed order and solves.  No atomics (bit-reproducible), no allocation, no host synchronisation, a launch count
+ *   fixed by `iterations`: capture-safe.  ws: caller-owned, mfn_affine_motion_workspace_bytes(N,H,W) bytes, 8-byte
+ *   aligned.
+ * mfn_warp_frames_affine: src, out (N,H,W,3) uint8 (any channel order); M (N,2,3) float64 ON THE DEVICE, 8-byte aligned,
+ *   mapping output pixels to source positions.  Output pixel o = (x,y) of sample n, in float64:
+ *     s = M [x,y,1]^T;  s clamped to [0,W-1] x [0,H-1] (fmin(fmax(s, 0), W-1): the border is replicated, NaN gives 0);
+ *     x0 = floor(sx), x1 = min(x0+1, W-1), wx = sx - x0, the same in y (the corner rule of flowcheck.cuh's fb_sample);
+ *     v = (1-wy) ((1-wx) I[y0,x0] + wx I[y0,x1]) + wy ((1-wx) I[y1,x0] + wx I[y1,x1]) per channel, evaluated in that order;
+ *     out = rint(v) (ties to even), clamped to [0,255].
+ *   No atomics, no allocation: deterministic and capture-safe.
+ * A null pointer, an extent below 1, iterations below 1, a non-positive or non-finite sigma, a misaligned pointer or a
+ * short workspace returns MFN_ERR_INVALID_ARG; H*W >= 2^31 or N > 65535 returns MFN_ERR_ALIGNMENT.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API long long mfn_affine_motion_workspace_bytes(int N, int H, int W);
+MFN_API int mfn_affine_motion(const float* flow, double* affine, unsigned char* ok, float* residual, void* ws,
+                              long long ws_bytes, int N, int H, int W, int iterations, float sigma, void* stream);
+MFN_API int mfn_warp_frames_affine(const unsigned char* src, const double* M, unsigned char* out, int N, int H, int W,
+                                   void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Deterministic mode: bit-reproducible variants of the entry points whose default kernels accumulate with fp32 atomics
  * (the scatter of a bilinear sample's gradient to its four corners, per-CTA weight partials, per-slice plane sums).  Same
  * arguments and results as the counterpart named without _det, plus a caller-owned workspace `det_ws` of `det_ws_bytes`

@@ -29,7 +29,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as tF
 
-from . import ops
+from . import camera, ops
 
 PYRAMID_CH = {1: 16, 2: 32, 3: 64, 4: 96, 5: 128, 6: 196}   # network/MaskFlownet.py:79-96
 DECODER_CH = (128, 128, 96, 64, 32)                           # convL_0 .. convL_4 (:102-130)
@@ -618,6 +618,37 @@ def track_video(net: nn.Module, frames: torch.Tensor, batch: int = 8, resize=Non
             ops.track_advance(st, flow_fw[j], flow_bw[j])
             ops.track_seed(st, lam[j + 1], lmax[j + 1:j + 2], xy[k], status[k], dropped[k:k + 1])
     return xy, status, dropped
+
+
+@torch.no_grad()
+def stabilize_video(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=None, radius: int = 15, crop: float = 0.9,
+                    iterations: int = ops.AFFINE_ITERATIONS, sigma: float = ops.AFFINE_SIGMA):
+    """A stabilised clip of uint8 frames (T,H,W,3) on the device, any channel order.  The pairs go through `predict`
+    `batch` at a time (the last batch padded with the last frame, as video.VideoStabilizer does) and each batch's flows
+    through ops.affine_motion(iterations, sigma); camera.camera_path smooths the camera path over `radius` frames and
+    zooms by `crop` (camera.stabilize_path states the rule; a pair whose fit failed, ok False, counts as no motion); one
+    ops.warp_frames_affine warps every frame.  This is the eager chain VideoStabilizer streams.  Returns (stabilised clip
+    (T,H,W,3) uint8 on the device, affine (T-1,2,3) float64 and ok (T-1,) bool on the device, M (T,2,3) float64 on the
+    host: the warp of each frame, output pixel -> source position)."""
+    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
+        raise ops.MaskflowError("stabilize_video: clip must be a (T,H,W,3) uint8 tensor")
+    if batch < 1:
+        raise ops.MaskflowError(f"stabilize_video: batch must be >= 1, got {batch}")
+    camera.check_path_args(radius, crop, "stabilize_video")
+    T, H, W, _ = clip.shape
+    dev = clip.device
+    P = T - 1
+    affine = torch.empty((max(P, 0), 2, 3), dtype=torch.float64, device=dev)
+    ok = torch.empty((max(P, 0),), dtype=torch.bool, device=dev)
+    for k0 in range(0, P, batch):
+        x = clip[[min(k0 + j, P) for j in range(batch + 1)]].permute(0, 3, 1, 2).contiguous()
+        flow, _ = predict(net, x[:batch], x[1:], resize)
+        a, g = ops.affine_motion(flow, iterations, sigma)
+        b = min(batch, P - k0)
+        affine[k0:k0 + b], ok[k0:k0 + b] = a[:b], g[:b]
+    M = camera.camera_path(affine.cpu().numpy(), ok.cpu().numpy(), H, W, radius, crop)
+    out = ops.warp_frames_affine(clip.contiguous(), torch.from_numpy(M).to(dev))
+    return out, affine, ok, M
 
 
 def precision_key(net: nn.Module) -> Tuple[str, ...]:

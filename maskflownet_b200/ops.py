@@ -881,6 +881,77 @@ def interpolate_frames(img0: torch.Tensor, img1: torch.Tensor, flow_fw: torch.Te
 
 
 # ----------------------------------------------------------------------------------------------------------
+# Video stabilisation (csrc/stabilize.cu)
+# ----------------------------------------------------------------------------------------------------------
+# Defaults of the robust fit, from the robustness scene of tests/test_stabilize.py (a known camera map, 0.3 px noise, a
+# square over 30 % of the frame moving 14 px relative to it): the largest error at the frame corners was 0.126 px with
+# 8 iterations at sigma 1, 0.064 px with 8 at 0.5, 0.054 px with 10 at 0.5 and 0.043 px with 10 at 0.25; with the square
+# moving 5.8 px: 0.51, 0.19, 0.14 and 0.099 px.  Cauchy weights never drop an outlier completely, so a smaller sigma and
+# more iterations help; sigma 0.5 keeps inliers with the flow noise of trained networks (about 0.3-0.5 px) weighted.
+AFFINE_ITERATIONS, AFFINE_SIGMA = 10, 0.5
+
+
+def _stab_tensor(t, nm: str, dtype, last, who: str) -> torch.Tensor:
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise MaskflowError(f"{who}: {nm} must be a CUDA tensor; the hot path has no CPU implementation")
+    if t.dtype != dtype or not t.is_contiguous():
+        raise MaskflowError(f"{who}: {nm} must be a contiguous {dtype} tensor")
+    if t.dim() != 4 or t.shape[-1] != last:
+        raise MaskflowError(f"{who}: expected {nm} of shape (N,H,W,{last}), got {tuple(t.shape)}")
+    return t
+
+
+def affine_motion(flow: torch.Tensor, iterations: int = AFFINE_ITERATIONS, sigma: float = AFFINE_SIGMA,
+                  want_residual: bool = False):
+    """The camera's motion between the two images of each pair: a robust affine fit to the flow (include/maskflow_b200.h,
+    mfn_affine_motion).  flow (N,H,W,2) float32 (x,y) pixels, the layout postprocess and network.predict return.  Pixels
+    whose target leaves the frame (or is not finite) are left out; iteration 0 is plain least squares, each later one
+    reweights every pixel by the Cauchy weight 1 / (1 + (r / sigma_k)^2) of its residual r under the previous fit, with
+    sigma_k = sigma 2^max(0, 4-k) annealed from 8 sigma down to sigma (pixels).
+    Returns (affine (N,2,3) float64 with affine @ [x,y,1] ~ [x,y] + flow[y,x], ok (N,) bool[, residual (N,H,W) float32]):
+    ok is False where the last solve was ill conditioned (too few valid pixels, or all of them on one line), and affine is
+    then the identity.  residual: |affine p - q| in pixels under the final fit, NaN where the pixel was left out.
+    Bit-reproducible; a sample's result does not depend on the batch it is in.  Forward only."""
+    if not (isinstance(iterations, int) and not isinstance(iterations, bool) and iterations >= 1):
+        raise MaskflowError(f"affine_motion: iterations must be an integer >= 1, got {iterations!r}")
+    try:
+        good = 0.0 < float(sigma) < float("inf")
+    except (TypeError, ValueError):
+        good = False
+    if not good:
+        raise MaskflowError(f"affine_motion: sigma must be positive and finite, got {sigma!r}")
+    f = _stab_tensor(flow, "flow", torch.float32, 2, "affine_motion")
+    _no_grad_path("affine_motion", f)
+    N, H, W, _ = f.shape
+    dev = f.device
+    affine = torch.empty((N, 2, 3), device=dev, dtype=torch.float64)
+    ok = torch.empty((N,), device=dev, dtype=torch.uint8)
+    residual = torch.empty((N, H, W), device=dev, dtype=torch.float32) if want_residual else None
+    nb = int(_lib.lib().mfn_affine_motion_workspace_bytes(N, H, W))
+    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    _call("mfn_affine_motion", dev, _p(f), _p(affine), _p(ok), _p(residual), _p(ws), nb, N, H, W, int(iterations),
+          float(sigma))
+    return (affine, ok.bool(), residual) if want_residual else (affine, ok.bool())
+
+
+def warp_frames_affine(frames: torch.Tensor, M: torch.Tensor) -> torch.Tensor:
+    """Each frame warped by its affine map (include/maskflow_b200.h, mfn_warp_frames_affine): out[n](o) = frames[n]
+    sampled bilinearly at M[n] @ [o, 1], the position clamped to the frame (the border is replicated), rounded to nearest.
+    frames (N,H,W,3) uint8, any channel order; M (N,2,3) float64 on the same device, output pixel -> source position.
+    Returns (N,H,W,3) uint8.  Deterministic."""
+    fr = _stab_tensor(frames, "frames", torch.uint8, 3, "warp_frames_affine")
+    if not isinstance(M, torch.Tensor) or M.device != fr.device:
+        raise MaskflowError(f"warp_frames_affine: M must be a tensor on {fr.device}")
+    if M.dtype != torch.float64 or not M.is_contiguous() or tuple(M.shape) != (fr.shape[0], 2, 3):
+        raise MaskflowError(f"warp_frames_affine: M must be a contiguous float64 tensor of shape ({fr.shape[0]},2,3), "
+                            f"got {M.dtype} {tuple(M.shape)}")
+    N, H, W, _ = fr.shape
+    out = torch.empty_like(fr)
+    _call("mfn_warp_frames_affine", fr.device, _p(fr), _p(M), _p(out), N, H, W)
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------
 # Dense point tracking (csrc/track.cu)
 # ----------------------------------------------------------------------------------------------------------
 TRACK_EMPTY, TRACK_TRACKED, TRACK_BORN, TRACK_LEFT, TRACK_OCCLUDED, TRACK_BOUNDARY = range(6)

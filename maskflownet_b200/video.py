@@ -20,6 +20,9 @@ VideoTracker extends the bidirectional chain with dense point tracking (ops.trac
 video frame:
     preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  track_texture(F)
     ->  per pair: track_advance, track_seed
+VideoStabilizer extends the one-direction chain with the camera's motion per pair (ops.affine_motion); the camera path is
+smoothed on the host (camera.stabilize_path) and the frames, kept on the device in a ring, are warped outside the graph:
+    preprocess(F[:B], F[1:])  ->  network  ->  postprocess  ->  affine_motion
 Copies follow network.PipelinedFlowPredictor's slot scheme: pinned host staging, H2D on one copy stream, D2H of the colours
 (and flows) on another, `depth` slots, so the copies of neighbouring batches run under the replay of this one.
 """
@@ -33,7 +36,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import network, ops
+from . import camera, network, ops
 from ._lib import MaskflowError
 
 _WARMUP = 2
@@ -174,6 +177,7 @@ class VideoFlowPredictor:
         else:
             F[0].copy_(F[B])
             F[1:].copy_(s["in"][:B])
+        self._loaded(st, first)
         s["ev_in_free"].record(cur)
         st["graph"].replay()
         if s["used"]:
@@ -191,6 +195,10 @@ class VideoFlowPredictor:
 
     def _start(self, st) -> None:
         """Runs on the compute stream once per video, after frame 0 is in the frame buffer and before the first replay."""
+
+    def _loaded(self, st, first: bool) -> None:
+        """Runs on the compute stream once per batch, after the batch's new frames are in the frame buffer (F[0..B] for
+        the first batch of a video, F[1..B] afterwards) and before its replay."""
 
     def _collect(self, s, b: int) -> Iterator:
         s["ev_out_free"].synchronize()
@@ -415,3 +423,156 @@ class VideoTracker(VideoFlowPredictor):
             return
         for xy, status in super().run(itertools.chain(head, it)):
             yield ids.frame(xy, status)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Video stabilisation
+# ---------------------------------------------------------------------------------------------------------------------
+class VideoStabilizer(VideoFlowPredictor):
+    """A stabilised video, streamed: run(frames) yields one stabilised (H,W,3) uint8 frame per input frame, frame 0
+    included, in order, `radius` frames behind the input.
+
+    The pairs go through VideoFlowPredictor's one-direction machinery (frame buffer, pinned slots, copy streams, one CUDA
+    graph per frame size and network.precision_key), and the graph continues after postprocess with ops.affine_motion
+    (iterations, sigma): only the fit of each pair, 6 doubles and an ok byte, comes back to the host.  There
+    camera.stabilize_path turns the fits into one warp per frame (smoothing window `radius`, zoom `crop`; a pair whose fit
+    failed counts as no motion) once the fits of the frame's window are in.  The frames wait for their warp on the device,
+    in a ring of radius + depth * batch + 1 frames filled from the frame buffer on the compute stream; once per collected
+    batch, ops.warp_frames_affine warps the frames that became ready, on a stream of its own.  Each frame crosses PCIe once
+    in each direction, and host memory is bounded by the radius and the batch, not the video's length.  The results
+    equal network.stabilize_video's bit for bit.  frames: host uint8 (H,W,3) arrays or tensors, any channel order."""
+
+    def __init__(self, net: nn.Module, batch: int = 8, resize=None, radius: int = 15, crop: float = 0.9,
+                 iterations: int = ops.AFFINE_ITERATIONS, sigma: float = ops.AFFINE_SIGMA,
+                 depth: int = 2):
+        super().__init__(net, batch=batch, resize=resize, depth=depth)
+        camera.check_path_args(radius, crop, "VideoStabilizer")
+        if not (isinstance(iterations, int) and not isinstance(iterations, bool) and iterations >= 1):
+            raise MaskflowError(f"VideoStabilizer: iterations must be an integer >= 1, got {iterations!r}")
+        try:
+            good = 0.0 < float(sigma) < float("inf")
+        except (TypeError, ValueError):
+            good = False
+        if not good:
+            raise MaskflowError(f"VideoStabilizer: sigma must be positive and finite, got {sigma!r}")
+        self.radius, self.crop, self.iterations, self.sigma = int(radius), float(crop), int(iterations), float(sigma)
+        self.ring_size = self.radius + self.depth * self.batch + 1
+        self._rings = {}
+        self._v = None          # the state of the video being run
+
+    def invalidate(self) -> None:
+        super().invalidate()
+        self._rings.clear()
+
+    def _chain(self, F: torch.Tensor, H: int, W: int):
+        B = self.batch
+        x = F.permute(0, 3, 1, 2).contiguous()
+        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
+        flow = ops.postprocess(self.net(a, b)[0][-1], H, W, flip_channels=True, is_flow=True)
+        affine, ok = ops.affine_motion(flow, self.iterations, self.sigma)
+        return {"affine": affine, "ok": ok}
+
+    def _outputs(self):
+        return ("affine", "ok")
+
+    def _ring(self, H: int, W: int, dev: torch.device):
+        """The device ring of frames waiting for their warp, its output buffers and the warp stream."""
+        e = self._rings.get((H, W))
+        if e is None:
+            n = self.ring_size
+            e = self._rings[(H, W)] = {
+                "frames": torch.empty((n, H, W, 3), dtype=torch.uint8, device=dev),
+                "out": torch.empty((n, H, W, 3), dtype=torch.uint8, device=dev),
+                "out_host": torch.empty((n, H, W, 3), dtype=torch.uint8, pin_memory=True),
+                "stream": torch.cuda.Stream(device=dev), "ev_ring": torch.cuda.Event(), "ev_warp": torch.cuda.Event(),
+                "ev_host": torch.cuda.Event(), "warped": False}
+        return e
+
+    def _loaded(self, st, first: bool) -> None:
+        """Copies the batch's new frames from the frame buffer into the ring, after the warps that read their slots."""
+        F = st["F"]
+        v = self._v
+        r = v["ring"]
+        cur = torch.cuda.current_stream(F.device)
+        if r["warped"]:
+            cur.wait_event(r["ev_warp"])
+        src = F if first else F[1:]
+        t0, n = v["loaded"], self.ring_size
+        for a, b in self._segments(t0, t0 + len(src)):
+            r["frames"][a % n:a % n + (b - a)].copy_(src[a - t0:b - t0])
+        v["loaded"] += len(src)
+        r["ev_ring"].record(cur)
+
+    def _segments(self, t0: int, t1: int):
+        """Frames [t0, t1) as runs that are contiguous in the ring."""
+        n, out = self.ring_size, []
+        while t0 < t1:
+            b = min(t1, t0 + n - t0 % n)
+            out.append((t0, b))
+            t0 = b
+        return out
+
+    def _warp_ready(self, n_frames=None) -> list:
+        """Warps the frames whose smoothing window is known and returns them on the host: all the rest when n_frames (the
+        video's length) is given, else those t with t + radius <= the last frame whose path is known."""
+        v = self._v
+        known = len(v["P"]) + v["P0"] - 1          # P_0 .. P_known are known
+        t0 = v["next"]
+        t1 = n_frames if n_frames is not None else known - self.radius + 1
+        if t1 <= t0:
+            return []
+        n = known + 1 if n_frames is None else n_frames
+        M = np.stack([camera.stabilize_path(v["P"], t, n, v["H"], v["W"], self.radius, self.crop, v["P0"])
+                      for t in range(t0, t1)])
+        r = v["ring"]
+        ws = r["stream"]
+        with torch.cuda.stream(ws):
+            ws.wait_event(r["ev_ring"])
+            Md = torch.from_numpy(M).to(v["dev"])
+            for a, b in self._segments(t0, t1):
+                i = a % self.ring_size
+                r["out"][a - t0:b - t0].copy_(ops.warp_frames_affine(r["frames"][i:i + (b - a)], Md[a - t0:b - t0]))
+            r["ev_warp"].record(ws)
+            r["warped"] = True
+            r["out_host"][:t1 - t0].copy_(r["out"][:t1 - t0], non_blocking=True)
+            r["ev_host"].record(ws)
+        r["ev_host"].synchronize()
+        v["next"] = t1
+        drop = min(max(0, t1 - self.radius - v["P0"]), len(v["P"]) - 1)   # P_s, s < next - radius, is no longer needed
+        del v["P"][:drop]
+        v["P0"] += drop
+        return [r["out_host"][j].numpy().copy() for j in range(t1 - t0)]
+
+    def _collect(self, s, b: int) -> Iterator:
+        s["ev_out_free"].synchronize()
+        v = self._v
+        aff, ok = s["affine_host"], s["ok_host"]
+        for j in range(b):
+            v["P"].append(camera.path_step(v["P"][-1], aff[j].numpy(), bool(ok[j])))
+        with torch.cuda.device(v["dev"]):
+            ready = self._warp_ready()
+        yield from ready
+
+    @torch.no_grad()
+    def run(self, frames: Iterable) -> Iterator[np.ndarray]:
+        it = iter(frames)
+        head = [fr for fr in (next(it, None), next(it, None)) if fr is not None]
+        if not head:
+            return
+        fr0 = self._frame(head[0], None)
+        H, W = int(fr0.shape[0]), int(fr0.shape[1])
+        dev = next(self.net.parameters()).device
+        with torch.cuda.device(dev):
+            self._v = {"H": H, "W": W, "dev": dev, "ring": self._ring(H, W, dev), "loaded": 0, "next": 0,
+                       "P": [np.eye(3)], "P0": 0}
+        if len(head) == 1:                   # one frame: no pair; its window is itself, so its warp is the zoom
+            with torch.cuda.device(dev):
+                M = camera.stabilize_path([np.eye(3)], 0, 1, H, W, self.radius, self.crop)
+                out = ops.warp_frames_affine(fr0.to(dev).unsqueeze(0).contiguous(), torch.from_numpy(M[None]).to(dev))
+                res = out[0].cpu().numpy()
+            yield res
+            return
+        yield from super().run(itertools.chain(head, it))
+        with torch.cuda.device(dev):
+            ready = self._warp_ready(len(self._v["P"]) + self._v["P0"])
+        yield from ready
