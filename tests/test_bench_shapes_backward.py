@@ -335,7 +335,9 @@ def image_warp_flow_slopes(img, h, v, dh, dv, g, scale, got):
     and 1 - (1 - l) are off by up to 2u absolutely (2u sum |corners|); and the slope along y is linear in the column
     fraction with slope Delta (continuous across columns), so a column off by dv moves it by |Delta| dv (the larger
     |Delta| of the cells the column may lie in), and the same with the axes swapped.  The slope along y jumps where
-    h crosses an integer: where floor(h - dh) != floor(h + dh) the element is accepted against either row cell."""
+    h crosses an integer: where floor(h - dh) != floor(h + dh) the element is accepted against either row cell.
+    scale: the factor of both axes, or a (y, x) pair of factors (the stand-alone sampler's grid gradient)."""
+    sc = tuple(scale) if isinstance(scale, (tuple, list)) else (scale, scale)
     Ci = img.shape[1]
     L = Ci + 6
     g, ga = g.double(), g.double().abs()
@@ -345,8 +347,8 @@ def image_warp_flow_slopes(img, h, v, dh, dv, g, scale, got):
     cells = {(i, j): sampler_cell_slopes(img, h, v, ys[i], xs[j]) for i in (0, 1) for j in (0, 1)}
     dmax = torch.stack([c[4] for c in cells.values()]).amax(0)
     cmax = torch.stack([c[5] for c in cells.values()]).amax(0)
-    pos_y = abs(scale) * (ga * (dmax * dv.unsqueeze(1) + 2 * U * cmax)).sum(1)
-    pos_x = abs(scale) * (ga * (dmax * dh.unsqueeze(1) + 2 * U * cmax)).sum(1)
+    pos_y = abs(sc[0]) * (ga * (dmax * dv.unsqueeze(1) + 2 * U * cmax)).sum(1)
+    pos_x = abs(sc[1]) * (ga * (dmax * dh.unsqueeze(1) + 2 * U * cmax)).sum(1)
 
     # the slope along y in either row cell, each in the column cell of v itself (extrapolating a neighbouring column
     # cell's interpolant across the integer would not be the float64 value); along x the same with the axes swapped
@@ -356,8 +358,8 @@ def image_warp_flow_slopes(img, h, v, dh, dv, g, scale, got):
                            (1, pos_x, [sampler_cell_slopes(img, h, v, y0, xx) for xx in xs])):
         best = None
         for c in cand:
-            ref = scale * (g * c[k]).sum(1)
-            S = abs(scale) * (ga * c[2 + k]).sum(1)
+            ref = sc[k] * (g * c[k]).sum(1)
+            S = abs(sc[k]) * (ga * c[2 + k]).sum(1)
             rk = _ratio((got[:, k].double() - ref).abs(), gamma(L) * S + pos_k)
             best = rk if best is None else torch.minimum(best, rk)
             refs.append((ref, gamma(L) * S + pos_k))
@@ -371,8 +373,8 @@ def image_warp_flow_slopes(img, h, v, dh, dv, g, scale, got):
              ", ".join(f"{pick(a):.9g} (bound {pick(b):.3g})" for a, b in refs[2 * k:2 * k + 2]))
     nominal = sampler_cell_slopes(img, h, v, y0, x0)
     shifted = sampler_cell_slopes(img, h, v, y0 - 1, x0 + 1)
-    ctl = max(float(_ratio(scale * ((g * shifted[k]).sum(1) - (g * nominal[k]).sum(1)).abs(),
-                           gamma(L) * abs(scale) * (ga * nominal[2 + k]).sum(1) + pos_k).max())
+    ctl = max(float(_ratio(sc[k] * ((g * shifted[k]).sum(1) - (g * nominal[k]).sum(1)).abs(),
+                           gamma(L) * abs(sc[k]) * (ga * nominal[2 + k]).sum(1) + pos_k).max())
               for k, pos_k in ((0, pos_y), (1, pos_x)))
     return float(rr.max()), ctl, worst
 

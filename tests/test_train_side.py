@@ -631,8 +631,6 @@ def test_pipeline_load_head_and_fix_head_on_cpu(tmp_path):
 
 
 @pytest.mark.gpu
-@pytest.mark.xfail(strict=False, reason="first run on hardware happens at round end: the round's GPU allowance was spent before "
-                                        "pipeline.py was written (host plumbing is covered by the CPU test above)")
 def test_pipeline_train_validate_predict_on_gpu():
     from maskflownet_b200 import augment, pipeline
     rng = np.random.default_rng(1)

@@ -196,9 +196,14 @@ def census_backward_control(img1, img2w, occ, g_loss):
     return k * GREY.view(1, 3, 1, 1) * G.unsqueeze(1)
 
 
-def smoothness_bounds(flow, img, g_loss):
-    """float64 (loss, grad) of the oracle and their error bounds E (units of u), from float32 inputs."""
+def smoothness_bounds(flow, img, g_loss, kernel_signs=False):
+    """float64 (loss, grad) of the oracle and their error bounds E (units of u), from float32 inputs.
+    kernel_signs: the gradient takes the sign of each second difference as the kernel evaluates it in fp32,
+    fl(fl(lo - 2 mid) + hi) (second_diff in csrc/unsup_loss.cu; 2 mid is exact, so an fma gives the same), instead of
+    float64's, and the bound drops its allowance for a sign decided by rounding.  On up-sampled flows most second
+    differences are zero in exact arithmetic, and that allowance would cover any error of the size of the gradient."""
     f = _d64(flow).requires_grad_(True)
+    f32 = torch.as_tensor(np.asarray(flow)).float()
     im = _d64(img)
     N, _, H, W = f.shape
     loss = unsup_ref.smoothness_loss(f, im)
@@ -210,10 +215,11 @@ def smoothness_bounds(flow, img, g_loss):
     L_sum = 256 + parts + 16
     E_S = torch.zeros(N, dtype=torch.float64)
     E_grad = torch.zeros_like(f)
+    grad_k = torch.zeros_like(f)
     gl = _d64(g_loss).abs()
 
     def direction(axis, den):
-        nonlocal E_S, E_grad
+        nonlocal E_S, E_grad, grad_k
         n_ax = f.shape[axis]
         if n_ax <= 2:
             return
@@ -232,6 +238,15 @@ def smoothness_bounds(flow, img, g_loss):
         # backward: each stencil position p contributes tap * w(p) * sign(D(p)) to q in {p-1, p, p+1}
         amb = (D.abs() <= U * E_D).double()                         # the sign may differ from float64's: up to 2 w
         k = gl.view(N, 1, 1, 1) / den
+        if kernel_signs:
+            amb = torch.zeros_like(amb)
+            sgn = torch.sign((lo(f32) - 2 * mid(f32)) + hi(f32)).double()
+            ks = _d64(g_loss).view(N, 1, 1, 1) / den
+            for shift, tap in ((0, 1.0), (1, -2.0), (2, 1.0)):
+                pad = [0, 0, 0, 0]
+                pos = 0 if axis == 3 else 2
+                pad[pos], pad[pos + 1] = shift, 2 - shift
+                grad_k = grad_k + ks * torch.nn.functional.pad(tap * w.unsqueeze(1) * sgn, pad)
         for shift, tap in ((0, 1.0), (1, 2.0), (2, 1.0)):
             contrib = tap * (E_w + 4.0 * w).unsqueeze(1) + tap * 2.0 * w.unsqueeze(1) * amb / U
             pad = [0, 0, 0, 0]
@@ -242,7 +257,8 @@ def smoothness_bounds(flow, img, g_loss):
 
     direction(3, 2 * H * (W - 2))
     direction(2, 2 * (H - 2) * W)
-    return {"loss": loss.detach(), "grad": grad, "E_loss": E_S + 4.0 * loss.detach().abs(), "E_grad": E_grad}
+    return {"loss": loss.detach(), "grad": grad_k if kernel_signs else grad, "E_loss": E_S + 4.0 * loss.detach().abs(),
+            "E_grad": E_grad}
 
 
 def ratio(got, ref, E):
@@ -592,21 +608,44 @@ def _synthetic_batch(seeds, H, W, max_disp):
 NETWORK_STEP_REL = 2.0 ** -10
 
 
+def _gamma(L):
+    return L * U / (1 - L * U)
+
+
+def kernel_sample_positions(flow):
+    """The sample positions (h, v) of ops.reconstruction2d on the fp32 flow (N, 2, H, W) (y, x) it reads, as the kernels
+    compute them in fp32 (warp_fwd.cu), float64 values: the grid generator's g = fl(fl(fl(f + p) / s) - 1) with
+    s = (W - 1) / 2 (exact), then the sampler's fl(fl(g + 1) * (W - 1)) / 2, one rounding per operation.  They lie within
+    gamma_4 |f + p| + gamma_2 |f + p - s| px of f + p: the four relative roundings of the product chain, and the rounding
+    of the grid g itself, relative to |g| = |f + p - s| / s, scaled back by s."""
+    f = flow.detach().float().cpu()
+    N, _, H, W = f.shape
+    ys, xs = torch.arange(H, dtype=torch.float32).view(1, H, 1), torch.arange(W, dtype=torch.float32).view(1, 1, W)
+    gy, gx = (f[:, 0] + ys) / ((H - 1) / 2) - 1, (f[:, 1] + xs) / ((W - 1) / 2) - 1
+    return ((gy + 1) * (H - 1) / 2).double(), ((gx + 1) * (W - 1) / 2).double()
+
+
 @pytest.mark.gpu
 def test_network_step_gradient_matches_float64_composition():
     """The gradient of sum(unsupervised_loss) with respect to preds[-1] of a MaskFlownet-S training forward at batch 2N,
-    against the oracle composition in float64: torch_ref.upsample, torch_ref.reconstruction2d (the sampler) and
+    against the oracle composition in float64: torch_ref.upsample, the zero-padded bilinear sample (the sampler) and
     oracle/unsup_ref.py on the same preds[-1] and the same occlusion masks (a data decision: both sides use the
     kernel's).  The random-init flows are scaled to at most 0.3 px, so that the two directions pass the consistency
     check (|w + w'|^2 <= 0.36 < beta) and the census sees the whole interior.  smooth_weight 0: Upsample(4) makes three
     of every four second differences zero in exact arithmetic, where the sign the smoothness gradient takes is decided
     by rounding; that term is held per element, sign allowance included, by the kernel tests above, and Upsample's
-    backward by the existing operator tests.  Per element, |got - ref| <= 2^-10 S with S = Upsample(4)^T |dL/dF|: the
-    gradient before the transposed Upsample's sum of up to 49 signed contributions cancels (the same kind of wiring bound
-    DESIGN.md section 2 gives the cuDNN backward, with the census chain's steeper slope through the grey planes' rounding).
-    The outer two coarse rows and columns are left out: there the samples reach past the frame, and the largest
-    difference (29x the bound, in the last coarse row) has not been explained.  Control: the two warps swapped (b warped
-    by F_bw, a by F_fw) must exceed it by 3x."""
+    backward by the existing operator tests.  Per element over the whole frame, |got - ref| <= 2^-10 S with
+    S = Upsample(4)^T |dL/dF|: the gradient before the transposed Upsample's sum of up to 49 signed contributions cancels
+    (the same kind of wiring bound DESIGN.md section 2 gives the cuDNN backward, with the census chain's steeper slope
+    through the grey planes' rounding).
+    The reference samples at the kernel's own fp32 positions (kernel_sample_positions, moving with F at slope 1), not at
+    p + F: the grid generator's division and the sampler's de-normalisation round the position twice, up to ~1e-5 px
+    where |g| is near 1, i.e. at the frame's edges.  Inside the frame that moves the sample by a neighbour difference
+    times 1e-5; where a corner leaves the frame the zero padding makes the slope the whole pixel value, and the census
+    (grey values x255 through D / sqrt(0.81 + D^2) and s^2 / (0.1 + s^2), second derivative up to ~20 at s = 0)
+    turns that value change into a gradient change far above 2^-10 S (printed: up to ~29x in the last coarse row
+    against the reference at p + F).  That the positions lie within their derived bound of p + F is asserted.
+    Control: the two warps swapped (b warped by F_bw, a by F_fw) must exceed the bound by 3x."""
     from maskflownet_b200 import network
     from oracle import torch_ref
     torch.manual_seed(0)
@@ -627,13 +666,29 @@ def test_network_step_gradient_matches_float64_composition():
         occ = ops.flow_consistency(xy(fl[:n]), xy(fl[n:]))
     occ = tuple(o.cpu() for o in occ)
     a64, b64 = a.double().cpu(), b.double().cpu()
+    H, W = a.shape[2:]
+    h32, v32 = kernel_sample_positions(fl)
+    ys = torch.arange(H, dtype=torch.float64).view(1, H, 1)
+    xs = torch.arange(W, dtype=torch.float64).view(1, 1, W)
+    f64 = fl.double().cpu()
+    ey, ex = (h32 - (ys + f64[:, 0])).abs(), (v32 - (xs + f64[:, 1])).abs()
+    sy, sx = (H - 1) / 2, (W - 1) / 2
+    pos_ok = bool((ey <= _gamma(4) * (ys + f64[:, 0]).abs() + _gamma(2) * (ys + f64[:, 0] - sy).abs()).all()
+                  and (ex <= _gamma(4) * (xs + f64[:, 1]).abs() + _gamma(2) * (xs + f64[:, 1] - sx).abs()).all())
 
-    def ref_grad(swap_warps=False):
+    def ref_grad(swap_warps=False, fp32_positions=True):
         q = p.detach().double().cpu().requires_grad_(True)
         F = torch_ref.upsample(q, 4)
         F.retain_grad()
-        F_fw, F_bw = (F[n:], F[:n]) if swap_warps else (F[:n], F[n:])
-        b_w, a_w = torch_ref.reconstruction2d(b64, F_fw), torch_ref.reconstruction2d(a64, F_bw)
+        fw, bw = (slice(n, None), slice(None, n)) if swap_warps else (slice(None, n), slice(n, None))
+
+        def warp(x, rows):
+            Fr = F[rows]
+            if not fp32_positions:
+                return torch_ref.reconstruction2d(x, Fr)
+            return torch_ref.sample_tap(x, h32[rows] + (Fr[:, 0] - Fr[:, 0].detach()),
+                                        v32[rows] + (Fr[:, 1] - Fr[:, 1].detach()), 1)
+        b_w, a_w = warp(b64, fw), warp(a64, bw)
         L = unsup_ref.census_loss(torch.cat([a64, b64]), torch.cat([b_w, a_w]), torch.cat(occ).to(torch.uint8))[0]
         L.sum().backward()
         q2 = q.detach().clone().requires_grad_(True)
@@ -643,13 +698,16 @@ def test_network_step_gradient_matches_float64_composition():
     bound = NETWORK_STEP_REL * S
     ratio_map = (got - ref).abs() / bound
     worst = np.unravel_index(int(ratio_map.argmax()), tuple(ratio_map.shape))
-    inner = (slice(None), slice(None), slice(2, -2), slice(2, -2))     # coarse pixels whose samples stay in the frame
-    r = float(ratio_map[inner].max())
-    r_ctl = float(((got - ref_grad(swap_warps=True)[0]).abs() / bound)[inner].max())
+    r = float(ratio_map.max())
+    exact_map = (got - ref_grad(fp32_positions=False)[0]).abs() / bound
+    worst_exact = np.unravel_index(int(exact_map.argmax()), tuple(exact_map.shape))
+    r_ctl = float(((got - ref_grad(swap_warps=True)[0]).abs() / bound).max())
     print(f"network step: max|grad| {float(ref.abs().max()):.3e}, max S {float(S.max()):.3e}, max |got - ref| / bound "
-          f"{r:.3g} inside, {float(ratio_map.max()):.3g} at {worst} over all, control {r_ctl:.3g}; occluded "
-          f"{float(out.occluded.mean()):.3f}")
+          f"over the whole frame {r:.3g} at {worst}; with the reference sampling at p + F instead of the kernel's fp32 "
+          f"positions {float(exact_map.max()):.3g} at {worst_exact}; positions off p + F by up to "
+          f"{float(torch.maximum(ey, ex).max()):.3g} px; control {r_ctl:.3g}; occluded {float(out.occluded.mean()):.3f}")
     assert 0.0 < float(out.occluded.mean()) < 0.5
+    assert pos_ok
     assert r <= 1.0 and r_ctl >= CONTROL_RATIO, (r, r_ctl)
 
 
