@@ -540,7 +540,9 @@ def test_c_argument_errors_need_no_gpu():
         assert seed(ptrs) == -1 and b"null pointer" in L.mfn_last_error(), k
     ptrs = [p] * 9
     ptrs[2] = None
-    assert seed(ptrs, M=0) == 0 or b"null" not in L.mfn_last_error()   # no queries: no query pointer needed
+    # no queries: no query pointer needed.  The short workspace, the last check before the launch, keeps the kernel from
+    # running on these host buffers where a GPU is present
+    assert seed(ptrs, M=0, nb=15) == -1 and b"workspace" in L.mfn_last_error()
     assert seed(out=(p, None)) == -1 and b"together" in L.mfn_last_error()
     assert seed(K=0, M=0) == -1 and b"extent" in L.mfn_last_error()
     assert seed(h=0) == -1 and b"spacing" in L.mfn_last_error()
