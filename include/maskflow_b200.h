@@ -499,6 +499,44 @@ MFN_API int mfn_warp_frames_affine(const unsigned char* src, const double* M, un
                                    void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Moving-object segmentation: the pixels that move relative to the camera, labelled into 8-connected objects.
+ * Output frame n has two optional sides, each sample n of which lies on frame n:
+ *   side a (the forward direction, frame n -> n+1): res_a (N,H,W) float32, mfn_affine_motion's residual of the forward
+ *     flow; occ_a (N,H,W) uint8, its mfn_flow_consistency mask (nonzero = occluded); flow_a (N,H,W,2) float32 (x,y)
+ *     pixels, the forward flow; affine_a (N,2,3) float64, the forward flow's fit A.  All four null, or none.
+ *   side b (the backward direction, frame n -> n-1): res_b (N,H,W) float32 and occ_b (N,H,W) uint8, the same for the
+ *     backward flow.  Both null, or neither.  Both sides null gives empty frames.
+ * Rule, per frame and pixel p:
+ *   a = res_a(p), defined when finite and occ_a(p) = 0; b likewise from side b.  s = min(a, b) when both are defined, the
+ *   defined one when one is, undefined otherwise.  L = {p : s(p) >= tau_lo} in float32.  The components are the
+ *   8-connected components of L; one is kept when some pixel of it has s >= tau_hi and its area is >= min_area.  Kept
+ *   components are numbered 1, 2, ... in raster order of their first pixel (smallest y W + x), up to max_objects.
+ *   labels (N,H,W) uint8: the component's number, 0 for the background, for components not kept and for kept ones past
+ *   max_objects; count (N) int32 = min(kept, max_objects), dropped (N) int32 = max(0, kept - max_objects).
+ *   objects (N,max_objects,10) float64, row j < count for label j + 1 (rows past count are 0):
+ *     area, x0, y0, x1, y1 (inclusive box), cx, cy (the sums of x and of y, exact 64-bit integers, over the area),
+ *     peak (the largest s), dx, dy: the mean over the object's pixels where a is defined of
+ *     d = (p + flow_a(p)) - A p, each component evaluated in float64 as (x + u) - ((A00 x + A01 y) + A02) with every
+ *     operation rounded on its own and clamped to [-2^16, 2^16]; NaN where a is defined nowhere in the object (always on
+ *     a side-a-less frame).  The sums of d are 64-bit fixed point at scale 2^S, S = 46 - k, k the bit length of H W:
+ *     |dx - mean(d)| <= 2^-(S+1) + 2^-50 (1 + |mean(d)|).
+ * The union-find links the larger root under the smaller (parent[i] <= i), so a component's root is its first pixel
+ * whatever order the unions run in; every sum is an integer atomic, the score and peak are exact float32: the result is
+ * bit-reproducible.  11 launches whatever the content, no allocation, no host synchronisation: capture-safe.
+ * ws: caller-owned, mfn_motion_segment_workspace_bytes(N,H,W) bytes, 16-byte aligned: 4 H W bytes of parents per frame,
+ * 12 bytes per possible component (at most ceil(H/2) ceil(W/2) per frame) and 16 KiB per frame for the objects.
+ * A null pointer (or an incomplete side), an extent below 1, a non-finite tau or tau_lo > tau_hi, min_area below 1,
+ * max_objects outside [1,255], a misaligned pointer or a short workspace returns MFN_ERR_INVALID_ARG; H*W >= 2^31 or
+ * N > 65535 returns MFN_ERR_ALIGNMENT.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API long long mfn_motion_segment_workspace_bytes(int N, int H, int W);
+MFN_API int mfn_motion_segment(const float* res_a, const unsigned char* occ_a, const float* res_b,
+                               const unsigned char* occ_b, const float* flow_a, const double* affine_a,
+                               unsigned char* labels, double* objects, int* count, int* dropped, void* ws,
+                               long long ws_bytes, int N, int H, int W, float tau_lo, float tau_hi, int min_area,
+                               int max_objects, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Deterministic mode: bit-reproducible variants of the entry points whose default kernels accumulate with fp32 atomics
  * (the scatter of a bilinear sample's gradient to its four corners, per-CTA weight partials, per-slice plane sums).  Same
  * arguments and results as the counterpart named without _det, plus a caller-owned workspace `det_ws` of `det_ws_bytes`

@@ -49,6 +49,8 @@ SIGNATURES = {
     "mfn_affine_motion_workspace_bytes": [_i, _i, _i],
     "mfn_affine_motion": [_f] * 5 + [_ll, _i, _i, _i, _i, _fl, _f],
     "mfn_warp_frames_affine": [_f, _f, _f, _i, _i, _i, _f],
+    "mfn_motion_segment_workspace_bytes": [_i, _i, _i],
+    "mfn_motion_segment": [_f] * 11 + [_ll, _i, _i, _i, _fl, _fl, _i, _i, _f],
     "mfn_warp_mask_backward_det": [_f] * 14 + [_i] * 5 + [_fl, _fl, _fl, _i, _f, _ll, _f],
     "mfn_deformable_conv_backward_det": [_f] * 8 + [_i] * 6 + [_f, _ll, _f],
     "mfn_bilinear_sampler_backward_det": [_f] * 5 + [_i] * 6 + [_f, _ll, _f],
@@ -73,7 +75,7 @@ SIGNATURES = {
 }
 # entries of SIGNATURES that do not return an int status
 RESTYPES = {"mfn_interpolate_frames_workspace_bytes": _ll, "mfn_track_seed_workspace_bytes": _ll,
-            "mfn_affine_motion_workspace_bytes": _ll}
+            "mfn_affine_motion_workspace_bytes": _ll, "mfn_motion_segment_workspace_bytes": _ll}
 
 
 class MaskflowError(RuntimeError):

@@ -651,6 +651,57 @@ def stabilize_video(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=N
     return out, affine, ok, M
 
 
+@torch.no_grad()
+def segment_motion(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=None, tau_lo: float = ops.SEG_TAU_LO,
+                   tau_hi: float = ops.SEG_TAU_HI, min_area: int = ops.SEG_MIN_AREA,
+                   max_objects: int = ops.SEG_MAX_OBJECTS, alpha: float = 0.01, beta: float = 0.5):
+    """The objects moving relative to the camera in every frame of a clip of uint8 frames (T,H,W,3) on the device, any
+    channel order (ops.segment_motion states the rule).  The pairs go through predict_bidirectional `batch` at a time (the
+    last batch padded with the last frame, as video.VideoMotionSegmenter does); each batch's 2B flows through one
+    ops.affine_motion(want_residual=True) at its defaults, and one ops.segment_motion segments the batch's first frames:
+    frame k0 + j takes side a from pair j and side b from pair j - 1, or for j = 0 from the previous batch's last pair
+    (for frame 0: none, given as NaN residuals, which are undefined).  The last frame is segmented from side b alone.  A
+    one-frame clip gives one empty frame.  This is the eager chain VideoMotionSegmenter captures.
+    Returns (labels (T,H,W) uint8, objects (T,max_objects,10) float64, count (T,) int32, dropped (T,) int32) on the
+    device."""
+    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
+        raise ops.MaskflowError("segment_motion: clip must be a (T,H,W,3) uint8 tensor")
+    if batch < 1:
+        raise ops.MaskflowError(f"segment_motion: batch must be >= 1, got {batch}")
+    ops.check_segment_args(tau_lo, tau_hi, min_area, max_objects, "segment_motion")
+    T, H, W, _ = clip.shape
+    dev = clip.device
+    kw = dict(tau_lo=tau_lo, tau_hi=tau_hi, min_area=min_area, max_objects=max_objects)
+    labels = torch.empty((T, H, W), dtype=torch.uint8, device=dev)
+    objects = torch.empty((T, max_objects, 10), dtype=torch.float64, device=dev)
+    count = torch.empty((T,), dtype=torch.int32, device=dev)
+    dropped = torch.empty((T,), dtype=torch.int32, device=dev)
+    P = T - 1
+    if P == 0:
+        with torch.cuda.device(dev):
+            labels[:], objects[:], count[:], dropped[:] = ops.segment_motion(shape=(1, H, W), **kw)
+        return labels, objects, count, dropped
+    carry_res = torch.full((1, H, W), float("nan"), dtype=torch.float32, device=dev)
+    carry_occ = torch.zeros((1, H, W), dtype=torch.uint8, device=dev)
+    B = batch
+    for k0 in range(0, P, B):
+        x = clip[[min(k0 + j, P) for j in range(B + 1)]].permute(0, 3, 1, 2).contiguous()
+        flow_fw, flow_bw, occ_fw, occ_bw = predict_bidirectional(net, x[:B], x[1:], resize, alpha, beta)
+        affine, _, res = ops.affine_motion(torch.cat([flow_fw, flow_bw]), want_residual=True)
+        res_b = torch.cat([carry_res, res[B:2 * B - 1]])
+        occ_b = torch.cat([carry_occ, occ_bw[:B - 1]])
+        out = ops.segment_motion(res[:B], occ_fw, res_b, occ_b, flow_fw, affine[:B], **kw)
+        nb = min(B, P - k0)
+        for dst, src in zip((labels, objects, count, dropped), out):
+            dst[k0:k0 + nb] = src[:nb]
+        carry_res, carry_occ = res[2 * B - 1:], occ_bw[B - 1:]
+        if k0 + nb == P:           # the last frame: side b of the last real pair
+            last = ops.segment_motion(res_b=res[B + nb - 1:B + nb], occ_b=occ_bw[nb - 1:nb], **kw)
+            for dst, src in zip((labels, objects, count, dropped), last):
+                dst[P:] = src
+    return labels, objects, count, dropped
+
+
 def precision_key(net: nn.Module) -> Tuple[str, ...]:
     """The inference_precision of every flow network inside `net` (the cascade's head may be set on its own): what a
     captured graph depends on besides the input shape."""

@@ -952,6 +952,94 @@ def warp_frames_affine(frames: torch.Tensor, M: torch.Tensor) -> torch.Tensor:
 
 
 # ----------------------------------------------------------------------------------------------------------
+# Moving-object segmentation (csrc/motionseg.cu)
+# ----------------------------------------------------------------------------------------------------------
+# Defaults, from the synthetic scene of tests/test_motion_segment.py (README, "Moving-object segmentation").
+SEG_TAU_LO, SEG_TAU_HI, SEG_MIN_AREA, SEG_MAX_OBJECTS = 1.0, 2.0, 64, 255
+
+
+def check_segment_args(tau_lo, tau_hi, min_area, max_objects, who: str) -> None:
+    try:
+        lo, hi = float(tau_lo), float(tau_hi)
+    except (TypeError, ValueError):
+        raise MaskflowError(f"{who}: tau_lo and tau_hi must be numbers, got {tau_lo!r}, {tau_hi!r}") from None
+    inf = float("inf")
+    lo, hi = (torch.tensor(v, dtype=torch.float32).item() for v in (lo, hi))     # the kernel compares in float32
+    if not (-inf < lo <= hi < inf):
+        raise MaskflowError(f"{who}: tau_lo and tau_hi must be finite with tau_lo <= tau_hi, got {tau_lo}, {tau_hi}")
+    if not (isinstance(min_area, int) and not isinstance(min_area, bool) and min_area >= 1):
+        raise MaskflowError(f"{who}: min_area must be an integer >= 1, got {min_area!r}")
+    if not (isinstance(max_objects, int) and not isinstance(max_objects, bool) and 1 <= max_objects <= 255):
+        raise MaskflowError(f"{who}: max_objects must be an integer in [1,255], got {max_objects!r}")
+
+
+def segment_motion(res_a=None, occ_a=None, res_b=None, occ_b=None, flow_a=None, affine_a=None, tau_lo: float = SEG_TAU_LO,
+                   tau_hi: float = SEG_TAU_HI, min_area: int = SEG_MIN_AREA, max_objects: int = SEG_MAX_OBJECTS,
+                   shape=None):
+    """The objects that move relative to the camera in each of N frames (include/maskflow_b200.h,
+    mfn_motion_segment).  Frame n takes up to two sides: side a, the forward direction of the pair (n, n+1) --
+    res_a (N,H,W) float32, affine_motion's residual of the forward flow; occ_a (N,H,W) uint8, its flow_consistency mask;
+    flow_a (N,H,W,2) float32, the forward flow; affine_a (N,2,3) float64, its fit -- and side b, the backward direction of
+    the pair (n-1, n): res_b, occ_b.  A side is given whole or not at all; with neither, `shape` = (N,H,W) gives empty
+    frames.  Per pixel s = the smaller of the defined residuals (finite and not occluded); the 8-connected components of
+    s >= tau_lo that reach s >= tau_hi somewhere and cover at least min_area pixels are the objects, numbered 1, 2, ...
+    in raster order of their first pixel, up to max_objects (at most 255).
+    Returns (labels (N,H,W) uint8, 0 = background; objects (N,max_objects,10) float64, rows (area, x0, y0, x1, y1, cx,
+    cy, peak, dx, dy) for the first count[n] labels, 0 past them -- dx, dy the mean camera-relative displacement
+    p + flow_a(p) - A p where side a is defined, NaN where it is nowhere; count (N,) int32; dropped (N,) int32, the objects
+    past max_objects).  Bit-reproducible and capture-safe.  Forward only."""
+    who = "segment_motion"
+    check_segment_args(tau_lo, tau_hi, min_area, max_objects, who)
+    side_a, side_b = (res_a, occ_a, flow_a, affine_a), (res_b, occ_b)
+    have_a, have_b = any(t is not None for t in side_a), any(t is not None for t in side_b)
+    if have_a and any(t is None for t in side_a):
+        raise MaskflowError(f"{who}: res_a, occ_a, flow_a and affine_a go together")
+    if have_b and any(t is None for t in side_b):
+        raise MaskflowError(f"{who}: res_b and occ_b go together")
+    args = []
+    if have_a:
+        args += [(res_a, "res_a", torch.float32, None), (occ_a, "occ_a", torch.uint8, None),
+                 (flow_a, "flow_a", torch.float32, 2)]
+    if have_b:
+        args += [(res_b, "res_b", torch.float32, None), (occ_b, "occ_b", torch.uint8, None)]
+    lead = dev = None
+    for t, nm, dtype, last in args:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise MaskflowError(f"{who}: {nm} must be a CUDA tensor; the hot path has no CPU implementation")
+        if t.dtype != dtype or not t.is_contiguous():
+            raise MaskflowError(f"{who}: {nm} must be a contiguous {dtype} tensor")
+        if t.dim() != (3 if last is None else 4) or (last is not None and t.shape[-1] != last):
+            raise MaskflowError(f"{who}: expected {nm} of shape (N,H,W{'' if last is None else ',2'}), got {tuple(t.shape)}")
+        ld = tuple(t.shape[:3])
+        if lead is None:
+            lead, dev = ld, t.device
+        elif ld != lead or t.device != dev:
+            raise MaskflowError(f"{who}: {nm} {tuple(t.shape)} on {t.device} does not match {lead} on {dev}")
+    if have_a:
+        if not isinstance(affine_a, torch.Tensor) or affine_a.device != dev or affine_a.dtype != torch.float64 or \
+                not affine_a.is_contiguous() or tuple(affine_a.shape) != (lead[0], 2, 3):
+            raise MaskflowError(f"{who}: affine_a must be a contiguous float64 tensor of shape ({lead[0]},2,3) on {dev}")
+        _no_grad_path(who, res_a, flow_a)
+    if have_b:
+        _no_grad_path(who, res_b)
+    if lead is None:
+        if shape is None or len(shape) != 3 or min(int(v) for v in shape) < 1:
+            raise MaskflowError(f"{who}: without either side, shape must be (N,H,W), got {shape!r}")
+        lead, dev = tuple(int(v) for v in shape), torch.device("cuda", torch.cuda.current_device())
+    N, H, W = lead
+    labels = torch.empty((N, H, W), device=dev, dtype=torch.uint8)
+    objects = torch.empty((N, max_objects, 10), device=dev, dtype=torch.float64)
+    count = torch.empty((N,), device=dev, dtype=torch.int32)
+    dropped = torch.empty((N,), device=dev, dtype=torch.int32)
+    nb = int(_lib.lib().mfn_motion_segment_workspace_bytes(N, H, W))
+    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    _call("mfn_motion_segment", dev, _p(res_a), _p(occ_a), _p(res_b), _p(occ_b), _p(flow_a), _p(affine_a), _p(labels),
+          _p(objects), _p(count), _p(dropped), _p(ws), nb, N, H, W, float(tau_lo), float(tau_hi), int(min_area),
+          int(max_objects))
+    return labels, objects, count, dropped
+
+
+# ----------------------------------------------------------------------------------------------------------
 # Dense point tracking (csrc/track.cu)
 # ----------------------------------------------------------------------------------------------------------
 TRACK_EMPTY, TRACK_TRACKED, TRACK_BORN, TRACK_LEFT, TRACK_OCCLUDED, TRACK_BOUNDARY = range(6)

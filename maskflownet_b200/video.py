@@ -23,6 +23,10 @@ video frame:
 VideoStabilizer extends the one-direction chain with the camera's motion per pair (ops.affine_motion); the camera path is
 smoothed on the host (camera.stabilize_path) and the frames, kept on the device in a ring, are warped outside the graph:
     preprocess(F[:B], F[1:])  ->  network  ->  postprocess  ->  affine_motion
+VideoMotionSegmenter extends the bidirectional chain with the camera-relative motion of both directions and the objects
+it forms (ops.segment_motion), carrying the last backward residual of each batch into the next on the device:
+    preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  flow_consistency
+    ->  affine_motion (2B flows, residuals)  ->  segment_motion (B frames)
 Copies follow network.PipelinedFlowPredictor's slot scheme: pinned host staging, H2D on one copy stream, D2H of the colours
 (and flows) on another, `depth` slots, so the copies of neighbouring batches run under the replay of this one.
 """
@@ -576,3 +580,106 @@ class VideoStabilizer(VideoFlowPredictor):
         with torch.cuda.device(dev):
             ready = self._warp_ready(len(self._v["P"]) + self._v["P0"])
         yield from ready
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Moving-object segmentation
+# ---------------------------------------------------------------------------------------------------------------------
+class MotionFrame(NamedTuple):
+    """The moving objects of one video frame.  labels (H,W) uint8: object k + 1 at the pixels of row k, 0 elsewhere;
+    objects (count,10) float64 rows (area, x0, y0, x1, y1, cx, cy, peak, dx, dy) (ops.segment_motion); dropped: the
+    objects found past max_objects, left unlabelled."""
+    labels: np.ndarray
+    objects: np.ndarray
+    dropped: int
+
+
+class VideoMotionSegmenter(VideoFlowPredictor):
+    """The objects moving relative to the camera, streamed: run(frames) yields one MotionFrame per video frame, frame 0
+    included, in order.
+
+    The pairs go through VideoFlowPredictor's bidirectional machinery (frame buffer, pinned slots, copy streams, one CUDA
+    graph per frame size and network.precision_key), and the graph continues after the occlusion masks with one
+    ops.affine_motion(want_residual=True) over the batch's 2B flows and one ops.segment_motion over the batch's first B
+    frames.  Frame t0 + j takes side a from pair j and side b from pair j - 1, or for j = 0 from a device copy of the
+    previous batch's last backward residual and mask (NaN residuals at the start of a video: undefined).  The last
+    frame is segmented from side b alone after the final batch.  Only the labels and the object rows cross PCIe; the
+    padded tail of a partial batch is discarded.  The results equal network.segment_motion's bit for bit.  frames: host
+    uint8 (H,W,3) arrays or tensors, any channel order."""
+
+    def __init__(self, net: nn.Module, batch: int = 8, resize=None, tau_lo: float = ops.SEG_TAU_LO,
+                 tau_hi: float = ops.SEG_TAU_HI, min_area: int = ops.SEG_MIN_AREA,
+                 max_objects: int = ops.SEG_MAX_OBJECTS, alpha: float = 0.01, beta: float = 0.5, depth: int = 2):
+        super().__init__(net, batch=batch, resize=resize, depth=depth, bidirectional=True, alpha=alpha, beta=beta)
+        ops.check_segment_args(tau_lo, tau_hi, min_area, max_objects, "VideoMotionSegmenter")
+        self.seg_args = dict(tau_lo=float(tau_lo), tau_hi=float(tau_hi), min_area=int(min_area),
+                             max_objects=int(max_objects))
+        self._carries = {}
+        self._run = None          # (graph state, pairs of the last collected batch) of the video being run
+
+    def invalidate(self) -> None:
+        super().invalidate()
+        self._carries.clear()
+
+    def _carry(self, H: int, W: int, dev: torch.device):
+        """The previous batch's last backward residual and mask, on the device."""
+        c = self._carries.get((H, W))
+        if c is None:
+            c = self._carries[(H, W)] = {"res": torch.empty((1, H, W), dtype=torch.float32, device=dev),
+                                         "occ": torch.empty((1, H, W), dtype=torch.uint8, device=dev)}
+        return c
+
+    def _chain(self, F: torch.Tensor, H: int, W: int):
+        B = self.batch
+        c = self._carry(H, W, F.device)
+        x = F.permute(0, 3, 1, 2).contiguous()
+        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
+        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
+        occ_fw, occ_bw = ops.flow_consistency(flows[:B], flows[B:], self.alpha, self.beta)
+        affine, _, res = ops.affine_motion(flows, want_residual=True)
+        res_b = torch.cat([c["res"], res[B:2 * B - 1]])
+        occ_b = torch.cat([c["occ"], occ_bw[:B - 1]])
+        labels, objects, count, dropped = ops.segment_motion(res[:B], occ_fw, res_b, occ_b, flows[:B], affine[:B],
+                                                             **self.seg_args)
+        c["res"].copy_(res[2 * B - 1:])
+        c["occ"].copy_(occ_bw[B - 1:])
+        return {"labels": labels, "objects": objects, "count": count, "dropped": dropped, "res_bw": res[B:],
+                "occ_bw": occ_bw}
+
+    def _outputs(self):
+        return ("labels", "objects", "count", "dropped")
+
+    def _start(self, st) -> None:
+        F = st["F"]
+        c = self._carry(F.shape[1], F.shape[2], F.device)
+        c["res"].fill_(float("nan"))
+        c["occ"].zero_()
+        self._run = (st, 0)
+
+    def _collect(self, s, b: int) -> Iterator:
+        self._run = (self._run[0], b)
+        for labels, objects, count, dropped in super()._collect(s, b):
+            yield MotionFrame(labels, objects[:int(count)], int(dropped))
+
+    def _segment_last(self, res_b, occ_b, shape) -> MotionFrame:
+        labels, objects, count, dropped = ops.segment_motion(res_b=res_b, occ_b=occ_b, shape=shape, **self.seg_args)
+        n = int(count[0])
+        return MotionFrame(labels[0].cpu().numpy(), objects[0, :n].cpu().numpy(), int(dropped[0]))
+
+    @torch.no_grad()
+    def run(self, frames: Iterable) -> Iterator[MotionFrame]:
+        it = iter(frames)
+        head = [fr for fr in (next(it, None), next(it, None)) if fr is not None]
+        if not head:
+            return
+        dev = next(self.net.parameters()).device
+        if len(head) == 1:                   # one frame: no pair, an empty frame
+            fr = self._frame(head[0], None)
+            with torch.cuda.device(dev):
+                yield self._segment_last(None, None, (1, int(fr.shape[0]), int(fr.shape[1])))
+            return
+        yield from super().run(itertools.chain(head, it))
+        st, b = self._run                    # the graph's outputs still hold the last batch
+        self._run = None
+        with torch.cuda.device(dev):
+            yield self._segment_last(st["out"]["res_bw"][b - 1:b], st["out"]["occ_bw"][b - 1:b], None)
