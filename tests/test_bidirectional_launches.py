@@ -34,8 +34,9 @@ strictly inside (0, 1) and both decisions are reached.  hd8 runs once more in bf
 (test_bf16_mode.py), and VideoFlowPredictor(bidirectional=True) must replay its eager chain bit for bit at batch 8 on a
 9-frame 1080p clip.
 
-Not checked here: frames larger than 1088x1920; the interpolation, tracking and stabilisation kernels (their own files
-check them at 1080p).
+Not checked here: frames larger than 1088x1920; the kernels of the video tools that follow this forward (interpolation,
+tracking, stabilisation and motion segmentation): test_video_chain_launches.py checks every one of their launches in
+the tools' chains against float64 at batch 8 on 1080p, and which pair each frame reads.
 """
 import time
 

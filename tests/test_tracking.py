@@ -155,6 +155,14 @@ def _compare_advance(prev_pos, prev_status, adv_pos, adv_status, ffw, fbw, tally
     return int(bad.sum())
 
 
+def _compare_seed(adv_pos, adv_status, lam, lmax, q, k, h, tau, H, W, xy, st, dropped, control=None):
+    """Mismatching slots and dropped counts of the seeding of frame k against the oracle from the state after the advance
+    (exact: no exclusion)."""
+    rp, rs, rd = R.seed(adv_pos, adv_status, lam, lmax, q, k, h, tau, H, W, control)
+    same = (rs == st) & ((rp == xy) | (np.isnan(rp) & np.isnan(xy))).all(-1)
+    return int((~same).sum()) + int(rd != dropped)
+
+
 def _run_chain(tr, frames, ffw, fbw, tally=None, control=None):
     """Runs a tracker over the frames; checks every advance (with exclusions) and every seeding (exact) against the
     oracle from the tracker's previous state.  Returns (xy (T,K,2), status (T,K), dropped (T,), mismatches)."""
@@ -174,10 +182,8 @@ def _run_chain(tr, frames, ffw, fbw, tally=None, control=None):
         assert np.array_equal(lam_np, R.texture(frames[k], tr.h)), k
         assert lmax_np[0] == R.texture(frames[k], tr.h).max(initial=0.0), k
         xy[k], st[k], dropped[k] = tr.seed(lam, lmax)
-        rp, rs, rd = R.seed(adv_pos, adv_status, lam_np, lmax_np, tr.q, k, tr.h, tr.tau, tr.H, tr.W,
-                            control if control not in R.ADVANCE_CONTROLS else None)
-        same = (rs == st[k]) & ((rp == xy[k]) | (np.isnan(rp) & np.isnan(xy[k]))).all(-1)
-        bad += int((~same).sum()) + int(rd != dropped[k])
+        bad += _compare_seed(adv_pos, adv_status, lam_np, lmax_np, tr.q, k, tr.h, tr.tau, tr.H, tr.W, xy[k], st[k],
+                             dropped[k], control if control not in R.ADVANCE_CONTROLS else None)
     return xy, st, dropped, bad
 
 
