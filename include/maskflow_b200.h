@@ -537,6 +537,53 @@ MFN_API int mfn_motion_segment(const float* res_a, const unsigned char* occ_a, c
                                int max_objects, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Video denoising: each frame averaged with its neighbours aligned along chained bidirectional flow, every neighbour
+ * weighted by a patch distance so that a wrong flow does not ghost (flow-guided temporal non-local means).
+ *
+ * mfn_denoise_frames: frames (S,H,W,3) uint8 (any channel order), a ring: frame t sits in slot t mod S.  flow_fw,
+ *   flow_bw (S,H,W,2) float32 (x,y) pixels (the layout mfn_postprocess_forward writes), rings, 8-byte aligned: slot
+ *   t mod S holds pair (t, t+1), flow_fw of t -> t+1 and flow_bw of t+1 -> t.  out (N,H,W,3) uint8: frames t0 .. t0+N-1.
+ *   The video's frames are [t_lo, t_hi]; every window is clamped to them.  A plain clip is S = T, t_lo = 0, t_hi = T-1
+ *   (its last flow slot is never read).
+ *   Trajectory of pixel p of frame t, in float32, q_0 = p:
+ *     forward, k = 1 .. min(R, t_hi - t): w = flow_fw[t+k-1] sampled bilinearly at q_{k-1} (corners x0 = floor(qx),
+ *       x1 = min(x0+1, W-1), the same in y, weights q - floor(q): mfn_flow_consistency's rule); q = q_{k-1} + w.  The
+ *       chain stops if q is non-finite or outside [0,W-1] x [0,H-1], or unless |w+b|^2 <= alpha (|w|^2 + |b|^2) + beta
+ *       with that right-hand side finite, b = flow_bw[t+k-1] sampled at q (mfn_track_advance, steps 1-3).  Otherwise
+ *       q_k = q and a_k(p) = frame t+k sampled bilinearly at q_k per channel with the same corner rule,
+ *       fl((1-wy) fl((1-wx) A + wx B) + wy fl((1-wx) C + wx D)) in float32 (flowcheck.cuh's fb_lerp).
+ *     backward, k = 1 .. min(R, t - t_lo): the same with flow_bw[t-k] as the step, flow_fw[t-k] as the check and frame
+ *       t-k as the colour.
+ *     Once a chain stops, a_k is undefined for that k and every later k of its direction.
+ *   Weight of neighbour k at p (float32): 0 where a_k(p) is undefined; otherwise over the offsets o in [-r,r]^2 (oy
+ *     outer, ox inner, ascending) for which p+o lies in the frame and a_k(p+o) is defined, n of them,
+ *     D = the sum over o and the channels c = 0,1,2 of (a_k,c(p+o) - I_t,c(p+o))^2 in that order, d2 = D / (3n), and
+ *     w_k = expf(-fmaxf(d2 - 2 sigma^2, 0) / (h_factor sigma)^2), with 2 sigma^2 = 2 (sigma sigma) and
+ *     (h_factor sigma)^2 = hs hs, hs = h_factor sigma, each rounded to float32.
+ *   Output, per channel: out = rint((I_t(p) + sum_k w_k a_k(p)) / (1 + sum_k w_k)) (ties to even), clamped to [0,255];
+ *     the sums run over the forward neighbours k = 1..R, then the backward ones k = 1..R, in float32.  R = 0, or no
+ *     defined neighbour, returns the input.
+ *   radius R >= 0, patch r in [0, 8] (r above 8 returns MFN_ERR_UNSUPPORTED), sigma > 0 in grey levels, h_factor > 0;
+ *   alpha = 0.01, beta = 0.5 are mfn_flow_consistency's constants.  The ring must hold every frame the windows read:
+ *   t_lo <= t0, t0+N-1 <= t_hi and min(t_hi, t0+N-1+R) - max(t_lo, t0-R) + 1 <= S.
+ *   One launch of 16 x 16-pixel tiles per frame, (16+2r)^2 x 32 bytes of shared memory per CTA.  No atomics (the result
+ *   does not depend on the thread schedule or on the other frames of the call), no allocation, no host synchronisation;
+ *   the launch configuration depends on the extents only: capture-safe.
+ * mfn_noise_sigma: frames (F,H,W,3) uint8 -> sigma (F) float64, 8-byte aligned: Immerkaer's estimator (CVIU 1996),
+ *   S = the sum over the three channels and the interior pixels (1 <= x <= W-2, 1 <= y <= H-2) of
+ *   |I * [[1,-2,1],[-2,4,-2],[1,-2,1]]|, exact in int64; sigma = max(0.5, sqrt(pi/2) S / (18 (W-2) (H-2))), evaluated
+ *   in float64 as (1.2533141373155003 S) / ((18 (W-2)) (H-2)).  The floor of 0.5 grey levels keeps sigma > 0 on clean
+ *   or flat frames.  Bit-reproducible; one CTA per frame.  H or W below 3 returns MFN_ERR_INVALID_ARG.
+ * A null pointer, an extent below 1, R or r below 0, a non-positive or non-finite sigma or h_factor, a negative or
+ * non-finite alpha or beta, a window outside [t_lo, t_hi] or not held by the ring, or a misaligned flow returns
+ * MFN_ERR_INVALID_ARG; H*W >= 2^31 or N (F) > 65535 returns MFN_ERR_ALIGNMENT.
+ * ------------------------------------------------------------------------------------------------- */
+MFN_API int mfn_denoise_frames(const unsigned char* frames, const float* flow_fw, const float* flow_bw,
+                               unsigned char* out, int S, int H, int W, int t0, int N, int t_lo, int t_hi, int radius,
+                               int patch, float sigma, float h_factor, float alpha, float beta, void* stream);
+MFN_API int mfn_noise_sigma(const unsigned char* frames, double* sigma, int F, int H, int W, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Deterministic mode: bit-reproducible variants of the entry points whose default kernels accumulate with fp32 atomics
  * (the scatter of a bilinear sample's gradient to its four corners, per-CTA weight partials, per-slice plane sums).  Same
  * arguments and results as the counterpart named without _det, plus a caller-owned workspace `det_ws` of `det_ws_bytes`

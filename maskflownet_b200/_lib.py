@@ -51,6 +51,8 @@ SIGNATURES = {
     "mfn_warp_frames_affine": [_f, _f, _f, _i, _i, _i, _f],
     "mfn_motion_segment_workspace_bytes": [_i, _i, _i],
     "mfn_motion_segment": [_f] * 11 + [_ll, _i, _i, _i, _fl, _fl, _i, _i, _f],
+    "mfn_denoise_frames": [_f] * 4 + [_i] * 9 + [_fl] * 4 + [_f],
+    "mfn_noise_sigma": [_f, _f, _i, _i, _i, _f],
     "mfn_warp_mask_backward_det": [_f] * 14 + [_i] * 5 + [_fl, _fl, _fl, _i, _f, _ll, _f],
     "mfn_deformable_conv_backward_det": [_f] * 8 + [_i] * 6 + [_f, _ll, _f],
     "mfn_bilinear_sampler_backward_det": [_f] * 5 + [_i] * 6 + [_f, _ll, _f],

@@ -702,6 +702,39 @@ def segment_motion(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=No
     return labels, objects, count, dropped
 
 
+@torch.no_grad()
+def denoise_video(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=None, radius: int = ops.DENOISE_RADIUS,
+                  sigma=None, h: float = ops.DENOISE_H, patch: int = ops.DENOISE_PATCH, alpha: float = 0.01,
+                  beta: float = 0.5):
+    """A denoised clip of uint8 frames (T,H,W,3) on the device, any channel order (ops.denoise_frames states the rule).
+    The pairs go through predict_bidirectional `batch` at a time (the last batch padded with the last frame, as
+    video.VideoDenoiser does), then one ops.denoise_frames over the whole clip averages each frame with up to `radius`
+    neighbours on each side along the chained flow.  sigma=None takes ops.median_noise of the clip's first
+    min(T, batch + 1) frames, the frames the stream sees first.  A one-frame clip comes back unchanged.  This is the
+    eager chain VideoDenoiser streams.  Returns (denoised clip (T,H,W,3) uint8 on the device, the sigma used)."""
+    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
+        raise ops.MaskflowError("denoise_video: clip must be a (T,H,W,3) uint8 tensor")
+    if batch < 1:
+        raise ops.MaskflowError(f"denoise_video: batch must be >= 1, got {batch}")
+    ops.check_denoise_args(radius, sigma, h, patch, alpha, beta, "denoise_video", sigma_optional=True)
+    T, H, W, _ = clip.shape
+    clip = clip.contiguous()
+    if sigma is None:
+        sigma = ops.median_noise(clip[:min(T, batch + 1)])
+    if T == 1:
+        return clip.clone(), float(sigma)
+    P = T - 1
+    fw = torch.zeros((T, H, W, 2), dtype=torch.float32, device=clip.device)   # slot T-1 (no pair) is never read
+    bw = torch.zeros_like(fw)
+    for k0 in range(0, P, batch):
+        x = clip[[min(k0 + j, P) for j in range(batch + 1)]].permute(0, 3, 1, 2).contiguous()
+        flow_fw, flow_bw, _, _ = predict_bidirectional(net, x[:batch], x[1:], resize, alpha, beta)
+        nb = min(batch, P - k0)
+        fw[k0:k0 + nb], bw[k0:k0 + nb] = flow_fw[:nb], flow_bw[:nb]
+    out = ops.denoise_frames(clip, fw, bw, radius, sigma, h, patch, alpha, beta)
+    return out, float(sigma)
+
+
 def precision_key(net: nn.Module) -> Tuple[str, ...]:
     """The inference_precision of every flow network inside `net` (the cascade's head may be set on its own): what a
     captured graph depends on besides the input shape."""

@@ -1040,6 +1040,112 @@ def segment_motion(res_a=None, occ_a=None, res_b=None, occ_b=None, flow_a=None, 
 
 
 # ----------------------------------------------------------------------------------------------------------
+# Video denoising (csrc/denoise.cu)
+# ----------------------------------------------------------------------------------------------------------
+# Defaults, from the sweep over the synthetic scene of tests/test_denoise.py through the oracle (README, "Video
+# denoising"): R neighbours on each side, a (2 DENOISE_PATCH + 1)^2 patch, h = DENOISE_H sigma.
+DENOISE_RADIUS, DENOISE_PATCH, DENOISE_H = 2, 1, 0.7
+DENOISE_MAX_PATCH = 8       # the kernel's shared-memory bound on the patch radius
+NOISE_FLOOR = 0.5           # estimate_noise never returns less (grey levels)
+
+
+def _positive_finite(v) -> bool:
+    try:
+        return 0.0 < float(v) < float("inf")
+    except (TypeError, ValueError):
+        return False
+
+
+def _int_at_least(v, lo) -> bool:
+    return isinstance(v, int) and not isinstance(v, bool) and v >= lo
+
+
+def check_denoise_args(radius, sigma, h, patch, alpha, beta, who: str, sigma_optional: bool = False) -> None:
+    if not _int_at_least(radius, 0):
+        raise MaskflowError(f"{who}: radius must be an integer >= 0, got {radius!r}")
+    if not (_int_at_least(patch, 0) and patch <= DENOISE_MAX_PATCH):
+        raise MaskflowError(f"{who}: patch must be an integer in [0,{DENOISE_MAX_PATCH}], got {patch!r}")
+    if not (sigma is None and sigma_optional) and not _positive_finite(sigma):
+        raise MaskflowError(f"{who}: sigma must be positive and finite, got {sigma!r}")
+    if not _positive_finite(h):
+        raise MaskflowError(f"{who}: h must be positive and finite, got {h!r}")
+    if not (_finite_nonneg(alpha) and _finite_nonneg(beta)):
+        raise MaskflowError(f"{who}: alpha and beta must be finite and non-negative, got {alpha!r}, {beta!r}")
+
+
+def denoise_frames(frames: torch.Tensor, flow_fw: torch.Tensor, flow_bw: torch.Tensor, radius: int, sigma: float,
+                   h: float = DENOISE_H, patch: int = DENOISE_PATCH, alpha: float = 0.01, beta: float = 0.5,
+                   t0: int = 0, n: Optional[int] = None, t_lo: int = 0, t_hi: Optional[int] = None,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Frames t0 .. t0+n-1 of a video, each averaged with up to `radius` neighbours on each side aligned along the
+    chained flow and weighted by a patch distance (include/maskflow_b200.h, mfn_denoise_frames).
+    frames (S,H,W,3) uint8, any channel order, a ring: frame t in slot t % S.  flow_fw, flow_bw (S,H,W,2) float32 (x,y)
+    pixels, rings: slot t % S holds pair (t, t+1), flow_fw t -> t+1 and flow_bw t+1 -> t (the layout
+    network.predict_bidirectional returns).  The video's frames are [t_lo, t_hi] (default t_lo + S - 1): a plain clip of
+    T frames is S = T with the defaults.  A chain stops where its target leaves the frame or the forward-backward check
+    (alpha, beta) fails.  Neighbour k of pixel p gets the weight exp(-max(d2 - 2 sigma^2, 0) / (h sigma)^2), d2 the mean
+    squared colour difference over the (2 patch + 1)^2 patch around p where the neighbour is defined; sigma is the noise
+    level in grey levels (estimate_noise).  n defaults to t_hi - t0 + 1.  Returns (n,H,W,3) uint8 (into `out` when
+    given).  Deterministic and capture-safe.  Forward only."""
+    who = "denoise_frames"
+    check_denoise_args(radius, sigma, h, patch, alpha, beta, who)
+    fr = _stab_tensor(frames, "frames", torch.uint8, 3, who)
+    fw = _stab_tensor(flow_fw, "flow_fw", torch.float32, 2, who)
+    bw = _stab_tensor(flow_bw, "flow_bw", torch.float32, 2, who)
+    S, H, W, _ = fr.shape
+    for t, nm in ((fw, "flow_fw"), (bw, "flow_bw")):
+        if tuple(t.shape[:3]) != (S, H, W) or t.device != fr.device:
+            raise MaskflowError(f"{who}: {nm} {tuple(t.shape)} on {t.device} does not match frames {tuple(fr.shape)} "
+                                f"on {fr.device}")
+    _no_grad_path(who, fw, bw)
+    for v, nm in ((t0, "t0"), (t_lo, "t_lo")):
+        if not _int_at_least(v, 0):
+            raise MaskflowError(f"{who}: {nm} must be an integer >= 0, got {v!r}")
+    t_hi = t_lo + S - 1 if t_hi is None else t_hi
+    n = t_hi - t0 + 1 if n is None else n
+    if not (_int_at_least(t_hi, 0) and _int_at_least(n, 1)):
+        raise MaskflowError(f"{who}: t_hi must be an integer >= 0 and n >= 1, got {t_hi!r}, {n!r}")
+    if not t_lo <= t0 <= t0 + n - 1 <= t_hi:
+        raise MaskflowError(f"{who}: frames {t0}..{t0 + n - 1} lie outside the video's frames {t_lo}..{t_hi}")
+    span = min(t_hi, t0 + n - 1 + radius) - max(t_lo, t0 - radius) + 1
+    if span > S:
+        raise MaskflowError(f"{who}: the windows span {span} frames, more than the ring's {S} slots")
+    if out is None:
+        out = torch.empty((n, H, W, 3), dtype=torch.uint8, device=fr.device)
+    elif not (isinstance(out, torch.Tensor) and out.dtype == torch.uint8 and out.is_contiguous() and
+              tuple(out.shape) == (n, H, W, 3) and out.device == fr.device):
+        raise MaskflowError(f"{who}: out must be a contiguous uint8 tensor of shape ({n},{H},{W},3) on {fr.device}")
+    _call("mfn_denoise_frames", fr.device, _p(fr), _p(fw), _p(bw), _p(out), S, H, W, int(t0), int(n), int(t_lo),
+          int(t_hi), int(radius), int(patch), float(sigma), float(h), float(alpha), float(beta))
+    return out
+
+
+def estimate_noise(frames: torch.Tensor) -> torch.Tensor:
+    """The noise level of each frame in grey levels, Immerkaer's estimator (include/maskflow_b200.h, mfn_noise_sigma):
+    sqrt(pi/2) / (18 (W-2) (H-2)) times the exact sum of |I * [[1,-2,1],[-2,4,-2],[1,-2,1]]| over the interior pixels and
+    the three channels, floored at NOISE_FLOOR so that it is always positive.  frames (F,H,W,3) or (H,W,3) uint8, H and
+    W at least 3.  Returns (F,) float64 on the device (a 0-d tensor for one (H,W,3) frame).  Bit-reproducible.  Sharp
+    edges count as noise: on clean, detailed footage the estimate is high."""
+    if not isinstance(frames, torch.Tensor) or frames.dim() not in (3, 4):
+        raise MaskflowError("estimate_noise: frames must be an (F,H,W,3) or (H,W,3) uint8 tensor")
+    fr = frames if frames.dim() == 4 else frames.unsqueeze(0)
+    fr = _stab_tensor(fr, "frames", torch.uint8, 3, "estimate_noise")
+    F, H, W, _ = fr.shape
+    if H < 3 or W < 3:
+        raise MaskflowError(f"estimate_noise: frames of {H}x{W} have no interior pixel (H and W must be >= 3)")
+    sigma = torch.empty((F,), dtype=torch.float64, device=fr.device)
+    _call("mfn_noise_sigma", fr.device, _p(fr), _p(sigma), F, H, W)
+    return sigma if frames.dim() == 4 else sigma[0]
+
+
+def median_noise(frames: torch.Tensor) -> float:
+    """The median of estimate_noise over the frames (the lower middle value for an even count), as a float: the sigma
+    the video denoisers use when none is given."""
+    s = estimate_noise(frames).sort().values
+    return float(s[(len(s) - 1) // 2])
+
+
+# ----------------------------------------------------------------------------------------------------------
 # Dense point tracking (csrc/track.cu)
 # ----------------------------------------------------------------------------------------------------------
 TRACK_EMPTY, TRACK_TRACKED, TRACK_BORN, TRACK_LEFT, TRACK_OCCLUDED, TRACK_BOUNDARY = range(6)

@@ -27,6 +27,9 @@ VideoMotionSegmenter extends the bidirectional chain with the camera-relative mo
 it forms (ops.segment_motion), carrying the last backward residual of each batch into the next on the device:
     preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)  ->  flow_consistency
     ->  affine_motion (2B flows, residuals)  ->  segment_motion (B frames)
+VideoDenoiser ends the bidirectional chain at the 2B flows; each batch's frames and flows are copied into a device ring,
+and the frames whose window of neighbours is complete are denoised outside the graph (ops.denoise_frames):
+    preprocess(F[:B], F[1:])  ->  bidirectional forward  ->  postprocess (2B flows)
 Copies follow network.PipelinedFlowPredictor's slot scheme: pinned host staging, H2D on one copy stream, D2H of the colours
 (and flows) on another, `depth` slots, so the copies of neighbouring batches run under the replay of this one.
 """
@@ -44,6 +47,21 @@ from . import camera, network, ops
 from ._lib import MaskflowError
 
 _WARMUP = 2
+
+
+class _FrameRing:
+    """The bookkeeping of a device ring of `ring_size` slots that holds frame t in slot t % ring_size (VideoStabilizer's
+    frames waiting for their warp, VideoDenoiser's frames and flows waiting for their window)."""
+    ring_size: int
+
+    def _segments(self, t0: int, t1: int):
+        """Frames [t0, t1) as runs that are contiguous in the ring."""
+        n, out = self.ring_size, []
+        while t0 < t1:
+            b = min(t1, t0 + n - t0 % n)
+            out.append((t0, b))
+            t0 = b
+        return out
 
 
 class VideoFlowPredictor:
@@ -184,6 +202,7 @@ class VideoFlowPredictor:
         self._loaded(st, first)
         s["ev_in_free"].record(cur)
         st["graph"].replay()
+        self._replayed(st)
         if s["used"]:
             cur.wait_event(s["ev_out_free"])
         for name in self._outputs():
@@ -203,6 +222,9 @@ class VideoFlowPredictor:
     def _loaded(self, st, first: bool) -> None:
         """Runs on the compute stream once per batch, after the batch's new frames are in the frame buffer (F[0..B] for
         the first batch of a video, F[1..B] afterwards) and before its replay."""
+
+    def _replayed(self, st) -> None:
+        """Runs on the compute stream once per batch, right after its replay, while the graph's outputs hold it."""
 
     def _collect(self, s, b: int) -> Iterator:
         s["ev_out_free"].synchronize()
@@ -432,7 +454,7 @@ class VideoTracker(VideoFlowPredictor):
 # ---------------------------------------------------------------------------------------------------------------------
 # Video stabilisation
 # ---------------------------------------------------------------------------------------------------------------------
-class VideoStabilizer(VideoFlowPredictor):
+class VideoStabilizer(_FrameRing, VideoFlowPredictor):
     """A stabilised video, streamed: run(frames) yields one stabilised (H,W,3) uint8 frame per input frame, frame 0
     included, in order, `radius` frames behind the input.
 
@@ -506,15 +528,6 @@ class VideoStabilizer(VideoFlowPredictor):
             r["frames"][a % n:a % n + (b - a)].copy_(src[a - t0:b - t0])
         v["loaded"] += len(src)
         r["ev_ring"].record(cur)
-
-    def _segments(self, t0: int, t1: int):
-        """Frames [t0, t1) as runs that are contiguous in the ring."""
-        n, out = self.ring_size, []
-        while t0 < t1:
-            b = min(t1, t0 + n - t0 % n)
-            out.append((t0, b))
-            t0 = b
-        return out
 
     def _warp_ready(self, n_frames=None) -> list:
         """Warps the frames whose smoothing window is known and returns them on the host: all the rest when n_frames (the
@@ -683,3 +696,150 @@ class VideoMotionSegmenter(VideoFlowPredictor):
         self._run = None
         with torch.cuda.device(dev):
             yield self._segment_last(st["out"]["res_bw"][b - 1:b], st["out"]["occ_bw"][b - 1:b], None)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Video denoising
+# ---------------------------------------------------------------------------------------------------------------------
+class VideoDenoiser(_FrameRing, VideoFlowPredictor):
+    """A denoised video, streamed: run(frames) yields one denoised (H,W,3) uint8 frame per input frame, frame 0 included,
+    in order, `radius` frames behind the input.
+
+    The pairs go through VideoFlowPredictor's bidirectional machinery (frame buffer, pinned slots, copy streams, one
+    CUDA graph per frame size and network.precision_key); the graph ends at the 2B flows, and nothing of it comes back to
+    the host.  On the compute stream each batch's new frames and both directions' flows are copied into a device ring of
+    2 radius + depth * batch + 1 slots.  Once per collected batch, on a stream of its own, one ops.denoise_frames call
+    denoises the frames whose window is complete (t + radius <= the last frame loaded); the last `radius` frames follow
+    after the final batch, their windows clamped to the video.  sigma=None takes ops.median_noise of the first
+    min(T, batch + 1) frames (the value used is left in `sigma_used`).  A one-frame video comes back unchanged.  Each
+    frame crosses PCIe once in each direction, and memory is bounded by the radius and the batch, not the video's length.
+    The results equal network.denoise_video's bit for bit.  frames: host uint8 (H,W,3) arrays or tensors, any channel
+    order."""
+
+    def __init__(self, net: nn.Module, batch: int = 8, resize=None, radius: int = ops.DENOISE_RADIUS, sigma=None,
+                 h: float = ops.DENOISE_H, patch: int = ops.DENOISE_PATCH, alpha: float = 0.01, beta: float = 0.5,
+                 depth: int = 2):
+        super().__init__(net, batch=batch, resize=resize, depth=depth, bidirectional=True, alpha=alpha, beta=beta)
+        ops.check_denoise_args(radius, sigma, h, patch, alpha, beta, "VideoDenoiser", sigma_optional=True)
+        self.radius, self.h, self.patch = int(radius), float(h), int(patch)
+        self.sigma = None if sigma is None else float(sigma)
+        self.sigma_used = None
+        self.ring_size = 2 * self.radius + self.depth * self.batch + 1
+        self._rings = {}
+        self._v = None          # the state of the video being run
+
+    def invalidate(self) -> None:
+        super().invalidate()
+        self._rings.clear()
+
+    def _chain(self, F: torch.Tensor, H: int, W: int):
+        B = self.batch
+        x = F.permute(0, 3, 1, 2).contiguous()
+        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
+        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
+        return {"flow": flows[:B], "flow_bw": flows[B:]}
+
+    def _outputs(self):
+        return ()
+
+    def _ring(self, H: int, W: int, dev: torch.device):
+        """The device rings of frames and flows, the output buffers and the denoising stream."""
+        e = self._rings.get((H, W))
+        if e is None:
+            n = self.ring_size
+            e = self._rings[(H, W)] = {
+                "frames": torch.empty((n, H, W, 3), dtype=torch.uint8, device=dev),
+                "fw": torch.empty((n, H, W, 2), dtype=torch.float32, device=dev),
+                "bw": torch.empty((n, H, W, 2), dtype=torch.float32, device=dev),
+                "out": torch.empty((n, H, W, 3), dtype=torch.uint8, device=dev),
+                "out_host": torch.empty((n, H, W, 3), dtype=torch.uint8, pin_memory=True),
+                "stream": torch.cuda.Stream(device=dev), "ev_done": torch.cuda.Event(), "ev_host": torch.cuda.Event(),
+                "used": False}
+        return e
+
+    def _loaded(self, st, first: bool) -> None:
+        """Copies the batch's new frames from the frame buffer into the ring, after the denoising that read their slots."""
+        F = st["F"]
+        v = self._v
+        r = v["ring"]
+        cur = torch.cuda.current_stream(F.device)
+        if r["used"]:
+            cur.wait_event(r["ev_done"])
+        src = F if first else F[1:]
+        t0 = v["loaded"]
+        n = self.ring_size
+        for a, b in self._segments(t0, t0 + len(src)):
+            r["frames"][a % n:a % n + (b - a)].copy_(src[a - t0:b - t0])
+        v["pair0"] = 0 if first else t0 - 1          # the batch's pairs are pair0 .. pair0 + B - 1
+        v["loaded"] += len(src)
+
+    def _replayed(self, st) -> None:
+        """Copies the batch's flows from the graph's outputs into the ring; the event marks the batch as loaded."""
+        v = self._v
+        r, out, p0, n = v["ring"], st["out"], v["pair0"], self.ring_size
+        for a, b in self._segments(p0, p0 + self.batch):
+            r["fw"][a % n:a % n + (b - a)].copy_(out["flow"][a - p0:b - p0])
+            r["bw"][a % n:a % n + (b - a)].copy_(out["flow_bw"][a - p0:b - p0])
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(st["F"].device))
+        v["marks"].append((p0, ev))
+
+    def _denoise_ready(self, ev, t_end: int, t_hi: int) -> list:
+        """Denoises frames next .. t_end of the video whose last frame so far is t_hi, and returns them on the host."""
+        v = self._v
+        t0 = v["next"]
+        n = t_end - t0 + 1
+        r = v["ring"]
+        ws = r["stream"]
+        if ev is not None:                   # also when nothing is ready: later calls rely on the stream's order
+            ws.wait_event(ev)
+        if n <= 0:
+            return []
+        with torch.cuda.stream(ws):
+            ops.denoise_frames(r["frames"], r["fw"], r["bw"], self.radius, v["sigma"], self.h, self.patch, self.alpha,
+                               self.beta, t0=t0, n=n, t_lo=0, t_hi=t_hi, out=r["out"][:n])
+            r["ev_done"].record(ws)
+            r["used"] = True
+            r["out_host"][:n].copy_(r["out"][:n], non_blocking=True)
+            r["ev_host"].record(ws)
+        r["ev_host"].synchronize()
+        v["next"] = t_end + 1
+        return [r["out_host"][j].numpy().copy() for j in range(n)]
+
+    def _collect(self, s, b: int) -> Iterator:
+        p0, ev = self._v["marks"].popleft()
+        last = p0 + b                                  # the batch's last real frame
+        with torch.cuda.device(self._v["dev"]):
+            ready = self._denoise_ready(ev, last - self.radius, last)
+        yield from ready
+
+    @torch.no_grad()
+    def run(self, frames: Iterable) -> Iterator[np.ndarray]:
+        it = iter(frames)
+        head = list(itertools.islice(it, self.batch + 1))
+        if not head:
+            return
+        fr0 = self._frame(head[0], None)
+        H, W = int(fr0.shape[0]), int(fr0.shape[1])
+        head = [fr0] + [self._frame(fr, (H, W)) for fr in head[1:]]
+        dev = next(self.net.parameters()).device
+        with torch.cuda.device(dev):
+            sigma = self.sigma if self.sigma is not None else ops.median_noise(torch.stack(head).to(dev))
+        self.sigma_used = sigma
+        if len(head) == 1:                   # one frame: no neighbours
+            yield head[0].numpy().copy()
+            return
+        count = [0]
+
+        def counted(src):
+            for fr in src:
+                count[0] += 1
+                yield fr
+
+        with torch.cuda.device(dev):
+            self._v = {"dev": dev, "ring": self._ring(H, W, dev), "loaded": 0, "next": 0, "pair0": 0,
+                       "marks": collections.deque(), "sigma": sigma}
+        yield from super().run(counted(itertools.chain(head, it)))
+        with torch.cuda.device(dev):
+            ready = self._denoise_ready(None, count[0] - 1, count[0] - 1)
+        yield from ready
