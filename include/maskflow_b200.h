@@ -54,8 +54,26 @@ MFN_API const char* mfn_last_error(void);
 MFN_API const char* mfn_last_kernel(void);
 /* Number of kernel launches issued by this library since load (process-wide, monotonically increasing). */
 MFN_API unsigned long long mfn_launch_count(void);
-/* Process-wide tuning / test knobs.  Keys: "corr_grid_cap" (>0 caps the persistent grid of the tensor-core correlation
- * kernels; tests use it to force long per-CTA tile runs), "corr_disable_ring" (1 = never pick the strip-marching kernel). */
+/* Process-wide tuning / test knobs.  The defaults are what the library runs; tests set the others to reach a fallback at
+ * small shapes, or to show that two paths give identical results.  This list is complete: any other key returns
+ * MFN_ERR_INVALID_ARG.
+ *   "corr_grid_cap"  default 0: > 0 caps the persistent grid of the tensor-core correlation kernels at that many CTAs
+ *                    (long per-CTA tile runs)
+ *   "corr_tma"       default 1: 0 = C <= 32 correlations skip the TMA pipeline kernel and take the strip-marching (ring)
+ *                    kernel, which otherwise serves only the shapes the TMA kernel declines
+ *   "corr_rb"        default 1: C > 32 correlations with N*H*W <= 1024 run on the row-block kernel; 2 = the row-block
+ *                    kernel for every shape it fits; 0 = never (the chunked tile kernel instead)
+ *   "warp_lin"       default 1: 0 = mfn_warp_mask_forward_resample takes the border-list path instead of the evaluation
+ *                    through linearity
+ *   "conv_wgmma"     default 1: 0 = the 3x3 convolutions the mma.sync kernel covers (stride 1, Cout <= 128, NCHW output)
+ *                    run on it instead of the wgmma kernel
+ *   "conv_grid_cap"  default 0: > 0 caps the persistent wgmma convolution's grid at that many CTAs (0 = one per SM)
+ *   "conv_splitk"    default 1: the plan splits the input channels of small layers (<= 8 parts); 0 = never split;
+ *                    k > 1 = at most k parts
+ *   "conv_narrow"    default 1: 0 = every wgmma convolution takes 128-pixel tile rows (no 64-pixel rows)
+ *   "conv_tma_in"    default 1: 0 = fp32 wgmma inputs are loaded per thread instead of staged by TMA
+ *   "conv_dbg"       default 0: profiling switches of the wgmma convolution (2 = producers skip global loads, 4 = no
+ *                    epilogue stores, 8 = no MMAs, 16 = no input path); any non-zero value makes results invalid */
 MFN_API int mfn_set_tuning(const char* key, int value);
 
 /* ---------------------------------------------------------------------------------------------------
@@ -245,8 +263,9 @@ MFN_API int mfn_image_warp_concat_backward(const float* grad_c40, const float* i
  * needs no concat copies.  fp32-accurate tensor-core arithmetic (bf16 hi/lo split, 3 MMAs per product, fp32 accumulate).
  * Weights are packed once per layer: mfn_conv3x3_packed_bytes() -> caller allocates -> mfn_conv3x3_pack_weights().
  * Cout <= 256.  leaky_slope = 1 disables the activation.
- * Two kernels serve it: warpgroup MMAs (csrc/conv3x3_wgmma.cu, default; tuning key "conv_wgmma") and
- * the mma.sync kernel (csrc/conv3x3.cu, stride 1, Cout <= 128); the packed buffer holds both weight images.
+ * Two kernels serve it: warpgroup MMAs (csrc/conv3x3_wgmma.cu, default) and the mma.sync kernel (csrc/conv3x3.cu,
+ * stride 1, Cout <= 128), which runs the shapes the wgmma kernel declines and everything it covers when tuning key
+ * "conv_wgmma" = 0; the packed buffer holds both weight images.
  * mfn_conv3x3_forward_ex adds
  *   - stride 2 (pad 1, dilation 1) = the feature pyramid's down-sampling convolutions conv{L}a / conv{L}x
  *     (network/MaskFlownet.py:147-165, 200-201: nn.Conv2D(3x3, strides=2, padding=1) + LeakyReLU); H, W are the INPUT
@@ -271,7 +290,7 @@ MFN_API int mfn_conv3x3_forward(const float* x, long long x_batch_stride, const 
  * weights are each rounded once to bf16 (nearest even: the "hi" of the split), each product is the one MMA hi*hi, exact
  * in fp32, and products accumulate in fp32; bias, activation, linear prefix, depth-to-space and split-K are unchanged.
  * Each product errs by up to about 2^-7 relative (two roundings to 8 significant bits) instead of about 2^-17.  Only the wgmma kernel has this variant: the bit
- * returns MFN_ERR_UNSUPPORTED where the mma.sync kernel would run (tuning "conv_wgmma" = 0, or W < "conv_wgmma_min_w").
+ * returns MFN_ERR_UNSUPPORTED where the mma.sync kernel would run (a shape the wgmma kernel declines, or tuning "conv_wgmma" = 0).
  * mfn_conv3x3_workspace_bytes does not depend on it. */
 #define MFN_CONV_BF16 0x10
 MFN_API int mfn_conv3x3_forward_ex(const float* x, long long x_batch_stride, const void* packed_weight, const float* bias,

@@ -123,7 +123,7 @@ def lib() -> ctypes.CDLL:
         # experiment hook: MFN_TUNING="key=value,key=value" applies mfn_set_tuning at load time
         for item in filter(None, os.environ.get("MFN_TUNING", "").split(",")):
             key, _, val = item.partition("=")
-            if key.strip() in ("corr_dbg", "conv_dbg"):
+            if key.strip() == "conv_dbg":
                 # the phase-ablation switches produce INVALID results: tools set them through set_tuning(), never the environment
                 raise MaskflowError(f"MFN_TUNING: {key.strip()} is a profiling switch (results invalid); set it from a tool, "
                                     "not the environment")

@@ -47,25 +47,15 @@ extern "C" unsigned long long mfn_launch_count(void) { return mfn::g_launches.lo
 extern "C" int mfn_set_tuning(const char* key, int value) {
   if (!key) return mfn::fail(MFN_ERR_INVALID_ARG, "mfn_set_tuning: null key");
   if (!strcmp(key, "corr_grid_cap")) mfn::tuning().corr_grid_cap = value;
-  else if (!strcmp(key, "corr_disable_ring")) mfn::tuning().corr_disable_ring = value;
-  else if (!strcmp(key, "warp_lin")) mfn::tuning().warp_lin = value;
+  else if (!strcmp(key, "corr_tma")) mfn::tuning().corr_tma = value;
   else if (!strcmp(key, "corr_rb")) mfn::tuning().corr_rb = value;
-  else if (!strcmp(key, "warp_lin_fch")) mfn::tuning().warp_lin_fch = value;
-  else if (!strcmp(key, "conv_as")) mfn::tuning().conv_as = value;
+  else if (!strcmp(key, "warp_lin")) mfn::tuning().warp_lin = value;
+  else if (!strcmp(key, "conv_wgmma")) mfn::tuning().conv_wgmma = value;
+  else if (!strcmp(key, "conv_grid_cap")) mfn::tuning().conv_grid_cap = value;
   else if (!strcmp(key, "conv_splitk")) mfn::tuning().conv_splitk = value;
   else if (!strcmp(key, "conv_narrow")) mfn::tuning().conv_narrow = value;
   else if (!strcmp(key, "conv_tma_in")) mfn::tuning().conv_tma_in = value;
-  else if (!strcmp(key, "corr_rb_twb")) mfn::tuning().corr_rb_twb = value;
-  else if (!strcmp(key, "corr_rb_rows")) mfn::tuning().corr_rb_rows = value;
-  else if (!strcmp(key, "corr_tma")) mfn::tuning().corr_tma = value;
-  else if (!strcmp(key, "corr_ts_lo")) mfn::tuning().corr_ts_lo = value;
-  else if (!strcmp(key, "corr_ts_hi")) mfn::tuning().corr_ts_hi = value;
-  else if (!strcmp(key, "corr_dbg")) mfn::tuning().corr_dbg = value;
   else if (!strcmp(key, "conv_dbg")) mfn::tuning().conv_dbg = value;
-  else if (!strcmp(key, "corr_ring_th")) mfn::tuning().corr_ring_th = value;
-  else if (!strcmp(key, "conv_wgmma")) mfn::tuning().conv_wgmma = value;
-  else if (!strcmp(key, "conv_grid_cap")) mfn::tuning().conv_grid_cap = value;
-  else if (!strcmp(key, "conv_wgmma_min_w")) mfn::tuning().conv_wgmma_min_w = value;
   else return mfn::fail(MFN_ERR_INVALID_ARG, "mfn_set_tuning: unknown key '%s'", key);
   return MFN_OK;
 }

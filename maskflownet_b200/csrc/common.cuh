@@ -14,28 +14,19 @@ int fail(int code, const char* fmt, ...);
 int check_launch(const char* kernel_name);  // cudaGetLastError -> return code, bumps launch counter
 void note_kernel(const char* name);
 
-// process-wide tuning / test knobs (mfn_set_tuning)
+// process-wide tuning / test knobs: the keys of mfn_set_tuning, with their defaults and effects, are listed in
+// include/maskflow_b200.h
 struct Tuning {
-  int corr_grid_cap = 0;      // > 0: cap the persistent grid of the MMA correlation kernels (tests force long tile runs)
-  int corr_disable_ring = 0;  // 1: use the tile kernel even for C <= 32
-  int conv_wgmma = 1;          // 1: 3x3 convolutions run on wgmma (conv3x3_wgmma.cu), 0: mma.sync kernel
-  int conv_grid_cap = 0;      // persistent wgmma convolution: CTAs (0 = one per SM); tests force long per-CTA tile runs
-  int conv_wgmma_min_w = 1;    // narrower images stay on the mma.sync kernel (a 128-pixel M tile would be mostly padding)
-  int corr_ring_th = 8;       // tile height of the strip-marching kernel: 4 (8 warps, 2 CTAs/SM) or 8 (16 warps, 1 CTA/SM)
-  int corr_rb = 1;            // 1: C > 32 correlations run on the row-block kernel (corr_rb.cu); 2: also C <= 32 when the TMA kernel declines; 0: chunked tile kernel
-  int warp_lin_fch = 0;       // > 0: channels per thread of warp_lin_kernel (a multiple of 8; default: 16 / 32 / 64 by level size)
-  int conv_as = 0;            // 2: wide wgmma layers keep 2 input stages (more weight stages); default 3
-  int conv_splitk = 1;        // 0: never split K; 1: plan decides (<= 8 parts); k > 1: cap on the number of parts
-  int conv_narrow = 1;        // 1: wgmma outputs at most 64 px wide run 64-px tile rows (one M block per row); 0: 128-px rows
-  int conv_tma_in = 1;        // 1: fp32 wgmma inputs that fit the tensor map are staged raw by TMA; 0: per-thread loads
-  int corr_rb_twb = 0;        // 2: force 16-pixel strips in the row-block kernel (two CTAs per SM when the tile fits 113 KB)
-  int corr_rb_rows = 0;       // > 0: start the row-block kernel's RB search at this value (4 / 2 / 1)
-  int corr_tma = 1;           // 1: C <= 32 correlations run on the TMA pipeline kernel (corr_tma.cu) when the shape fits
-  int warp_lin = 1;           // 1: mfn_warp_mask_forward_resample evaluates every pixel through linearity (warp_lin.cu); 0: border list
-  int corr_ts_lo = 0, corr_ts_hi = 0;   // development: device pointer (two halves) of the timeline buffer of corr_tma_kernel, 0 = off
-  int corr_dbg = 0;           // profiling aid for the ring kernel: 2 = producers idle, 4 = no epilogue, 8 = no MMA (results invalid)
-  int conv_dbg = 0;           // profiling aid for the wgmma convolution: 2 = producers skip global loads, 4 = no epilogue
-                              // stores, 8 = no MMAs, 16 = no input path at all (results invalid; tools/conv_bound.py)
+  int corr_grid_cap = 0;
+  int corr_tma = 1;
+  int corr_rb = 1;
+  int warp_lin = 1;
+  int conv_wgmma = 1;
+  int conv_grid_cap = 0;
+  int conv_splitk = 1;
+  int conv_narrow = 1;
+  int conv_tma_in = 1;
+  int conv_dbg = 0;
 };
 Tuning& tuning();
 

@@ -331,7 +331,7 @@ extern "C" long long mfn_conv3x3_workspace_bytes(int N, int Cin, int H, int W, i
   if (N <= 0 || Cin <= 0 || H <= 0 || W <= 0 || Cout <= 0 || Cout > 256 || dilation < 1 ||
       !(stride == 1 || (stride == 2 && dilation == 1)))
     return 0;
-  if (!(tuning().conv_wgmma && W >= tuning().conv_wgmma_min_w) && Cout <= 128 && stride == 1) return 0;   // mma.sync kernel
+  if (!tuning().conv_wgmma && Cout <= 128 && stride == 1) return 0;   // mma.sync kernel
   return conv3x3_wgmma_workspace_bytes(N, Cin, H, W, Cout, stride, dilation);
 }
 
@@ -365,7 +365,7 @@ extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, 
   const unsigned char* wp = static_cast<const unsigned char*>(packed_weight);
   cudaStream_t st = as_stream(stream);
   const bool sync_ok = Cout <= 128 && stride == 1 && mode == MFN_CONV_OUT_NCHW;   // what the mma.sync kernels cover
-  if ((tuning().conv_wgmma && W >= tuning().conv_wgmma_min_w) || !sync_ok) {   // wgmma kernel
+  if (tuning().conv_wgmma || !sync_ok) {   // wgmma kernel
     const int rc = conv3x3_wgmma_launch(x, xbs, wp + conv3x3_sync_packed_bytes(Cin, Cout), bias, out, obs, N, Cin, H, W,
                                        Cout, stride, dilation, out_mode | bf16, leaky_slope, st, 0,
                                        static_cast<float*>(workspace), workspace_bytes);
@@ -375,7 +375,7 @@ extern "C" int mfn_conv3x3_forward_ws(const float* x, long long x_batch_stride, 
   }
   MFN_REQUIRE(!bf16, MFN_ERR_UNSUPPORTED,
               "mfn_conv3x3_forward: MFN_CONV_BF16 runs on the wgmma kernel only, and this launch would take the mma.sync "
-              "kernel (tuning conv_wgmma = 0, or W = %d < conv_wgmma_min_w)", W);
+              "kernel (tuning conv_wgmma = 0, or a shape the wgmma kernel declines)");
   const int nt = (Cout + 7) / 8;   // n8 tiles needed
   if (nt <= 4) return launch_conv<1, 4>(x, xbs, wp, bias, out, obs, N, Cin, H, W, Cout, dilation, leaky_slope, lin_prefix, st);
   if (nt <= 8) return launch_conv<1, 8>(x, xbs, wp, bias, out, obs, N, Cin, H, W, Cout, dilation, leaky_slope, lin_prefix, st);

@@ -289,7 +289,7 @@ __host__ __device__ inline SmemMap smem_map(int E, int CoutP, int as_wide = 3, i
     m.AS = 2;
   else if (taps_per_stage(CoutP) > 1)
     m.AS = (4 * m.a_stage + 4 * m.w_stage <= budget) ? 4 : ((3 * m.a_stage + 3 * m.w_stage <= budget) ? 3 : 2);
-  else   // as_wide (tuning "conv_as"): 2 trades an input stage for four more single-tap weight stages
+  else   // as_wide = 2 would trade an input stage for four more single-tap weight stages; the launcher passes 3
     m.AS = (as_wide >= 3 && 3 * m.a_stage + 8 * m.w_stage <= budget) ? 3 : 2;
   int ws = (budget - m.AS * m.a_stage) / m.w_stage;
   m.WS = ws > MAX_WS ? MAX_WS : ws;
@@ -1128,7 +1128,7 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   if ((out_mode >> 8) != 0 && (out_mode & 0xff) != 0) return -1;   // linear prefix only with plain NCHW output
   const int CoutP = um::cout_pad(Cout), nChunks = (Cin + 15) / 16;
   const int E = n_slots(stride, dil) * row_pitch(MT, stride, dil);
-  const int as_wide = tuning().conv_as == 2 ? 2 : 3;
+  const int as_wide = 3;   // input stages of the wide layers (smem_map)
   // staged epilogue (bulk copies of whole output row segments): plain NCHW output whose rows start 16-byte aligned
   // (split output: every row segment is 16-byte aligned; the register epilogue takes the linear prefix)
   const bool staged = (out_mode & 0xff) == 0 && ext == 0 &&

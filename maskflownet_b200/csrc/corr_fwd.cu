@@ -410,35 +410,30 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1)
 // configs[1]: 64 strips x 2 pieces of 7 tiles = 128 CTAs), so only the first tile of a CTA loads its full halo.
 // =====================================================================================================
 namespace r4 {
-// Two shapes, selected by the tile height TH (template parameter of the kernel):
-//   TH = 8: 16 warps, 1 CTA per SM, 24-row ring, two data1 stages (the original shape)
-//   TH = 4:  8 warps, 2 CTAs per SM (<= 113 KB shared memory and 128 registers each), 16-row ring, one data1 stage
-//            guarded by an mbarrier -- two independent CTAs per SM drift apart, so one CTA's loads / epilogue run under
-//            the other's tensor work.
-constexpr int TW = 32, HX = 4, HWP = TW + 2 * HX;
+constexpr int TH = 8, TW = 32, HX = 4, HWP = TW + 2 * HX;
+constexpr int NTHREADS = 64 * TH;                // 16 warps
 constexpr int PXB = 64;                          // bytes per pixel (32 channels bf16), no padding
 constexpr int ROW_BYTES = HWP * PXB;             // 2560: one split row (hi or lo)
 constexpr int F1_ROW_BYTES = TW * PXB;           // 2048
 constexpr int PASS = 3;
 constexpr int SSTR = TW + 4;                     // staging row: the tile's 32 pixels + 4 pad (keeps float4 alignment)
 constexpr int UPW = 5;                           // units per warp per batch: 4*TH + 6*TH = 10*TH = 2*TH warps x 5
-__host__ __device__ constexpr int ring_rows(int th) { return 2 * th + 8; }       // halo rows of a tile (md = 4) + TH new rows
-__host__ __device__ constexpr int f1_stages(int th) { return th == 8 ? 2 : 1; }
+constexpr int RING_ROWS = 2 * TH + 8;            // halo rows of a tile (md = 4) + TH new rows
 __host__ __device__ constexpr int stg_group_bytes(int md) { return 2 * PASS * (2 * md + 1) * SSTR * 4; }  // 2 buffers
-__host__ __device__ constexpr int smem_bytes(int md, int th) {
-  return 2 * ring_rows(th) * ROW_BYTES + f1_stages(th) * 2 * th * F1_ROW_BYTES + (th / 2) * stg_group_bytes(md) + 16;
+__host__ __device__ constexpr int smem_bytes(int md) {
+  return 2 * RING_ROWS * ROW_BYTES + 2 * 2 * TH * F1_ROW_BYTES + (TH / 2) * stg_group_bytes(md);
 }
 }  // namespace r4
 
-template <int MD, bool VEC, int TH>
-__global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
+template <int MD, bool VEC>
+__global__ void __launch_bounds__(r4::NTHREADS, 1)
     corr_mma_ring_kernel(const float* __restrict__ d1, const float* __restrict__ d2, float* __restrict__ out,
                          int N, int C, int H, int W, long long out_bs, float slope, int tilesX, int tilesY,
-                         int numTiles, int ovec, int dbg) {
+                         int numTiles, int ovec) {
   using namespace r4;
-  constexpr int NWARPS = 2 * TH, NTHREADS = 32 * NWARPS;
-  constexpr int R = ring_rows(TH), RING_LO = R * ROW_BYTES, RING_BYTES = 2 * RING_LO;
-  constexpr int F1_LO = TH * F1_ROW_BYTES, F1_STAGE = 2 * F1_LO, F1_STAGES = f1_stages(TH);
+  constexpr int NWARPS = 2 * TH;
+  constexpr int R = RING_ROWS, RING_LO = R * ROW_BYTES, RING_BYTES = 2 * RING_LO;
+  constexpr int F1_LO = TH * F1_ROW_BYTES, F1_STAGE = 2 * F1_LO;
   constexpr int UNITS_F1 = TH * 4;                 // load units (32 lanes x 8 channels) of the data1 rows
   static_assert(UNITS_F1 + 6 * TH == UPW * NWARPS, "unit split of a continuing tile must be exact");
   constexpr int G = 2 * MD + 1;
@@ -450,7 +445,6 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
   unsigned char* ring = smem_raw;
   unsigned char* f1s = smem_raw + RING_BYTES;
 
-  if (dbg & 16) return;   // profiling aid: launch overhead only
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work assignment: a CTA owns one contiguous piece of one (n, x-strip) column of tiles -- numTiles here is the number
   // of pieces per strip; strips are never changed mid-run, so only the prologue tile is "fresh"
@@ -579,13 +573,7 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
     sto[i] = dxi * SSTR + 8 * oc + 2 * j + (i & 1);
   }
   // the four warps of a row pair share a staging area (two buffers: one per pixel row) and a named barrier
-  float* stg_g = reinterpret_cast<float*>(smem_raw + RING_BYTES + F1_STAGES * F1_STAGE) + rp * (2 * SROWS * SSTR);
-  // single data1 stage: the next tile's data1 rows may only be written once every warp holds its B fragments
-  const uint32_t bar_b = smem_u32(smem_raw + RING_BYTES + F1_STAGES * F1_STAGE + (TH / 2) * stg_group_bytes(MD));
-  if (F1_STAGES == 1 && threadIdx.x == 0) {
-    mbar_init(bar_b, NWARPS);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  float* stg_g = reinterpret_cast<float*>(smem_raw + RING_BYTES + 2 * F1_STAGE) + rp * (2 * SROWS * SSTR);
   const int tig = threadIdx.x & 127;  // thread index inside the row-pair group
   auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + rp) : "memory"); };
 
@@ -701,43 +689,28 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
   TileGeo cur = geo(0, wr);
   {
     constexpr int UALL = UNITS_F1 + 6 * HR;               // units of a fresh tile
-    constexpr int UB = TH == 8 ? 8 : 6;                   // units per warp per batch of loads (registers: 8 floats each)
+    constexpr int UB = 8;                                 // units per warp per batch of loads (registers: 8 floats each)
     constexpr int NB = (UALL + UB * NWARPS - 1) / (UB * NWARPS);
-    if (!(dbg & 32)) {
 #pragma unroll 1
-      for (int b = 0; b < NB; ++b) {
-        float e[UB][8];
-        const int u0 = (b * NWARPS + warp) * UB;
+    for (int b = 0; b < NB; ++b) {
+      float e[UB][8];
+      const int u0 = (b * NWARPS + warp) * UB;
 #pragma unroll
-        for (int k = 0; k < UB; ++k) load_unit(cur, u0 + k, e[k]);
+      for (int k = 0; k < UB; ++k) load_unit(cur, u0 + k, e[k]);
 #pragma unroll
-        for (int k = 0; k < UB; ++k) store_unit(cur, u0 + k, 0, e[k]);
-      }
+      for (int k = 0; k < UB; ++k) store_unit(cur, u0 + k, 0, e[k]);
     }
   }
   __syncthreads();
-  // experiment: de-phase the two co-resident CTAs (dbg >> 16 = delay of the second-wave CTAs in units of 32 ns)
-  if ((dbg >> 16) && blockIdx.x >= kNumSMs) __nanosleep((unsigned)(dbg >> 16) * 32u);
 
   for (int s = 0; s < nStages; ++s) {
-    // ---- 1. prefetch the next tile's rows into registers (40 independent 4-byte loads per thread) ----
+    // ---- 1. L2-prefetch the next tile's rows ----
     const bool has_next = s + 1 < nStages;
     TileGeo nxt = cur;
     float pe1[16], pe2[16], peh[8];
     if (has_next) {
       nxt = geo(s + 1, wr);   // always a continuing tile: its 8 new rows go to the 8 ring slots the current tile does not use
-      if (!(dbg & 2)) {
-        if (dbg & 64) {   // profiling aid: conversion / stores without the global loads
-#pragma unroll
-          for (int c = 0; c < 16; ++c) { pe1[c] = (float)c; pe2[c] = (float)(c + lane); }
-#pragma unroll
-          for (int c = 0; c < 8; ++c) peh[c] = 1.f;
-        } else if (dbg & 256) {
-          prefetch_next(nxt, pe1, pe2, peh);   // previous scheme: register prefetch at tile start
-        } else {
-          l2_prefetch_tile(nxt);
-        }
-      }
+      l2_prefetch_tile(nxt);
     }
 
     // ---- 2. current tile ----
@@ -746,12 +719,7 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
     for (int rw = 0; rw < 2; ++rw)
 #pragma unroll
       for (int kk = 0; kk < 2; ++kk)
-        ldsm_x4(f1_u32 + (uint32_t)((F1_STAGES == 2 ? (s & 1) : 0) * F1_STAGE + (2 * rp + rw) * F1_ROW_BYTES) + offB[kk],
-                bq[rw][kk]);
-    if (F1_STAGES == 1) {   // this warp no longer needs the data1 stage
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_b);
-    }
+        ldsm_x4(f1_u32 + (uint32_t)((s & 1) * F1_STAGE + (2 * rp + rw) * F1_ROW_BYTES) + offB[kk], bq[rw][kk]);
     const int yA = cur.y0 + 2 * rp;
     float* obase = out + (size_t)cur.n * out_bs + (size_t)yA * W + cur.x0;
     const bool two_k = C > 16;
@@ -761,7 +729,7 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
       const int d0 = ps * PASS;
       // the next tile's lines were L2-prefetched at tile start: pull them into registers one pass before they are needed
       // (short L2-hit latency, hidden behind the last pass)
-      if (ps == NPASS - 1 && has_next && !(dbg & (2 | 64 | 256 | 512))) prefetch_next(nxt, pe1, pe2, peh);
+      if (ps == NPASS - 1 && has_next) prefetch_next(nxt, pe1, pe2, peh);
       float acc[2][PASS][4];
 #pragma unroll
       for (int rw = 0; rw < 2; ++rw)
@@ -769,7 +737,7 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
         for (int dd = 0; dd < PASS; ++dd)
 #pragma unroll
           for (int i = 0; i < 4; ++i) acc[rw][dd][i] = 0.f;
-      if (!(dbg & 8)) {
+      {
         // flat list of (kk, hh) steps; the fragments of step i+1 are fetched before the MMAs of step i are issued
         constexpr int NST = 2 * (PASS + 1);
         uint32_t ah[2][4], al[2][4];
@@ -806,7 +774,6 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
           }
         }
       }
-      if (dbg & 4) continue;
       // ---- epilogue of this pass (cooperative across the 4 warps of the row pair): each warp drops its 8-pixel band
       //      pieces into the group's [plane][32 px] staging buffer; then the 128 threads store full 128-byte plane rows ----
       const int nrow = (G - d0 < PASS ? G - d0 : PASS) * G;   // planes of this pass
@@ -858,20 +825,7 @@ __global__ void __launch_bounds__(64 * TH, TH == 8 ? 1 : 2)
     }
 
     // ---- 3. split / transpose the prefetched rows (a fresh strip is fetched here, after everybody left the ring) ----
-    if (has_next && !(dbg & 2)) {
-      if (dbg & 128) {   // profiling aid: global loads without conversion / stores (keep the loads alive)
-        float acc0 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) acc0 += pe1[c] + pe2[c];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) acc0 += peh[c];
-        if (acc0 == 123.456f) out[0] = acc0;
-      } else {
-        if (dbg & 512) prefetch_next(nxt, pe1, pe2, peh);   // variant: L2-hit loads only at the very end of the tile
-        if (F1_STAGES == 1) mbar_wait(bar_b, (uint32_t)(s & 1));
-        store_next(nxt, F1_STAGES == 2 ? ((s + 1) & 1) : 0, pe1, pe2, peh);
-      }
-    }
+    if (has_next) store_next(nxt, (s + 1) & 1, pe1, pe2, peh);
     cur = nxt;
     __syncthreads();
   }
@@ -929,36 +883,33 @@ static int launch_mma_impl(const float* d1, const float* d2, float* out, int N, 
                               : (VEC ? "corr_mma_kernel<2,vec>" : "corr_mma_kernel<2,scalar>"));
 }
 
-template <int MD, bool VEC, int TH>
+template <int MD, bool VEC>
 static int launch_mma_ring_impl(const float* d1, const float* d2, float* out, int N, int C, int H, int W,
                                 long long obs, float slope, cudaStream_t st) {
   using namespace r4;
   const int tilesX = (W + TW - 1) / TW, tilesY = (H + TH - 1) / TH;
   const long long tiles = (long long)N * tilesX * tilesY;
-  constexpr int NTHREADS = 64 * TH;
-  const int smem = r4::smem_bytes(MD, TH);
+  const int smem = r4::smem_bytes(MD);
   const int ovec = ((W % 4) == 0 && (obs % 4) == 0 && aligned(out, 16)) ? 1 : 0;
   static SmemOptIn opt;
   {
-    const cudaError_t e = ensure_dyn_smem(corr_mma_ring_kernel<MD, VEC, TH>, smem, opt);
+    const cudaError_t e = ensure_dyn_smem(corr_mma_ring_kernel<MD, VEC>, smem, opt);
     if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(corr_mma_ring_kernel): %s", cudaGetErrorString(e));
   }
   // strip-aligned work pieces: T = tiles per CTA if all SMs were used; each (n, x-strip) column is cut into
   // ceil(tilesY / T) pieces, one CTA per piece (e.g. level 2 of configs[1]: 64 strips x 2 pieces of 7 tiles = 128 CTAs)
-  const int cap = tuning().corr_grid_cap > 0 ? tuning().corr_grid_cap : kNumSMs * (TH == 8 ? 1 : 2);
+  const int cap = tuning().corr_grid_cap > 0 ? tuning().corr_grid_cap : kNumSMs;
   const long long strips = (long long)N * tilesX;
   const int T = (int)((tiles + cap - 1) / cap);
   int pps = (tilesY + T - 1) / T;
   if (pps < 1) pps = 1;
   if (pps > tilesY) pps = tilesY;
   const unsigned grid = (unsigned)(strips * pps);
-  corr_mma_ring_kernel<MD, VEC, TH><<<grid, NTHREADS, smem, st>>>(d1, d2, out, N, C, H, W, obs, slope, tilesX, tilesY, pps,
-                                                              ovec, tuning().corr_dbg);
-  if (TH == 8)
-    return check_launch(MD == 4 ? (VEC ? "corr_mma_ring_kernel<4,vec,th8>" : "corr_mma_ring_kernel<4,scalar,th8>")
-                                : (VEC ? "corr_mma_ring_kernel<2,vec,th8>" : "corr_mma_ring_kernel<2,scalar,th8>"));
-  return check_launch(MD == 4 ? (VEC ? "corr_mma_ring_kernel<4,vec,th4>" : "corr_mma_ring_kernel<4,scalar,th4>")
-                              : (VEC ? "corr_mma_ring_kernel<2,vec,th4>" : "corr_mma_ring_kernel<2,scalar,th4>"));
+  corr_mma_ring_kernel<MD, VEC><<<grid, NTHREADS, smem, st>>>(d1, d2, out, N, C, H, W, obs, slope, tilesX, tilesY, pps,
+                                                              ovec);
+  // the reported names keep their ",th8" suffix so that logs and tests matching them do not change
+  return check_launch(MD == 4 ? (VEC ? "corr_mma_ring_kernel<4,vec,th8>" : "corr_mma_ring_kernel<4,scalar,th8>")
+                              : (VEC ? "corr_mma_ring_kernel<2,vec,th8>" : "corr_mma_ring_kernel<2,scalar,th8>"));
 }
 
 template <int MD>
@@ -980,13 +931,9 @@ static int launch_mma(const float* d1, const float* d2, float* out, int N, int C
     const int rc = launch_corr_rb(MD, d1, d2, out, N, C, H, W, obs, slope, st);
     if (rc != -1) return rc;
   }
-  if (C <= 32 && !tuning().corr_disable_ring) {
-    if (tuning().corr_ring_th == 8)
-      return vec ? launch_mma_ring_impl<MD, true, 8>(d1, d2, out, N, C, H, W, obs, slope, st)
-                 : launch_mma_ring_impl<MD, false, 8>(d1, d2, out, N, C, H, W, obs, slope, st);
-    return vec ? launch_mma_ring_impl<MD, true, 4>(d1, d2, out, N, C, H, W, obs, slope, st)
-               : launch_mma_ring_impl<MD, false, 4>(d1, d2, out, N, C, H, W, obs, slope, st);
-  }
+  if (C <= 32)   // strip-marching ring kernel: C <= 32 shapes the TMA kernel declines
+    return vec ? launch_mma_ring_impl<MD, true>(d1, d2, out, N, C, H, W, obs, slope, st)
+               : launch_mma_ring_impl<MD, false>(d1, d2, out, N, C, H, W, obs, slope, st);
   return vec ? launch_mma_impl<MD, true>(d1, d2, out, N, C, H, W, obs, slope, st)
              : launch_mma_impl<MD, false>(d1, d2, out, N, C, H, W, obs, slope, st);
 }

@@ -207,11 +207,11 @@ int launch_corr_rb(int md, const float* d1, const float* d2, float* out, int N, 
                    cudaStream_t st) {
   using namespace rb;
   const int budget = 227 * 1024;
-  // 16-pixel strips for narrow images (half the data2 positions) -- or when forced (tuning "corr_rb_twb" = 2): the smaller
-  // tile lets two CTAs share an SM, so one CTA's load phase runs under the other's MMA phase
-  const int twb = (W <= 16 || tuning().corr_rb_twb == 2) ? 2 : 4;
+  // 16-pixel strips for narrow images (half the data2 positions): the smaller tile lets two CTAs share an SM, so one
+  // CTA's load phase runs under the other's MMA phase
+  const int twb = W <= 16 ? 2 : 4;
   const int tilesX = (W + 8 * twb - 1) / (8 * twb);
-  int rbs = tuning().corr_rb_rows > 0 ? tuning().corr_rb_rows : 4;
+  int rbs = 4;
   auto ctas = [&](int r) { return (long long)N * tilesX * ((H + r - 1) / r); };
   while (rbs > 1 && (smem_bytes(C, md, rbs, twb) > budget || ctas(rbs) < kNumSMs)) rbs >>= 1;
   if (smem_bytes(C, md, rbs, twb) > budget) return -1;

@@ -214,7 +214,6 @@ int launch_warp_lin(const float* x, const float* flow_c, const float* mask_c, co
   // channels per thread: doubled while at least one resident wave of threads (one per SM x 512) remains
   int fch = FCH;
   while (fch < 64 && fch < F && total * ((F + 2 * fch - 1) / (2 * fch)) >= (long long)kNumSMs * 512) fch *= 2;
-  if (tuning().warp_lin_fch > 0) fch = tuning().warp_lin_fch;
   const dim3 grid((unsigned)blocks, (unsigned)((F + fch - 1) / fch));
   if (border_mode == MFN_BORDER_MXNET15)
     warp_lin_kernel<MFN_BORDER_MXNET15><<<grid, 256, 0, st>>>(Yall, flow_c, mask_c, bias, tradeoff, out, fup, mup, N, H, W, F, up,

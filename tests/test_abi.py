@@ -22,6 +22,26 @@ def declared_functions():
     return out
 
 
+TUNING_KEYS = {"corr_grid_cap", "corr_tma", "corr_rb", "warp_lin", "conv_wgmma", "conv_grid_cap", "conv_splitk",
+               "conv_narrow", "conv_tma_in", "conv_dbg"}
+RETIRED_TUNING_KEYS = ("corr_ts_lo", "corr_ts_hi", "corr_disable_ring", "corr_ring_th", "corr_dbg", "corr_rb_twb",
+                       "corr_rb_rows", "warp_lin_fch", "conv_as", "conv_wgmma_min_w")
+
+
+def documented_tuning_keys():
+    """{key: default} from the list in the comment above mfn_set_tuning."""
+    src = open(HEADER).read()
+    block = re.search(r"/\*((?:(?!/\*).)*?)\*/\s*MFN_API int mfn_set_tuning", src, flags=re.S).group(1)
+    return {k: int(v) for k, v in re.findall(r'^\s*\*\s+"(\w+)"\s+default (-?\d+):', block, flags=re.M)}
+
+
+def struct_tuning_defaults():
+    """{field: default} of mfn::Tuning (csrc/common.cuh)."""
+    src = open(os.path.join(ROOT, "maskflownet_b200", "csrc", "common.cuh")).read()
+    body = re.search(r"struct Tuning \{(.*?)\};", src, flags=re.S).group(1)
+    return {k: int(v) for k, v in re.findall(r"int (\w+) = (-?\d+);", body)}
+
+
 def test_every_declared_symbol_is_exported():
     decl = declared_functions()
     assert len(decl) >= 16
@@ -68,6 +88,15 @@ def test_argument_errors_need_no_gpu():
     assert rc == -1 and b"multiples" in L.mfn_last_error()
     with pytest.raises(_lib.MaskflowError):
         _lib.set_tuning("no_such_key", 1)
+    # the header's list of tuning keys is the set the library accepts, with the defaults the library starts from
+    documented = documented_tuning_keys()
+    assert set(documented) == TUNING_KEYS, set(documented) ^ TUNING_KEYS
+    assert documented == struct_tuning_defaults()
+    for key, default in documented.items():
+        _lib.set_tuning(key, default)
+    for key in RETIRED_TUNING_KEYS:
+        with pytest.raises(_lib.MaskflowError, match="unknown key"):
+            _lib.set_tuning(key, 0)
     assert _lib.launch_count() == 0 or _lib.launch_count() >= 0
 
 

@@ -510,12 +510,8 @@ def test_bf16_bit_is_refused_where_the_wgmma_kernel_does_not_run():
     try:
         _lib.set_tuning("conv_wgmma", 0)
         assert L.mfn_conv3x3_forward_ex(*args) == -2                          # MFN_ERR_UNSUPPORTED
-        _lib.set_tuning("conv_wgmma", 1)
-        _lib.set_tuning("conv_wgmma_min_w", 64)
-        assert L.mfn_conv3x3_forward_ex(*args) == -2
     finally:
         _lib.set_tuning("conv_wgmma", 1)
-        _lib.set_tuning("conv_wgmma_min_w", 1)
     assert L.mfn_conv3x3_forward_ex(*args) == 0
     torch.cuda.synchronize()
     ref = tF.leaky_relu(tF.conv2d(x.bfloat16().double(), w.bfloat16().double(), padding=1), 0.1)

@@ -313,24 +313,21 @@ def test_native_launch_counter_moves():
 
 
 @pytest.mark.parametrize("engine", ["new", "legacy"])
-@pytest.mark.parametrize("ring_th", [4, 8])
-@pytest.mark.parametrize("cap", [1, 3, 7, 148])
+@pytest.mark.parametrize("cap", [0, 1, 3, 7, 148])
 @pytest.mark.parametrize("shape,md", [((2, 32, 45, 70), 4), ((3, 24, 31, 64), 2), ((2, 16, 27, 15), 4),
+                                      ((2, 32, 37, 64), 4), ((2, 32, 21, 50), 2), ((8, 32, 112, 256), 4),
                                       ((2, 64, 30, 40), 4), ((1, 100, 14, 36), 2)])
-def test_correlation_mma_long_tile_runs(shape, md, cap, ring_th, engine):
+def test_correlation_mma_long_tile_runs(shape, md, cap, engine):
     """Persistent-grid bookkeeping: with the grid capped, each CTA marches through many tiles / units (ring-slot recycling,
-    strip changes, barrier phase flips), and results must not depend on the grid size.  engine "new": the round-2 kernels
-    (TMA pipeline for C <= 32 with W % 4 == 0, row-block kernel for C > 32); "legacy": the round-1 ring / tile kernels,
-    which remain the fallback for shapes the new ones decline."""
+    strip changes, barrier phase flips), and results must not depend on the grid size (cap 0 = the library's own grid).
+    engine "new": the round-2 kernels (TMA pipeline for C <= 32 with W % 4 == 0, row-block kernel for C > 32); "legacy":
+    the round-1 ring / tile kernels, which remain the fallback for shapes the new ones decline.  The C <= 32 shapes give
+    the ring kernel both max displacements with vector (W % 4 == 0) and scalar loads, and the level-2 shape of the
+    benchmark (8 x 32 x 112 x 256)."""
     rng = np.random.default_rng(21)
     f1, f2 = feat(rng, shape), feat(rng, shape)
     ref = cref.correlation_forward(f1, f2, pad_size=md, max_displacement=md, threads=8)
-    if shape[1] > 32 and ring_th == 8:
-        pytest.skip("tile kernel (C > 32) has no ring shape")
-    if engine == "new" and ring_th == 8:
-        pytest.skip("ring_th only selects among the legacy kernels")
     _lib.set_tuning("corr_grid_cap", cap)
-    _lib.set_tuning("corr_ring_th", ring_th)
     if engine == "legacy":
         _lib.set_tuning("corr_tma", 0)
         _lib.set_tuning("corr_rb", 0)
@@ -340,16 +337,17 @@ def test_correlation_mma_long_tile_runs(shape, md, cap, ring_th, engine):
         name = _lib.last_kernel()
     finally:
         _lib.set_tuning("corr_grid_cap", 0)
-        _lib.set_tuning("corr_ring_th", 8)     # library default (common.cuh)
         _lib.set_tuning("corr_tma", 1)
         _lib.set_tuning("corr_rb", 1)
     assert np.abs(got - ref).max() <= 1e-4, name
     if engine == "legacy":
-        assert "corr_mma" in name, name
+        assert ("corr_mma_ring_kernel" if shape[1] <= 32 else "corr_mma_kernel") in name, name
     elif shape[1] > 32 and shape[0] * shape[2] * shape[3] <= 1024:
         assert "corr_rb_kernel" in name, name
     elif shape[1] <= 32 and shape[3] % 4 == 0:
         assert "corr_tma_kernel" in name, name
+    elif shape[1] <= 32:
+        assert "corr_mma_ring_kernel" in name, name
 
 
 def test_real_checkpoint_distribution_level2():

@@ -56,10 +56,7 @@ def main():
     ap.add_argument("--md", type=int, default=4)
     ap.add_argument("--levels", default="2,3,4,5,6")
     ap.add_argument("--algos", default="simt,mma_bf16x3,generic")
-    ap.add_argument("--ring-th", type=int, default=0, help="corr_ring_th tuning (4 or 8); 0 = library default")
     args = ap.parse_args()
-    if args.ring_th:
-        _lib.set_tuning("corr_ring_th", args.ring_th)
     H0, W0 = map(int, args.hw.split("x"))
     N = args.n
     what = args.what.split(",")
