@@ -549,6 +549,22 @@ def predict(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, resize=None)
     return flow, mask
 
 
+def _pair_flows(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, resize, bidirectional: bool) -> torch.Tensor:
+    """preprocess -> forward -> postprocess of the finest flow: (N,H,W,2) (x,y) flows of pairs (N,3,H,W), or with
+    bidirectional (2N,H,W,2), img1 -> img2 then img2 -> img1."""
+    _, _, H, W = img1.shape
+    a, b, _ = ops.preprocess(img1, img2, ops.padded_size(H, W, resize))
+    preds = net(a, b, bidirectional=True)[0] if bidirectional else net(a, b)[0]
+    return ops.postprocess(preds[-1], H, W, flip_channels=True, is_flow=True)
+
+
+def _frame_pair_flows(net: nn.Module, F: torch.Tensor, resize, bidirectional: bool) -> torch.Tensor:
+    """_pair_flows of the B pairs (F[j], F[j+1]) of a frame buffer F (B+1,H,W,3) uint8: B flows, or 2B."""
+    B = F.shape[0] - 1
+    x = F.permute(0, 3, 1, 2).contiguous()
+    return _pair_flows(net, x[:B], x[1:], resize, bidirectional)
+
+
 @torch.no_grad()
 def predict_bidirectional(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, resize=None, alpha: float = 0.01,
                           beta: float = 0.5):
@@ -563,10 +579,8 @@ def predict_bidirectional(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor
     ops.postprocess over the 2N finest flows, one ops.flow_consistency.  Returns (flow_fw, flow_bw, occ_fw, occ_bw) at the
     input size: flows (N,H,W,2) in (x,y) pixels, img1 -> img2 and img2 -> img1; masks (N,H,W) uint8, of img1's and of
     img2's pixels."""
-    N, _, H, W = img1.shape
-    a, b, _ = ops.preprocess(img1, img2, ops.padded_size(H, W, resize))
-    preds = net(a, b, bidirectional=True)[0]
-    flows = ops.postprocess(preds[-1], H, W, flip_channels=True, is_flow=True)
+    N = img1.shape[0]
+    flows = _pair_flows(net, img1, img2, resize, True)
     flow_fw, flow_bw = flows[:N], flows[N:]
     occ_fw, occ_bw = ops.flow_consistency(flow_fw, flow_bw, alpha, beta)
     return flow_fw, flow_bw, occ_fw, occ_bw
@@ -588,64 +602,100 @@ def interpolate_frames(net: nn.Module, img1: torch.Tensor, img2: torch.Tensor, t
     return ops.interpolate_frames(a, b, flow_fw, flow_bw, occ_fw, occ_bw, ts, occ_weight)
 
 
+def _check_clip(clip, batch: int, who: str, name: str = "clip") -> None:
+    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
+        raise ops.MaskflowError(f"{who}: {name} must be a (T,H,W,3) uint8 tensor")
+    if batch < 1:
+        raise ops.MaskflowError(f"{who}: batch must be >= 1, got {batch}")
+
+
+def _clip_batches(clip: torch.Tensor, batch: int):
+    """(k0, nb, F) per batch of a clip's pairs: F holds frames k0 .. k0 + batch, padded with the last frame as the
+    streamed classes pad it, and nb of its pairs are real."""
+    P = clip.shape[0] - 1
+    for k0 in range(0, P, batch):
+        yield k0, min(batch, P - k0), clip[[min(k0 + j, P) for j in range(batch + 1)]]
+
+
+def _track_batch(st, F: torch.Tensor, flows: torch.Tensor, n: int, xy=None, status=None, dropped=None):
+    """ops.track_texture of F (B+1,H,W,3), then for pairs j < n track_advance along its 2B flows and track_seed of frame
+    j + 1 into row j of xy, status and dropped (B rows allocated when not given)."""
+    B = F.shape[0] - 1
+    lam, lmax = ops.track_texture(F, st.spacing)
+    if xy is None:
+        xy = torch.empty((B, st.K, 2), dtype=torch.float32, device=F.device)
+        status = torch.empty((B, st.K), dtype=torch.uint8, device=F.device)
+        dropped = torch.empty((B,), dtype=torch.int32, device=F.device)
+    for j in range(n):
+        ops.track_advance(st, flows[j], flows[B + j])
+        ops.track_seed(st, lam[j + 1], lmax[j + 1:j + 2], xy[j], status[j], dropped[j:j + 1])
+    return xy, status, dropped
+
+
+def _segment_batch(flows: torch.Tensor, carry, alpha: float, beta: float, kw: dict):
+    """segment_motion's rule for a batch's first B frames from its 2B flows.  carry: the previous batch's last backward
+    residual and mask (frame 0's side b), overwritten with this batch's.  Returns (segment_motion's four results, the
+    backward residuals, the backward masks)."""
+    B = flows.shape[0] // 2
+    occ_fw, occ_bw = ops.flow_consistency(flows[:B], flows[B:], alpha, beta)
+    affine, _, res = ops.affine_motion(flows, want_residual=True)
+    res_b = torch.cat([carry[0], res[B:2 * B - 1]])
+    occ_b = torch.cat([carry[1], occ_bw[:B - 1]])
+    out = ops.segment_motion(res[:B], occ_fw, res_b, occ_b, flows[:B], affine[:B], **kw)
+    carry[0].copy_(res[2 * B - 1:])
+    carry[1].copy_(occ_bw[B - 1:])
+    return out, res[B:], occ_bw
+
+
+def _segment_last(res_bw, occ_bw, nb: int, shape, kw: dict):
+    """The last frame from side b alone, row nb - 1 of the last batch's; with no pair (res_bw None) an empty frame."""
+    if res_bw is None:
+        return ops.segment_motion(shape=shape, **kw)
+    return ops.segment_motion(res_b=res_bw[nb - 1:nb], occ_b=occ_bw[nb - 1:nb], **kw)
+
+
 @torch.no_grad()
 def track_video(net: nn.Module, frames: torch.Tensor, batch: int = 8, resize=None, spacing: int = 8, tau: float = 0.001,
                 alpha: float = 0.01, beta: float = 0.5, boundary=(0.01, 0.002), max_tracks=None, queries=None):
     """Dense point tracks through a clip of uint8 frames (T,H,W,3) on the device, any channel order (ops.TrackState
     for the arguments; include/maskflow_b200.h, "Dense point tracking").  Frame 0 is seeded; then the pairs go through
-    predict_bidirectional `batch` at a time (the last batch padded with the last frame, as video.VideoTracker does), the
-    texture of each batch's frames in one ops.track_texture, and per pair ops.track_advance and ops.track_seed.  This is
-    the eager chain VideoTracker captures.  Returns (xy (T,K,2) float32, status (T,K) uint8, dropped (T,) int32) on the
+    the bidirectional forward `batch` at a time (the last batch padded with the last frame, as video.VideoTracker does),
+    the texture of each batch's frames in one ops.track_texture, and per pair ops.track_advance and ops.track_seed.  This
+    is the eager chain VideoTracker captures.  Returns (xy (T,K,2) float32, status (T,K) uint8, dropped (T,) int32) on the
     device: every slot's position and status in every frame, and the seeding candidates left without a slot."""
-    if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
-        raise ops.MaskflowError("track_video: frames must be a (T,H,W,3) uint8 tensor")
-    if batch < 1:
-        raise ops.MaskflowError(f"track_video: batch must be >= 1, got {batch}")
+    _check_clip(frames, batch, "track_video", "frames")
     T, H, W, _ = frames.shape
     st = ops.TrackState(H, W, spacing, tau, alpha, beta, boundary, max_tracks, queries, device=frames.device)
     xy = torch.empty((T, st.K, 2), dtype=torch.float32, device=frames.device)
     status = torch.empty((T, st.K), dtype=torch.uint8, device=frames.device)
     dropped = torch.empty((T,), dtype=torch.int32, device=frames.device)
     ops.track_start(st, frames[0].contiguous(), xy[0], status[0], dropped[0:1])
-    P = T - 1
-    for k0 in range(0, P, batch):
-        F = frames[[min(k0 + j, P) for j in range(batch + 1)]]
-        x = F.permute(0, 3, 1, 2).contiguous()
-        flow_fw, flow_bw, _, _ = predict_bidirectional(net, x[:batch], x[1:], resize, alpha, beta)
-        lam, lmax = ops.track_texture(F, spacing)
-        for j in range(min(batch, P - k0)):
-            k = k0 + j + 1
-            ops.track_advance(st, flow_fw[j], flow_bw[j])
-            ops.track_seed(st, lam[j + 1], lmax[j + 1:j + 2], xy[k], status[k], dropped[k:k + 1])
+    for k0, nb, F in _clip_batches(frames, batch):
+        flows = _frame_pair_flows(net, F, resize, True)
+        _track_batch(st, F, flows, nb, xy[k0 + 1:], status[k0 + 1:], dropped[k0 + 1:])
     return xy, status, dropped
 
 
 @torch.no_grad()
 def stabilize_video(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=None, radius: int = 15, crop: float = 0.9,
                     iterations: int = ops.AFFINE_ITERATIONS, sigma: float = ops.AFFINE_SIGMA):
-    """A stabilised clip of uint8 frames (T,H,W,3) on the device, any channel order.  The pairs go through `predict`
+    """A stabilised clip of uint8 frames (T,H,W,3) on the device, any channel order.  The pairs go through the network
     `batch` at a time (the last batch padded with the last frame, as video.VideoStabilizer does) and each batch's flows
     through ops.affine_motion(iterations, sigma); camera.camera_path smooths the camera path over `radius` frames and
     zooms by `crop` (camera.stabilize_path states the rule; a pair whose fit failed, ok False, counts as no motion); one
     ops.warp_frames_affine warps every frame.  This is the eager chain VideoStabilizer streams.  Returns (stabilised clip
     (T,H,W,3) uint8 on the device, affine (T-1,2,3) float64 and ok (T-1,) bool on the device, M (T,2,3) float64 on the
     host: the warp of each frame, output pixel -> source position)."""
-    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
-        raise ops.MaskflowError("stabilize_video: clip must be a (T,H,W,3) uint8 tensor")
-    if batch < 1:
-        raise ops.MaskflowError(f"stabilize_video: batch must be >= 1, got {batch}")
+    _check_clip(clip, batch, "stabilize_video")
     camera.check_path_args(radius, crop, "stabilize_video")
     T, H, W, _ = clip.shape
     dev = clip.device
     P = T - 1
     affine = torch.empty((max(P, 0), 2, 3), dtype=torch.float64, device=dev)
     ok = torch.empty((max(P, 0),), dtype=torch.bool, device=dev)
-    for k0 in range(0, P, batch):
-        x = clip[[min(k0 + j, P) for j in range(batch + 1)]].permute(0, 3, 1, 2).contiguous()
-        flow, _ = predict(net, x[:batch], x[1:], resize)
-        a, g = ops.affine_motion(flow, iterations, sigma)
-        b = min(batch, P - k0)
-        affine[k0:k0 + b], ok[k0:k0 + b] = a[:b], g[:b]
+    for k0, nb, F in _clip_batches(clip, batch):
+        a, g = ops.affine_motion(_frame_pair_flows(net, F, resize, False), iterations, sigma)
+        affine[k0:k0 + nb], ok[k0:k0 + nb] = a[:nb], g[:nb]
     M = camera.camera_path(affine.cpu().numpy(), ok.cpu().numpy(), H, W, radius, crop)
     out = ops.warp_frames_affine(clip.contiguous(), torch.from_numpy(M).to(dev))
     return out, affine, ok, M
@@ -656,50 +706,39 @@ def segment_motion(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=No
                    tau_hi: float = ops.SEG_TAU_HI, min_area: int = ops.SEG_MIN_AREA,
                    max_objects: int = ops.SEG_MAX_OBJECTS, alpha: float = 0.01, beta: float = 0.5):
     """The objects moving relative to the camera in every frame of a clip of uint8 frames (T,H,W,3) on the device, any
-    channel order (ops.segment_motion states the rule).  The pairs go through predict_bidirectional `batch` at a time (the
-    last batch padded with the last frame, as video.VideoMotionSegmenter does); each batch's 2B flows through one
+    channel order (ops.segment_motion states the rule).  The pairs go through the bidirectional forward `batch` at a time
+    (the last batch padded with the last frame, as video.VideoMotionSegmenter does); each batch's 2B flows through one
     ops.affine_motion(want_residual=True) at its defaults, and one ops.segment_motion segments the batch's first frames:
     frame k0 + j takes side a from pair j and side b from pair j - 1, or for j = 0 from the previous batch's last pair
     (for frame 0: none, given as NaN residuals, which are undefined).  The last frame is segmented from side b alone.  A
     one-frame clip gives one empty frame.  This is the eager chain VideoMotionSegmenter captures.
     Returns (labels (T,H,W) uint8, objects (T,max_objects,10) float64, count (T,) int32, dropped (T,) int32) on the
     device."""
-    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
-        raise ops.MaskflowError("segment_motion: clip must be a (T,H,W,3) uint8 tensor")
-    if batch < 1:
-        raise ops.MaskflowError(f"segment_motion: batch must be >= 1, got {batch}")
+    _check_clip(clip, batch, "segment_motion")
     ops.check_segment_args(tau_lo, tau_hi, min_area, max_objects, "segment_motion")
     T, H, W, _ = clip.shape
     dev = clip.device
     kw = dict(tau_lo=tau_lo, tau_hi=tau_hi, min_area=min_area, max_objects=max_objects)
-    labels = torch.empty((T, H, W), dtype=torch.uint8, device=dev)
-    objects = torch.empty((T, max_objects, 10), dtype=torch.float64, device=dev)
-    count = torch.empty((T,), dtype=torch.int32, device=dev)
-    dropped = torch.empty((T,), dtype=torch.int32, device=dev)
+    results = (torch.empty((T, H, W), dtype=torch.uint8, device=dev),
+               torch.empty((T, max_objects, 10), dtype=torch.float64, device=dev),
+               torch.empty((T,), dtype=torch.int32, device=dev), torch.empty((T,), dtype=torch.int32, device=dev))
     P = T - 1
     if P == 0:
         with torch.cuda.device(dev):
-            labels[:], objects[:], count[:], dropped[:] = ops.segment_motion(shape=(1, H, W), **kw)
-        return labels, objects, count, dropped
-    carry_res = torch.full((1, H, W), float("nan"), dtype=torch.float32, device=dev)
-    carry_occ = torch.zeros((1, H, W), dtype=torch.uint8, device=dev)
-    B = batch
-    for k0 in range(0, P, B):
-        x = clip[[min(k0 + j, P) for j in range(B + 1)]].permute(0, 3, 1, 2).contiguous()
-        flow_fw, flow_bw, occ_fw, occ_bw = predict_bidirectional(net, x[:B], x[1:], resize, alpha, beta)
-        affine, _, res = ops.affine_motion(torch.cat([flow_fw, flow_bw]), want_residual=True)
-        res_b = torch.cat([carry_res, res[B:2 * B - 1]])
-        occ_b = torch.cat([carry_occ, occ_bw[:B - 1]])
-        out = ops.segment_motion(res[:B], occ_fw, res_b, occ_b, flow_fw, affine[:B], **kw)
-        nb = min(B, P - k0)
-        for dst, src in zip((labels, objects, count, dropped), out):
-            dst[k0:k0 + nb] = src[:nb]
-        carry_res, carry_occ = res[2 * B - 1:], occ_bw[B - 1:]
-        if k0 + nb == P:           # the last frame: side b of the last real pair
-            last = ops.segment_motion(res_b=res[B + nb - 1:B + nb], occ_b=occ_bw[nb - 1:nb], **kw)
-            for dst, src in zip((labels, objects, count, dropped), last):
-                dst[P:] = src
-    return labels, objects, count, dropped
+            last = _segment_last(None, None, 0, (1, H, W), kw)
+    elif P > 0:
+        carry = (torch.full((1, H, W), float("nan"), dtype=torch.float32, device=dev),
+                 torch.zeros((1, H, W), dtype=torch.uint8, device=dev))
+        for k0, nb, F in _clip_batches(clip, batch):
+            out, res_bw, occ_bw = _segment_batch(_frame_pair_flows(net, F, resize, True), carry, alpha, beta, kw)
+            for dst, src in zip(results, out):
+                dst[k0:k0 + nb] = src[:nb]
+        last = _segment_last(res_bw, occ_bw, nb, None, kw)      # side b of the last real pair
+    else:                                                       # an empty clip
+        return results
+    for dst, src in zip(results, last):
+        dst[P:] = src
+    return results
 
 
 @torch.no_grad()
@@ -707,15 +746,12 @@ def denoise_video(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=Non
                   sigma=None, h: float = ops.DENOISE_H, patch: int = ops.DENOISE_PATCH, alpha: float = 0.01,
                   beta: float = 0.5):
     """A denoised clip of uint8 frames (T,H,W,3) on the device, any channel order (ops.denoise_frames states the rule).
-    The pairs go through predict_bidirectional `batch` at a time (the last batch padded with the last frame, as
+    The pairs go through the bidirectional forward `batch` at a time (the last batch padded with the last frame, as
     video.VideoDenoiser does), then one ops.denoise_frames over the whole clip averages each frame with up to `radius`
     neighbours on each side along the chained flow.  sigma=None takes ops.median_noise of the clip's first
     min(T, batch + 1) frames, the frames the stream sees first.  A one-frame clip comes back unchanged.  This is the
     eager chain VideoDenoiser streams.  Returns (denoised clip (T,H,W,3) uint8 on the device, the sigma used)."""
-    if not isinstance(clip, torch.Tensor) or clip.dtype != torch.uint8 or clip.dim() != 4 or clip.shape[3] != 3:
-        raise ops.MaskflowError("denoise_video: clip must be a (T,H,W,3) uint8 tensor")
-    if batch < 1:
-        raise ops.MaskflowError(f"denoise_video: batch must be >= 1, got {batch}")
+    _check_clip(clip, batch, "denoise_video")
     ops.check_denoise_args(radius, sigma, h, patch, alpha, beta, "denoise_video", sigma_optional=True)
     T, H, W, _ = clip.shape
     clip = clip.contiguous()
@@ -723,14 +759,11 @@ def denoise_video(net: nn.Module, clip: torch.Tensor, batch: int = 8, resize=Non
         sigma = ops.median_noise(clip[:min(T, batch + 1)])
     if T == 1:
         return clip.clone(), float(sigma)
-    P = T - 1
     fw = torch.zeros((T, H, W, 2), dtype=torch.float32, device=clip.device)   # slot T-1 (no pair) is never read
     bw = torch.zeros_like(fw)
-    for k0 in range(0, P, batch):
-        x = clip[[min(k0 + j, P) for j in range(batch + 1)]].permute(0, 3, 1, 2).contiguous()
-        flow_fw, flow_bw, _, _ = predict_bidirectional(net, x[:batch], x[1:], resize, alpha, beta)
-        nb = min(batch, P - k0)
-        fw[k0:k0 + nb], bw[k0:k0 + nb] = flow_fw[:nb], flow_bw[:nb]
+    for k0, nb, F in _clip_batches(clip, batch):
+        flows = _frame_pair_flows(net, F, resize, True)
+        fw[k0:k0 + nb], bw[k0:k0 + nb] = flows[:nb], flows[batch:batch + nb]
     out = ops.denoise_frames(clip, fw, bw, radius, sigma, h, patch, alpha, beta)
     return out, float(sigma)
 

@@ -901,6 +901,17 @@ def _stab_tensor(t, nm: str, dtype, last, who: str) -> torch.Tensor:
     return t
 
 
+def check_affine_args(iterations, sigma, who: str) -> None:
+    if not (isinstance(iterations, int) and not isinstance(iterations, bool) and iterations >= 1):
+        raise MaskflowError(f"{who}: iterations must be an integer >= 1, got {iterations!r}")
+    try:
+        good = 0.0 < float(sigma) < float("inf")
+    except (TypeError, ValueError):
+        good = False
+    if not good:
+        raise MaskflowError(f"{who}: sigma must be positive and finite, got {sigma!r}")
+
+
 def affine_motion(flow: torch.Tensor, iterations: int = AFFINE_ITERATIONS, sigma: float = AFFINE_SIGMA,
                   want_residual: bool = False):
     """The camera's motion between the two images of each pair: a robust affine fit to the flow (include/maskflow_b200.h,
@@ -912,14 +923,7 @@ def affine_motion(flow: torch.Tensor, iterations: int = AFFINE_ITERATIONS, sigma
     ok is False where the last solve was ill conditioned (too few valid pixels, or all of them on one line), and affine is
     then the identity.  residual: |affine p - q| in pixels under the final fit, NaN where the pixel was left out.
     Bit-reproducible; a sample's result does not depend on the batch it is in.  Forward only."""
-    if not (isinstance(iterations, int) and not isinstance(iterations, bool) and iterations >= 1):
-        raise MaskflowError(f"affine_motion: iterations must be an integer >= 1, got {iterations!r}")
-    try:
-        good = 0.0 < float(sigma) < float("inf")
-    except (TypeError, ValueError):
-        good = False
-    if not good:
-        raise MaskflowError(f"affine_motion: sigma must be positive and finite, got {sigma!r}")
+    check_affine_args(iterations, sigma, "affine_motion")
     f = _stab_tensor(flow, "flow", torch.float32, 2, "affine_motion")
     _no_grad_path("affine_motion", f)
     N, H, W, _ = f.shape
@@ -1158,6 +1162,20 @@ def _finite_nonneg(v) -> bool:
         return False
 
 
+def check_track_args(spacing, queries, who: str) -> torch.Tensor:
+    """TrackState's rules for spacing and queries.  Returns the queries as an (M,3) float64 host tensor."""
+    if not (isinstance(spacing, int) and not isinstance(spacing, bool) and spacing >= 1):
+        raise MaskflowError(f"{who}: spacing must be an integer >= 1, got {spacing!r}")
+    q = torch.zeros((0, 3), dtype=torch.float32) if queries is None else torch.as_tensor(queries).detach()
+    if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_complex:
+        raise MaskflowError(f"{who}: queries must be (M,3) rows (t, x, y), got {tuple(q.shape)}")
+    q = q.to("cpu", torch.float64)
+    t = q[:, 0]
+    if q.shape[0] and not bool(((t >= 0) & (t < 1 << 24) & (t == torch.floor(t))).all()):
+        raise MaskflowError(f"{who}: every query's t must be an integer frame index in [0, 2^24)")
+    return q
+
+
 class TrackState:
     """Device-side state of the dense point tracker (include/maskflow_b200.h, "Dense point tracking") for H x W frames.
 
@@ -1172,8 +1190,7 @@ class TrackState:
 
     def __init__(self, H: int, W: int, spacing: int = 8, tau: float = 0.001, alpha: float = 0.01, beta: float = 0.5,
                  boundary=(0.01, 0.002), max_tracks: Optional[int] = None, queries=None, device=None):
-        if not (isinstance(spacing, int) and not isinstance(spacing, bool) and spacing >= 1):
-            raise MaskflowError(f"TrackState: spacing must be an integer >= 1, got {spacing!r}")
+        q = check_track_args(spacing, queries, "TrackState")
         if int(H) < 1 or int(W) < 1 or int(H) * int(W) >= 1 << 31:
             raise MaskflowError(f"TrackState: frame size {H}x{W} outside 1 <= H, W and H*W < 2^31")
         try:
@@ -1183,13 +1200,6 @@ class TrackState:
         for v, nm in ((tau, "tau"), (alpha, "alpha"), (beta, "beta"), (ab, "boundary alpha_b"), (bb, "boundary beta_b")):
             if not _finite_nonneg(v):
                 raise MaskflowError(f"TrackState: {nm} must be finite and non-negative, got {v!r}")
-        q = torch.zeros((0, 3), dtype=torch.float32) if queries is None else torch.as_tensor(queries).detach()
-        if q.dim() != 2 or q.shape[1] != 3 or q.dtype.is_complex:
-            raise MaskflowError(f"TrackState: queries must be (M,3) rows (t, x, y), got {tuple(q.shape)}")
-        q = q.to("cpu", torch.float64)
-        t = q[:, 0]
-        if q.shape[0] and not bool(((t >= 0) & (t < 1 << 24) & (t == torch.floor(t))).all()):
-            raise MaskflowError("TrackState: every query's t must be an integer frame index in [0, 2^24)")
         self.H, self.W, self.spacing = int(H), int(W), int(spacing)
         self.Gx, self.Gy = self.W // self.spacing, self.H // self.spacing
         self.tau, self.alpha, self.beta = float(tau), float(alpha), float(beta)

@@ -63,6 +63,12 @@ class _FrameRing:
             t0 = b
         return out
 
+    def _store(self, ring: torch.Tensor, src: torch.Tensor, t0: int) -> None:
+        """Copies frames t0 .. t0 + len(src) - 1 (src[0] is frame t0) into their slots of `ring`."""
+        n = self.ring_size
+        for a, b in self._segments(t0, t0 + len(src)):
+            ring[a % n:a % n + (b - a)].copy_(src[a - t0:b - t0])
+
 
 class VideoFlowPredictor:
     """run(frames) yields one result per consecutive pair (t, t+1), in order: the colour image (H,W,3) uint8, or
@@ -117,13 +123,10 @@ class VideoFlowPredictor:
         """The captured chain: {"rgb", "flow"}, and with bidirectional also {"flow_bw", "occ_fw", "occ_bw"}; with
         interpolate {"frames", "flow", "flow_bw", "occ_fw", "occ_bw"}."""
         B = self.batch
-        x = F.permute(0, 3, 1, 2).contiguous()
-        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
+        flows = network._frame_pair_flows(self.net, F, self.resize, self.bidirectional)
         if not self.bidirectional:
-            flow = ops.postprocess(self.net(a, b)[0][-1], H, W, flip_channels=True, is_flow=True)
-            rgb, _ = ops.flow_to_color(flow, self.max_radius, self.bgr)
-            return {"rgb": rgb, "flow": flow}
-        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
+            rgb, _ = ops.flow_to_color(flows, self.max_radius, self.bgr)
+            return {"rgb": rgb, "flow": flows}
         flow, flow_bw = flows[:B], flows[B:]
         if self.interpolate:
             occ_fw, occ_bw = ops.flow_consistency(flow, flow_bw, self.alpha, self.beta)
@@ -370,14 +373,10 @@ class VideoTracker(VideoFlowPredictor):
                  alpha: float = 0.01, beta: float = 0.5, boundary=(0.01, 0.002), max_tracks=None, queries=None,
                  depth: int = 2):
         super().__init__(net, batch=batch, resize=resize, depth=depth, bidirectional=True, alpha=alpha, beta=beta)
+        q = ops.check_track_args(spacing, None if queries is None else np.asarray(queries, np.float64), "VideoTracker")
         self.track_args = dict(spacing=spacing, tau=tau, alpha=alpha, beta=beta, boundary=boundary, max_tracks=max_tracks,
-                               queries=None if queries is None else np.asarray(queries, np.float64))
-        if not (isinstance(spacing, int) and not isinstance(spacing, bool) and spacing >= 1):
-            raise MaskflowError(f"VideoTracker: spacing must be an integer >= 1, got {spacing!r}")
-        q = self.track_args["queries"]
-        if q is not None and (q.ndim != 2 or q.shape[1] != 3):
-            raise MaskflowError(f"VideoTracker: queries must be (M,3) rows (t, x, y), got {q.shape}")
-        self.num_queries = 0 if q is None else int(q.shape[0])
+                               queries=None if queries is None else q.numpy())
+        self.num_queries = int(q.shape[0])
         self._tracks = {}
         self._first = None
 
@@ -399,18 +398,9 @@ class VideoTracker(VideoFlowPredictor):
         return e
 
     def _chain(self, F: torch.Tensor, H: int, W: int):
-        B = self.batch
         st = self._track(H, W, F.device)["state"]
-        x = F.permute(0, 3, 1, 2).contiguous()
-        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
-        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
-        lam, lmax = ops.track_texture(F, st.spacing)
-        xy = torch.empty((B, st.K, 2), dtype=torch.float32, device=F.device)
-        status = torch.empty((B, st.K), dtype=torch.uint8, device=F.device)
-        dropped = torch.empty((B,), dtype=torch.int32, device=F.device)
-        for j in range(B):
-            ops.track_advance(st, flows[j], flows[B + j])
-            ops.track_seed(st, lam[j + 1], lmax[j + 1:j + 2], xy[j], status[j], dropped[j:j + 1])
+        flows = network._frame_pair_flows(self.net, F, self.resize, True)
+        xy, status, dropped = network._track_batch(st, F, flows, self.batch)
         return {"xy": xy, "status": status, "dropped": dropped}
 
     def _outputs(self):
@@ -473,14 +463,7 @@ class VideoStabilizer(_FrameRing, VideoFlowPredictor):
                  depth: int = 2):
         super().__init__(net, batch=batch, resize=resize, depth=depth)
         camera.check_path_args(radius, crop, "VideoStabilizer")
-        if not (isinstance(iterations, int) and not isinstance(iterations, bool) and iterations >= 1):
-            raise MaskflowError(f"VideoStabilizer: iterations must be an integer >= 1, got {iterations!r}")
-        try:
-            good = 0.0 < float(sigma) < float("inf")
-        except (TypeError, ValueError):
-            good = False
-        if not good:
-            raise MaskflowError(f"VideoStabilizer: sigma must be positive and finite, got {sigma!r}")
+        ops.check_affine_args(iterations, sigma, "VideoStabilizer")
         self.radius, self.crop, self.iterations, self.sigma = int(radius), float(crop), int(iterations), float(sigma)
         self.ring_size = self.radius + self.depth * self.batch + 1
         self._rings = {}
@@ -491,10 +474,7 @@ class VideoStabilizer(_FrameRing, VideoFlowPredictor):
         self._rings.clear()
 
     def _chain(self, F: torch.Tensor, H: int, W: int):
-        B = self.batch
-        x = F.permute(0, 3, 1, 2).contiguous()
-        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
-        flow = ops.postprocess(self.net(a, b)[0][-1], H, W, flip_channels=True, is_flow=True)
+        flow = network._frame_pair_flows(self.net, F, self.resize, False)
         affine, ok = ops.affine_motion(flow, self.iterations, self.sigma)
         return {"affine": affine, "ok": ok}
 
@@ -523,9 +503,7 @@ class VideoStabilizer(_FrameRing, VideoFlowPredictor):
         if r["warped"]:
             cur.wait_event(r["ev_warp"])
         src = F if first else F[1:]
-        t0, n = v["loaded"], self.ring_size
-        for a, b in self._segments(t0, t0 + len(src)):
-            r["frames"][a % n:a % n + (b - a)].copy_(src[a - t0:b - t0])
+        self._store(r["frames"], src, v["loaded"])
         v["loaded"] += len(src)
         r["ev_ring"].record(cur)
 
@@ -643,20 +621,11 @@ class VideoMotionSegmenter(VideoFlowPredictor):
         return c
 
     def _chain(self, F: torch.Tensor, H: int, W: int):
-        B = self.batch
         c = self._carry(H, W, F.device)
-        x = F.permute(0, 3, 1, 2).contiguous()
-        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
-        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
-        occ_fw, occ_bw = ops.flow_consistency(flows[:B], flows[B:], self.alpha, self.beta)
-        affine, _, res = ops.affine_motion(flows, want_residual=True)
-        res_b = torch.cat([c["res"], res[B:2 * B - 1]])
-        occ_b = torch.cat([c["occ"], occ_bw[:B - 1]])
-        labels, objects, count, dropped = ops.segment_motion(res[:B], occ_fw, res_b, occ_b, flows[:B], affine[:B],
-                                                             **self.seg_args)
-        c["res"].copy_(res[2 * B - 1:])
-        c["occ"].copy_(occ_bw[B - 1:])
-        return {"labels": labels, "objects": objects, "count": count, "dropped": dropped, "res_bw": res[B:],
+        flows = network._frame_pair_flows(self.net, F, self.resize, True)
+        (labels, objects, count, dropped), res_bw, occ_bw = network._segment_batch(
+            flows, (c["res"], c["occ"]), self.alpha, self.beta, self.seg_args)
+        return {"labels": labels, "objects": objects, "count": count, "dropped": dropped, "res_bw": res_bw,
                 "occ_bw": occ_bw}
 
     def _outputs(self):
@@ -674,8 +643,8 @@ class VideoMotionSegmenter(VideoFlowPredictor):
         for labels, objects, count, dropped in super()._collect(s, b):
             yield MotionFrame(labels, objects[:int(count)], int(dropped))
 
-    def _segment_last(self, res_b, occ_b, shape) -> MotionFrame:
-        labels, objects, count, dropped = ops.segment_motion(res_b=res_b, occ_b=occ_b, shape=shape, **self.seg_args)
+    def _segment_last(self, res_bw, occ_bw, nb: int, shape) -> MotionFrame:
+        labels, objects, count, dropped = network._segment_last(res_bw, occ_bw, nb, shape, self.seg_args)
         n = int(count[0])
         return MotionFrame(labels[0].cpu().numpy(), objects[0, :n].cpu().numpy(), int(dropped[0]))
 
@@ -689,13 +658,13 @@ class VideoMotionSegmenter(VideoFlowPredictor):
         if len(head) == 1:                   # one frame: no pair, an empty frame
             fr = self._frame(head[0], None)
             with torch.cuda.device(dev):
-                yield self._segment_last(None, None, (1, int(fr.shape[0]), int(fr.shape[1])))
+                yield self._segment_last(None, None, 0, (1, int(fr.shape[0]), int(fr.shape[1])))
             return
         yield from super().run(itertools.chain(head, it))
         st, b = self._run                    # the graph's outputs still hold the last batch
         self._run = None
         with torch.cuda.device(dev):
-            yield self._segment_last(st["out"]["res_bw"][b - 1:b], st["out"]["occ_bw"][b - 1:b], None)
+            yield self._segment_last(st["out"]["res_bw"], st["out"]["occ_bw"], b, None)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -734,9 +703,7 @@ class VideoDenoiser(_FrameRing, VideoFlowPredictor):
 
     def _chain(self, F: torch.Tensor, H: int, W: int):
         B = self.batch
-        x = F.permute(0, 3, 1, 2).contiguous()
-        a, b, _ = ops.preprocess(x[:B], x[1:], ops.padded_size(H, W, self.resize))
-        flows = ops.postprocess(self.net(a, b, bidirectional=True)[0][-1], H, W, flip_channels=True, is_flow=True)
+        flows = network._frame_pair_flows(self.net, F, self.resize, True)
         return {"flow": flows[:B], "flow_bw": flows[B:]}
 
     def _outputs(self):
@@ -767,19 +734,16 @@ class VideoDenoiser(_FrameRing, VideoFlowPredictor):
             cur.wait_event(r["ev_done"])
         src = F if first else F[1:]
         t0 = v["loaded"]
-        n = self.ring_size
-        for a, b in self._segments(t0, t0 + len(src)):
-            r["frames"][a % n:a % n + (b - a)].copy_(src[a - t0:b - t0])
+        self._store(r["frames"], src, t0)
         v["pair0"] = 0 if first else t0 - 1          # the batch's pairs are pair0 .. pair0 + B - 1
         v["loaded"] += len(src)
 
     def _replayed(self, st) -> None:
         """Copies the batch's flows from the graph's outputs into the ring; the event marks the batch as loaded."""
         v = self._v
-        r, out, p0, n = v["ring"], st["out"], v["pair0"], self.ring_size
-        for a, b in self._segments(p0, p0 + self.batch):
-            r["fw"][a % n:a % n + (b - a)].copy_(out["flow"][a - p0:b - p0])
-            r["bw"][a % n:a % n + (b - a)].copy_(out["flow_bw"][a - p0:b - p0])
+        r, out, p0 = v["ring"], st["out"], v["pair0"]
+        self._store(r["fw"], out["flow"], p0)
+        self._store(r["bw"], out["flow_bw"], p0)
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(st["F"].device))
         v["marks"].append((p0, ev))

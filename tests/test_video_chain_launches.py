@@ -6,9 +6,10 @@ Each tool runs the bidirectional (or one-way) forward on batches of B pairs, the
 then its own kernels.  test_bidirectional_launches.py checks the forward launch by launch; the tools' kernels are checked
 in their own files on synthetic flows.  Here ChainRecorder replaces the ops the chains call through the module
 (ops.affine_motion, ops.segment_motion, ops.track_start / track_texture / track_advance / track_seed,
-ops.warp_frames_affine, ops.interpolate_frames) and network.predict_bidirectional / network.predict.  Each wrapper runs
-the original, synchronises, copies what the launch read and wrote to the host and judges that launch alone against the
-oracle on the inputs it read, with the judges of the kernels' own files:
+ops.warp_frames_affine, ops.interpolate_frames, ops.flow_consistency) and network._pair_flows, which every forward of
+the chains and of network.predict_bidirectional goes through.  Each wrapper runs the original, synchronises, copies what
+the launch read and wrote to the host and judges that launch alone against the oracle on the inputs it read, with the
+judges of the kernels' own files (the forward and the masks are logged for the wiring only):
   * affine_motion: test_stabilize._check_fit against stabilize_ref.fit (corners within 1e-6 px, residual within 1e-5 px
     plus one float32 ulp, NaN in the same places);
   * segment_motion: test_motion_segment._check against motionseg_ref.segment (labels, count, dropped, area, box,
@@ -20,10 +21,10 @@ oracle on the inputs it read, with the judges of the kernels' own files:
     against interp_ref.interpolate.
 Per-launch judging cannot see the wiring, because each launch is judged on whatever it read.  So the recorded flows,
 masks, residuals and fits are indexed by global pair p = k0 + j (the real pairs j < nb of each batch only) and the
-wiring is checked bit for bit: every fit read cat(flow_fw, flow_bw) of its batch; every segmentation read side a from
-its batch and side b from the backward rows shifted by one, row 0 from the previous batch's last pair (NaN and 0 at
-k0 = 0); the last frame reads pair P - 1's backward side alone; advance k read pair k - 1's flows and frame k - 1's
-state; seed k read frame k's texture; the padded pairs are never advanced; queries are born in their frames; the
+wiring is checked bit for bit: every fit and every pair of occlusion masks read the flows of its batch; every
+segmentation read side a from its batch and side b from the backward rows shifted by one, row 0 from the previous
+batch's last pair (NaN and 0 at k0 = 0); tracking and stabilisation compute no masks; the last frame reads pair P - 1's
+backward side alone; advance k read pair k - 1's flows and frame k - 1's state; seed k read frame k's texture; the padded pairs are never advanced; queries are born in their frames; the
 stabiliser's affine and ok rows are the fits of pairs 0..P-1, M is stabilize_ref.path of them within 1e-9 px at the
 corners and the warp read the clip and M.  Segmentation is then restated with the batching removed: frame t takes side a
 from pair t (t < P) and side b from pair t - 1 (t >= 1), through motionseg_ref.segment, and must equal the chain's
@@ -43,9 +44,9 @@ segmentation, weights never updated for the fit, the warp half a pixel off, the 
 every advance that starts from a TRACKED slot, seeding that ignores coverage, a dropped corner for the interpolation),
 and each wrong wiring must disagree with the chain: side b from pair t, frame 0's side b as residual 0 (a carry never
 reset), the last frame from pair P - 2, advance k against pair k's flows, seed k against frame k - 1's texture, the
-camera path from fits shifted by one pair.  test_wiring_restatements_on_host runs the same recorder and wiring checks
-on the CPU, with the oracles standing in for the kernels and hand-made per-pair flows, at B = 3 and P = 7: the right
-assignment passes and every wiring control fails.
+camera path from fits shifted by one pair.  test_shared_chain_wiring_restatements_on_host runs the same recorder and
+wiring checks on the CPU, with the oracles standing in for the kernels and hand-made per-pair flows, at B = 3 and P = 7:
+the right assignment passes and every wiring control fails.
 """
 import os
 import time
@@ -71,7 +72,7 @@ from test_stabilize import CORNER_TOL, WARP_EXACT, _check_fit, _check_warp, _fit
 from test_tracking import Tally, _compare_advance, _compare_seed
 
 OPS = ("affine_motion", "segment_motion", "track_start", "track_texture", "track_advance", "track_seed",
-       "warp_frames_affine", "interpolate_frames")
+       "warp_frames_affine", "interpolate_frames", "flow_consistency")
 KINDS = ("fit", "segment", "texture", "advance", "seed", "warp", "interp")
 CONTROL_KINDS = ("fit", "segment", "advance", "seed", "warp", "interp")     # the texture is compared bit for bit
 MAX_OBJECTS = 4
@@ -133,12 +134,11 @@ class ChainRecorder:
 
     def __init__(self, monkeypatch, impl=None, controls=False, workers=None):
         self.orig = {n: getattr(ops, n) for n in OPS}
-        self.orig.update(predict_bidirectional=network.predict_bidirectional, predict=network.predict)
+        self.orig.update(_pair_flows=network._pair_flows)
         self.orig.update(impl or {})
         for n in OPS:
             monkeypatch.setattr(ops, n, getattr(self, n))
-        monkeypatch.setattr(network, "predict_bidirectional", self.predict_bidirectional)
-        monkeypatch.setattr(network, "predict", self.predict)
+        monkeypatch.setattr(network, "_pair_flows", self._pair_flows)
         self.controls = controls
         self.pool = ThreadPoolExecutor(workers or min(8, os.cpu_count() or 1))
         self.tally = Tally()
@@ -149,24 +149,28 @@ class ChainRecorder:
         self.begin()
 
     def begin(self):
-        self.log = {k: [] for k in ("bidir", "predict", "start") + KINDS}
+        self.log = {k: [] for k in ("flows", "occ", "start") + KINDS}
         self.in_start = False
 
     def _map(self, fn, items):
         return self.pool.map(fn, items)
 
-    # ---- the forwards ---------------------------------------------------------------------------------------------
-    def predict_bidirectional(self, net, img1, img2, resize=None, alpha=0.01, beta=0.5):
-        res = self.orig["predict_bidirectional"](net, img1, img2, resize, alpha, beta)
+    # ---- the forwards and the occlusion masks ----------------------------------------------------------------------
+    def _pair_flows(self, net, img1, img2, resize, bidirectional):
+        flows = self.orig["_pair_flows"](net, img1, img2, resize, bidirectional)
         _sync()
-        self.log["bidir"].append(tuple(_host(t) for t in res))
-        return res
+        self.log["flows"].append(dict(flows=_host(flows), bidirectional=bidirectional))
+        return flows
 
-    def predict(self, net, img1, img2, resize=None):
-        res = self.orig["predict"](net, img1, img2, resize)
+    def flow_consistency(self, flow_fw, flow_bw, alpha=0.01, beta=0.5):
+        occ_fw, occ_bw = self.orig["flow_consistency"](flow_fw, flow_bw, alpha, beta)
         _sync()
-        self.log["predict"].append(tuple(_host(t) for t in res))
-        return res
+        i = len(self.log["flows"]) - 1
+        last = self.log["flows"][i]["flows"] if i >= 0 else None
+        n = len(flow_fw)
+        read = last is not None and _eq(_host(flow_fw), last[:n]) and _eq(_host(flow_bw), last[n:])
+        self.log["occ"].append(dict(occ_fw=_host(occ_fw), occ_bw=_host(occ_bw), flows=i if read else None))
+        return occ_fw, occ_bw
 
     # ---- stabilisation and segmentation ---------------------------------------------------------------------------
     def affine_motion(self, flow, iterations=ops.AFFINE_ITERATIONS, sigma=ops.AFFINE_SIGMA, want_residual=False):
@@ -333,29 +337,31 @@ def _seg_pairs(log, B, P):
     """Per global pair p: its forward and backward flows, masks, residuals and forward fit, from the batch launches."""
     pairs = []
     for i, j, p in _real_pairs(P, B):
-        fw, bw, ofw, obw = log["bidir"][i]
-        fit = log["fit"][i]
-        pairs.append(dict(fw=fw[j], ofw=ofw[j], obw=obw[j], res_fw=fit["res"][j], A_fw=fit["A"][j],
-                          res_bw=fit["res"][B + j]))
+        occ, fit = log["occ"][i], log["fit"][i]
+        pairs.append(dict(fw=log["flows"][i]["flows"][j], ofw=occ["occ_fw"][j], obw=occ["occ_bw"][j],
+                          res_fw=fit["res"][j], A_fw=fit["A"][j], res_bw=fit["res"][B + j]))
     return pairs
 
 
 def _seg_wiring(log, B, P, H, W):
     n = _batches(P, B)
     w = {"launches: ceil(P/B) forwards and fits, ceil(P/B) + 1 segmentations":
-         len(log["bidir"]) == n and len(log["fit"]) == n and len(log["segment"]) == n + 1}
+         len(log["flows"]) == n and all(f["bidirectional"] for f in log["flows"]) and len(log["occ"]) == n and
+         len(log["fit"]) == n and len(log["segment"]) == n + 1}
     if not all(w.values()):
         return w
     for i in range(n):
-        fw, bw, ofw, obw = log["bidir"][i]
+        fw, bw = log["flows"][i]["flows"][:B], log["flows"][i]["flows"][B:]
+        ofw, obw = log["occ"][i]["occ_fw"], log["occ"][i]["occ_bw"]
         fit, (res_a, occ_a, res_b, occ_b, flow_a, affine_a) = log["fit"][i], log["segment"][i]["ins"]
+        w[f"masks {i} read flow_fw and flow_bw of forward {i}"] = log["occ"][i]["flows"] == i
         w[f"fit {i} read cat(flow_fw, flow_bw)"] = _eq(fit["flow"], np.concatenate([fw, bw]))
         w[f"segment {i} side a: residual rows [0, B), occ_fw, flow_fw, affine[:B]"] = \
             _eq(res_a, fit["res"][:B]) and _eq(occ_a, ofw) and _eq(flow_a, fw) and _eq(affine_a, fit["A"][:B])
         if i == 0:
             carry = np.full((1, H, W), np.nan, np.float32), np.zeros((1, H, W), np.uint8)
         else:
-            carry = log["fit"][i - 1]["res"][2 * B - 1:], log["bidir"][i - 1][3][B - 1:]
+            carry = log["fit"][i - 1]["res"][2 * B - 1:], log["occ"][i - 1]["occ_bw"][B - 1:]
         w[f"segment {i} side b row 0: pair k0 - 1's backward residual and mask (NaN and 0 at k0 = 0)"] = \
             _eq(res_b[:1], carry[0]) and _eq(occ_b[:1], carry[1])
         w[f"segment {i} side b rows 1..B-1: backward rows 0..B-2"] = \
@@ -367,7 +373,7 @@ def _seg_wiring(log, B, P, H, W):
         i, nb = n - 1, P - (n - 1) * B
         w["last frame: pair P - 1's backward residual and mask alone"] = \
             all(last[k] is None for k in (0, 1, 4, 5)) and _eq(last[2], log["fit"][i]["res"][B + nb - 1:B + nb]) and \
-            _eq(last[3], log["bidir"][i][3][nb - 1:nb])
+            _eq(last[3], log["occ"][i]["occ_bw"][nb - 1:nb])
     return w
 
 
@@ -403,12 +409,14 @@ def _track_wiring(log, B, P, clip, result, queries, spacing, variant=None):
     seeds = [s for s in log["seed"] if not s["start"]]
     starts = [s for s in log["seed"] if s["start"]]
     w = {"launches: ceil(P/B) forwards and textures, P advances, P seeds (and the start's texture and seed)":
-         len(log["bidir"]) == n and len(tex) == n and len(log["advance"]) == P and len(seeds) == P and
-         len(log["start"]) == 1 and len(starts) == 1 and len(log["texture"]) == n + 1}
+         len(log["flows"]) == n and all(f["bidirectional"] for f in log["flows"]) and not log["occ"] and
+         len(tex) == n and len(log["advance"]) == P and len(seeds) == P and len(log["start"]) == 1 and
+         len(starts) == 1 and len(log["texture"]) == n + 1}
     if not all(w.values()):
         return w
-    pairs = {p: (log["bidir"][i][0][j], log["bidir"][i][1][j]) for i, j, p in _real_pairs(P, B)}
-    padded = [(log["bidir"][i][0][j], log["bidir"][i][1][j]) for i in range(n) for j in range(min(B, P - i * B), B)]
+    fl = [f["flows"] for f in log["flows"]]
+    pairs = {p: (fl[i][j], fl[i][B + j]) for i, j, p in _real_pairs(P, B)}
+    padded = [(fl[i][j], fl[i][B + j]) for i in range(n) for j in range(min(B, P - i * B), B)]
     ref0 = TR.texture(clip[0], spacing)
     w["start: frame 0's texture, frame counter 0"] = _eq(log["start"][0], clip[0]) and starts[0]["frame"] == 0 and \
         np.array_equal(starts[0]["lam"], ref0) and starts[0]["lmax"][0] == ref0.max(initial=0.0)
@@ -438,11 +446,12 @@ def _stab_wiring(log, B, P, clip, result, radius, crop, variant=None):
     H, W = clip.shape[1:3]
     n = _batches(P, B)
     w = {"launches: ceil(P/B) forwards and fits, one warp":
-         len(log["predict"]) == n and len(log["fit"]) == n and len(log["warp"]) == 1}
+         len(log["flows"]) == n and not any(f["bidirectional"] for f in log["flows"]) and not log["occ"] and
+         len(log["fit"]) == n and len(log["warp"]) == 1}
     if not all(w.values()):
         return w, float("inf")
     for i in range(n):
-        w[f"fit {i} read forward {i}'s flow"] = _eq(log["fit"][i]["flow"], log["predict"][i][0])
+        w[f"fit {i} read forward {i}'s flow"] = _eq(log["fit"][i]["flow"], log["flows"][i]["flows"])
     w["affine and ok rows are the fits of pairs 0..P-1"] = len(affine) == P and all(
         _eq(affine[p], log["fit"][i]["A"][j]) and ok[p] == log["fit"][i]["ok"][j] for i, j, p in _real_pairs(P, B))
     A, g = affine, ok
@@ -549,15 +558,20 @@ def _host_impl():
     def ids(a, b):
         return [(int(u[0, 0, 0]), int(v[0, 0, 0])) for u, v in zip(a, b)]
 
-    def predict_bidirectional(net, img1, img2, resize=None, alpha=0.01, beta=0.5):
+    served = {}          # the pair ids of each flow tensor _pair_flows returned, by its data pointer
+
+    def _pair_flows(net, img1, img2, resize, bidirectional):
         H, W = img1.shape[2:]
         p = ids(img1, img2)
-        return tuple(T(np.stack([fn(*(ij[::-1] if rev else ij), H, W) for ij in p]))
-                     for fn, rev in ((_hand_flow, False), (_hand_flow, True), (_hand_occ, False), (_hand_occ, True)))
+        flows = T(np.stack([_hand_flow(*(ij[::-1] if rev else ij), H, W)
+                            for rev in ((False, True) if bidirectional else (False,)) for ij in p]))
+        served[flows.data_ptr()] = p
+        return flows
 
-    def predict(net, img1, img2, resize=None):
-        H, W = img1.shape[2:]
-        return T(np.stack([_hand_flow(i, j, H, W) for i, j in ids(img1, img2)])), None
+    def flow_consistency(flow_fw, flow_bw, alpha=0.01, beta=0.5):
+        H, W = flow_fw.shape[1:3]
+        p = served[flow_fw.data_ptr()]
+        return tuple(T(np.stack([_hand_occ(*(ij[::-1] if rev else ij), H, W) for ij in p])) for rev in (False, True))
 
     def affine_motion(flow, iterations=ops.AFFINE_ITERATIONS, sigma=ops.AFFINE_SIGMA, want_residual=False):
         A, ok, r = SR.fit(flow.numpy(), iterations, sigma)
@@ -600,7 +614,7 @@ def _host_impl():
     def warp_frames_affine(frames, M):
         return T(SR.warp(frames.numpy(), M.numpy()))
 
-    return dict(predict_bidirectional=predict_bidirectional, predict=predict, affine_motion=affine_motion,
+    return dict(_pair_flows=_pair_flows, flow_consistency=flow_consistency, affine_motion=affine_motion,
                 segment_motion=segment_motion, track_texture=track_texture, track_advance=track_advance,
                 track_seed=track_seed, warp_frames_affine=warp_frames_affine)
 
@@ -612,7 +626,7 @@ def _hand_clip(T, H, W):
     return torch.from_numpy(clip)
 
 
-def test_wiring_restatements_on_host(monkeypatch):
+def test_shared_chain_wiring_restatements_on_host(monkeypatch):
     """B = 3, P = 7 (pairs 3 + 3 + 1, two carries): the chains run on the host with the oracles as their kernels; the
     wiring checks and the batch-free restatement pass, launch counts are the chain's, and every wrong assignment
     disagrees with the chain."""
@@ -656,7 +670,7 @@ def _thresholds(model, clip, B):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", list(RUNS))
-def test_every_launch_of_the_video_chains_against_float64(run, monkeypatch):
+def test_every_launch_of_the_shared_video_chains_against_float64(run, monkeypatch):
     cls, B, lengths, H, W, seed, interp = RUNS[run]
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
@@ -671,7 +685,8 @@ def test_every_launch_of_the_video_chains_against_float64(run, monkeypatch):
             x = clips[0][:B + 1].permute(0, 3, 1, 2).contiguous()
             rec.begin()
             frames = network.interpolate_frames(model, x[:B], x[1:], (0.25, 0.5, 0.75))
-            assert frames.shape == (B, 3, H, W, 3) and len(rec.log["bidir"]) == 1 and rec.judged["interp"] == 1
+            assert frames.shape == (B, 3, H, W, 3) and len(rec.log["flows"]) == 1 and rec.log["occ"][0]["flows"] == 0 \
+                and rec.judged["interp"] == 1
     torch.cuda.synchronize()
     secs, peak = time.perf_counter() - t0, torch.cuda.max_memory_allocated() / 2 ** 30
     monkeypatch.undo()

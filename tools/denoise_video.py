@@ -24,7 +24,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from maskflownet_b200 import ops  # noqa: E402
 from maskflownet_b200.video import VideoDenoiser  # noqa: E402
-from predict_new_data import NETWORKS, load_model, open_video, open_video_writer, video_frames  # noqa: E402
+from predict_new_data import add_model_args, model_from_args, parse_model_args, open_video, open_video_writer, video_frames  # noqa: E402
 
 
 @torch.no_grad()
@@ -52,42 +52,24 @@ def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("out_filepath", help="destination video")
     ap.add_argument("--video_filepath", required=True, help="input video")
-    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
-    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
+    add_model_args(ap)
     ap.add_argument("--radius", type=int, default=ops.DENOISE_RADIUS, help="neighbouring frames averaged on each side")
     ap.add_argument("--sigma", type=float, default=None,
                     help="noise level in grey levels (default: estimated from the first frames)")
     ap.add_argument("--h", type=float, default=ops.DENOISE_H, help="weight scale, in units of the noise level")
     ap.add_argument("--patch", type=int, default=ops.DENOISE_PATCH,
                     help=f"patch radius of the weights, in [0,{ops.DENOISE_MAX_PATCH}]")
-    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay")
-    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
-    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
-                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
-    a = ap.parse_args(argv)
-    if a.radius < 0:
-        ap.error(f"--radius must be >= 0, got {a.radius}")
-    if a.sigma is not None and not 0.0 < a.sigma < float("inf"):
-        ap.error(f"--sigma must be positive and finite, got {a.sigma}")
-    if not 0.0 < a.h < float("inf"):
-        ap.error(f"--h must be positive and finite, got {a.h}")
-    if not 0 <= a.patch <= ops.DENOISE_MAX_PATCH:
-        ap.error(f"--patch must lie in [0,{ops.DENOISE_MAX_PATCH}], got {a.patch}")
-    if a.batch < 1:
-        ap.error(f"--batch must be >= 1, got {a.batch}")
+    a = parse_model_args(ap, argv)
     try:
-        a.resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
-    except ValueError:
-        ap.error(f"--resize takes H,W, got {a.resize!r}")
-    if a.resize is not None and len(a.resize) != 2:
-        ap.error(f"--resize takes H,W, got {a.resize}")
+        ops.check_denoise_args(a.radius, a.sigma, a.h, a.patch, 0.01, 0.5, "denoise_video", sigma_optional=True)
+    except ops.MaskflowError as e:
+        ap.error(str(e))
     return a
 
 
 def main(argv=None):
     a = parse_args(argv)
-    model = load_model(a.network, a.checkpoint)
-    model.inference_precision = a.precision
+    model = model_from_args(a)
     n, fps, sigma = denoise_file(model, a.out_filepath, a.video_filepath, a.radius, a.sigma, a.h, a.patch, a.batch,
                                  a.resize)
     print(f"wrote {n} frames at {fps:g} fps to {a.out_filepath} (noise level {sigma:.2f} grey levels)")

@@ -23,7 +23,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from maskflownet_b200.video import VideoFlowPredictor  # noqa: E402
-from predict_new_data import NETWORKS, load_model, open_video, open_video_writer, video_frames  # noqa: E402
+from predict_new_data import add_model_args, model_from_args, parse_model_args, open_video, open_video_writer, video_frames  # noqa: E402
 
 
 @torch.no_grad()
@@ -69,35 +69,21 @@ def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("out_filepath", help="destination video")
     ap.add_argument("--video_filepath", required=True, help="input video")
-    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
-    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
+    add_model_args(ap)
     ap.add_argument("--factor", type=int, required=True, help="F >= 2: F-1 new frames between consecutive input frames")
-    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay")
-    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
-    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
-                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
     ap.add_argument("--fps", type=float, default=None,
                     help="output frame rate (default: the input's times F; the input's own rate gives slow motion)")
-    a = ap.parse_args(argv)
+    a = parse_model_args(ap, argv)
     if a.factor < 2:
         ap.error(f"--factor must be >= 2, got {a.factor}")
-    if a.batch < 1:
-        ap.error(f"--batch must be >= 1, got {a.batch}")
     if a.fps is not None and not 0.0 < a.fps < float("inf"):
         ap.error(f"--fps must be positive, got {a.fps}")
-    try:
-        a.resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
-    except ValueError:
-        ap.error(f"--resize takes H,W, got {a.resize!r}")
-    if a.resize is not None and len(a.resize) != 2:
-        ap.error(f"--resize takes H,W, got {a.resize}")
     return a
 
 
 def main(argv=None):
     a = parse_args(argv)
-    model = load_model(a.network, a.checkpoint)
-    model.inference_precision = a.precision
+    model = model_from_args(a)
     n, fps = interpolate_file(model, a.out_filepath, a.video_filepath, a.factor, a.batch, a.resize, a.fps)
     print(f"wrote {n} frames at {fps:g} fps to {a.out_filepath}")
 

@@ -45,6 +45,38 @@ def load_model(name: str, checkpoint: str, device="cuda") -> torch.nn.Module:
     return model.to(device).eval()
 
 
+def add_model_args(ap: argparse.ArgumentParser) -> None:
+    """The options every tool shares: -c/-n (the model), --batch, --resize and --precision.  parse_model_args checks
+    them and model_from_args loads the model they name."""
+    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
+    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
+    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay")
+    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
+    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
+                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
+
+
+def parse_model_args(ap: argparse.ArgumentParser, argv=None) -> argparse.Namespace:
+    """ap.parse_args(argv) with --batch checked and --resize turned into (H, W) (None when not given)."""
+    a = ap.parse_args(argv)
+    if a.batch < 1:
+        ap.error(f"--batch must be >= 1, got {a.batch}")
+    try:
+        a.resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
+    except ValueError:
+        ap.error(f"--resize takes H,W, got {a.resize!r}")
+    if a.resize is not None and len(a.resize) != 2:
+        ap.error(f"--resize takes H,W, got {a.resize}")
+    return a
+
+
+def model_from_args(a: argparse.Namespace) -> torch.nn.Module:
+    """The model of -c/-n on the GPU, at the arithmetic of --precision."""
+    model = load_model(a.network, a.checkpoint)
+    model.inference_precision = a.precision
+    return model
+
+
 def open_video(path: str):
     """(cv2.VideoCapture, frame rate) of a video file; the rate is 0 when the container does not give one."""
     import cv2
@@ -141,25 +173,17 @@ def main(argv=None):
     ap.add_argument("--image_1", help="first image")
     ap.add_argument("--image_2", help="second image")
     ap.add_argument("--video_filepath", help="input video")
-    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
-    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
-    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay (video)")
-    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
+    add_model_args(ap)
     ap.add_argument("--max_radius", type=float, default=None,
                     help="fixed flow magnitude (pixels) of the colour wheel's rim; default: each frame's largest flow")
-    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
-                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
     ap.add_argument("--occlusion", default=None, metavar="PATH",
                     help="also write the forward-backward occlusion mask of each pair (255 = occluded) to PATH: an image "
                          "for an image pair, a video for a video")
-    a = ap.parse_args(argv)
+    a = parse_model_args(ap, argv)
     if a.video_filepath is None and (a.image_1 is None or a.image_2 is None):
         ap.error("give --image_1 and --image_2, or --video_filepath")
-    resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
-    model = load_model(a.network, a.checkpoint)
-    model.inference_precision = a.precision
-    n = predict_files(model, a.flow_filepath, a.image_1, a.image_2, a.video_filepath, a.batch, resize, a.max_radius,
-                      a.occlusion)
+    n = predict_files(model_from_args(a), a.flow_filepath, a.image_1, a.image_2, a.video_filepath, a.batch, a.resize,
+                      a.max_radius, a.occlusion)
     print(f"wrote {n} image(s) to {a.flow_filepath}" + (f" and their occlusion masks to {a.occlusion}" if a.occlusion else ""))
 
 

@@ -20,8 +20,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from maskflownet_b200 import MaskflowError, camera  # noqa: E402
 from maskflownet_b200.video import VideoStabilizer  # noqa: E402
-from predict_new_data import NETWORKS, load_model, open_video, open_video_writer, video_frames  # noqa: E402
+from predict_new_data import add_model_args, model_from_args, parse_model_args, open_video, open_video_writer, video_frames  # noqa: E402
 
 
 @torch.no_grad()
@@ -48,34 +49,20 @@ def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("out_filepath", help="destination video")
     ap.add_argument("--video_filepath", required=True, help="input video")
-    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
-    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
+    add_model_args(ap)
     ap.add_argument("--radius", type=int, default=15, help="frames on each side of the camera path's smoothing window")
     ap.add_argument("--crop", type=float, default=0.9, help="zoom about the centre, in (0,1]: the share of the frame shown")
-    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay")
-    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
-    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
-                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
-    a = ap.parse_args(argv)
-    if a.radius < 0:
-        ap.error(f"--radius must be >= 0, got {a.radius}")
-    if not 0.0 < a.crop <= 1.0:
-        ap.error(f"--crop must lie in (0,1], got {a.crop}")
-    if a.batch < 1:
-        ap.error(f"--batch must be >= 1, got {a.batch}")
+    a = parse_model_args(ap, argv)
     try:
-        a.resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
-    except ValueError:
-        ap.error(f"--resize takes H,W, got {a.resize!r}")
-    if a.resize is not None and len(a.resize) != 2:
-        ap.error(f"--resize takes H,W, got {a.resize}")
+        camera.check_path_args(a.radius, a.crop, "stabilize_video")
+    except MaskflowError as e:
+        ap.error(str(e))
     return a
 
 
 def main(argv=None):
     a = parse_args(argv)
-    model = load_model(a.network, a.checkpoint)
-    model.inference_precision = a.precision
+    model = model_from_args(a)
     n, fps = stabilize_file(model, a.out_filepath, a.video_filepath, a.radius, a.crop, a.batch, a.resize)
     print(f"wrote {n} frames at {fps:g} fps to {a.out_filepath}")
 

@@ -24,8 +24,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from maskflownet_b200 import ops  # noqa: E402
 from maskflownet_b200.video import VideoTracker, collect_tracks  # noqa: E402
-from predict_new_data import NETWORKS, load_model, open_video, open_video_writer, video_frames  # noqa: E402
+from predict_new_data import add_model_args, model_from_args, parse_model_args, open_video, open_video_writer, video_frames  # noqa: E402
 
 
 def read_queries(path: str) -> np.ndarray:
@@ -99,36 +100,24 @@ def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("out_filepath", help="destination .npz of the tracks")
     ap.add_argument("--video_filepath", required=True, help="input video")
-    ap.add_argument("-c", "--checkpoint", required=True, help=".params checkpoint or .pt state_dict")
-    ap.add_argument("-n", "--network", choices=sorted(NETWORKS), default="MaskFlownet")
+    add_model_args(ap)
     ap.add_argument("--spacing", type=int, default=8, help="seeding grid spacing in pixels")
     ap.add_argument("--queries", default=None, help="CSV file of query points t,x,y")
     ap.add_argument("--overlay", default=None, help="also write the video with the tracks drawn")
     ap.add_argument("--tail", type=int, default=15, help="positions drawn per track in the overlay")
-    ap.add_argument("--batch", type=int, default=8, help="frame pairs per graph replay")
-    ap.add_argument("--resize", default="", help="network input size H,W (default: the next multiples of 64)")
-    ap.add_argument("--precision", choices=("fp32", "bf16"), default="fp32",
-                    help="arithmetic of the 3x3 convolutions: fp32-accurate (default) or the faster bf16 mode")
-    a = ap.parse_args(argv)
-    if a.spacing < 1:
-        ap.error(f"--spacing must be >= 1, got {a.spacing}")
+    a = parse_model_args(ap, argv)
+    try:
+        ops.check_track_args(a.spacing, None, "track_video")
+    except ops.MaskflowError as e:
+        ap.error(str(e))
     if a.tail < 1:
         ap.error(f"--tail must be >= 1, got {a.tail}")
-    if a.batch < 1:
-        ap.error(f"--batch must be >= 1, got {a.batch}")
-    try:
-        a.resize = tuple(int(s) for s in a.resize.split(",")) if a.resize else None
-    except ValueError:
-        ap.error(f"--resize takes H,W, got {a.resize!r}")
-    if a.resize is not None and len(a.resize) != 2:
-        ap.error(f"--resize takes H,W, got {a.resize}")
     return a
 
 
 def main(argv=None):
     a = parse_args(argv)
-    model = load_model(a.network, a.checkpoint)
-    model.inference_precision = a.precision
+    model = model_from_args(a)
     q = read_queries(a.queries) if a.queries else None
     n = track_file(model, a.out_filepath, a.video_filepath, a.spacing, q, a.overlay, a.tail, a.batch, a.resize)
     print(f"tracked {n} frames of {a.video_filepath} into {a.out_filepath}")
