@@ -8,7 +8,7 @@ plane of a bf16 activation, or x.to(bfloat16) for fp32 input, and w.to(bfloat16)
     |got - ref| <= 2^-20 S        plus 2^-8 |ref| where the output is stored as a bf16 activation.
 The storage term is bf16's unit roundoff: 8 significant bits, round to nearest, |v - bf16(v)| <= 2^-8 |v| (reached
 within a factor 2 by test_bf16_checker_separates_kernel_arithmetic_from_near_misses; 2^-9 would not hold).
-The LeakyReLU slope is handled by test_bench_shapes.judge.  Sensitivity: on one real launch of each kind the bound must
+The LeakyReLU slope is handled by launchcheck.bounds.judge.  Sensitivity: on one real launch of each kind the bound must
 reject, by CONTROL_MARGIN, the fp32-accurate result (float64 of the unrounded operands) and one dropped tap.
 
 The rest of the forward (correlation, warps, sampler, pre/post-processing) is the fp32 path, checked by
@@ -28,46 +28,14 @@ import torch
 import torch.nn.functional as tF
 
 from maskflownet_b200 import _lib, network, ops, video
-from test_bench_shapes import (CONTROL_MARGIN, Recorder, _conv_op, _cout_pad, _expected_convs, _groups_unchanged,
-                               _images_u8, _named_model, _outside_unchanged, _split_values, activate, channel_slopes,
-                               judge, named_init)
-from test_serving_shapes import _deterministic, _same
 
-EPS_S = 2.0 ** -20
-EPS_BF16_STORE = 2.0 ** -8
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.bounds import (CONTROL_MARGIN, EPS_S, _expected_convs, activate, bf16_bound, bf16_near_misses,
+                                bf16_terms, channel_slopes, judge)
+from launchcheck.inputs import _deterministic, _images_u8, _named_model, _same, named_init
+from launchcheck.recorders import BF16Recorder
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _bf(t):
-    return t.to(torch.bfloat16).double()
-
-
-def bf16_terms(x, w, b, stride=1, dilation=1, transposed=False):
-    """Float64 pre-activation and S of one convolution of the ROUNDED operands x, w (b as given)."""
-    op = _conv_op(transposed, stride, dilation)
-    bias = b.view(1, -1, 1, 1) if b is not None else 0.0
-    pre = op(x, w) + bias
-    S = op(x.abs(), w.abs()) + (b.abs().view(1, -1, 1, 1) if b is not None else 0.0)
-    return pre, S
-
-
-def bf16_bound(pre, S, store_from=None):
-    """2^-20 S, plus the bf16 storage rounding 2^-8 |pre| on channels >= store_from (None: fp32 output)."""
-    bound = EPS_S * S
-    if store_from is not None:
-        t = EPS_BF16_STORE * pre.abs()
-        t[:, :store_from] = 0
-        bound = bound + t
-    return bound
-
-
-def bf16_near_misses(x_full, w_full, x, w, b, stride=1, dilation=1, transposed=False):
-    """The fp32-accurate result (float64 of the unrounded operands) and the rounded operands with the first tap dropped."""
-    op = _conv_op(transposed, stride, dilation)
-    bias = b.view(1, -1, 1, 1) if b is not None else 0.0
-    w_drop = w.clone()
-    w_drop[:, :, 0, 0] = 0
-    return {"fp32": op(x_full, w_full) + bias, "tap": op(x, w_drop) + bias}
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -114,151 +82,6 @@ def test_inference_precision_values():
 # ------------------------------------------------------------------------------------------------------------------
 # GPU: the recorder
 # ------------------------------------------------------------------------------------------------------------------
-def _bf16_pad_is_zero(act):
-    N, C, H, W = act.shape
-    G = act.buf.shape[2]
-    raw = act.buf.view(torch.int16).view(N, 1, G, H, W, 8).permute(0, 1, 2, 5, 3, 4).reshape(N, G * 8, H, W)
-    return not bool(raw[:, C:].any())
-
-
-class BF16Recorder(Recorder):
-    """test_bench_shapes.Recorder with the bf16 bound: every convolution must have run the one-product variant."""
-
-    KINDS = ("fp32-s2", "bf16-io", "d2s", "lin", "dil>=4", "split-k")
-
-    def _check_conv(self, op, packed, bias, Cout, slope, dil, stride, d2s, lp, x_of, got_of, N, Cin, H, W, ws, kern,
-                    tags, store_from=None, x_full_of=None):
-        w_full, transposed = self.packs[packed.data_ptr()]
-        name = self.names.get(packed.data_ptr(), "?")
-        assert transposed == d2s, name
-        w_full = w_full.double()
-        w = w_full.float().bfloat16().double()
-        b = bias.detach().double() if bias is not None else None
-        F = Cout // 4 if d2s else Cout
-        sl = channel_slopes(F, slope, lp, w.device)
-        worst = 0.0
-        if ws:
-            tags = tags + ["split-k"]
-        with torch.no_grad():
-            for n in range(N):
-                x = x_of(n)
-                pre, S = bf16_terms(x, w, b, stride, dil, transposed)
-                bound = bf16_bound(pre, S, store_from)
-                worst = max(worst, judge(got_of(n), pre, sl, bound, S)[0])
-                for tag in tags:
-                    if tag not in self.controls:
-                        xf = x_full_of(n) if x_full_of is not None else x
-                        self.controls[tag] = (name, {k: judge(activate(v, sl), pre, sl, bound, S)[0] for k, v in
-                                                     bf16_near_misses(xf, w_full, x, w, b, stride, dil, transposed).items()})
-                del x, pre, S, bound
-        if ws:
-            ok = kern == "conv3x3_wgmma_reduce_kernel<bf16>"
-        else:
-            ok = kern.startswith(f"conv3x3_wgmma_kernel<CoutP={_cout_pad(Cout)}") and kern.endswith(",bf16>")
-        if not ok:
-            self._fail(f"{name}: kernel {kern}, expected the one-product (bf16) variant")
-        if worst > 1.0:
-            self._fail(f"{name} ({op}, N={N} Cin={Cin} Cout={Cout} {H}x{W} d={dil} s={stride}): err/bound {worst:.3g}")
-        self.rows.append(dict(op=op, name=name, kernel=kern, N=N, Cin=Cin, Cout=Cout, H=H, W=W, dil=dil, stride=stride,
-                              ws=ws, err_q=0.0, ratio=worst, tags=tags, split_out=store_from is not None))
-
-    def conv3x3_slices(self, *args, **kw):
-        a = self._bind("conv3x3_slices", args, kw)
-        if not a["bf16"]:
-            self._fail("conv3x3_slices ran without bf16 in a bf16 forward")
-        buf_in, buf_out = a["buf_in"], a["buf_out"]
-        c_in0, Cin, c_out0, Cout = a["c_in0"], a["Cin"], a["c_out0"], a["Cout"]
-        N, _, H, W = buf_in.shape
-        d2s, lp, dil, stride = a["depth_to_space"], a["linear_prefix"], a["dilation"], a["stride"]
-        ws = int(_lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, int(stride), int(dil)))
-        before = buf_out.detach().clone()
-        self.orig["conv3x3_slices"](*args, **kw)
-        torch.cuda.synchronize()
-        kern = _lib.last_kernel()
-        region = buf_out[:, c_out0:c_out0 + (Cout // 4 if d2s else Cout)]
-        if not _outside_unchanged(buf_out, before, region):
-            self._fail(f"conv3x3_slices wrote outside channels [{c_out0}, {c_out0 + Cout}) of its output buffer")
-        del before
-        tags = (["fp32-s2"] if stride == 2 else []) + (["dil>=4"] if dil >= 4 else [])
-        self._check_conv("conv3x3_slices", a["packed"], a["bias"], Cout, a["leaky_slope"], dil, stride, d2s, lp,
-                         lambda n: _bf(buf_in[n:n + 1, c_in0:c_in0 + Cin].detach()),
-                         lambda n: region[n:n + 1].detach(), N, Cin, H, W, ws, kern, tags,
-                         x_full_of=lambda n: buf_in[n:n + 1, c_in0:c_in0 + Cin].detach().double())
-
-    def conv3x3_split(self, *args, **kw):
-        a = self._bind("conv3x3_split", args, kw)
-        x, out, out_split = a["x"], a["out"], a["out_split"]
-        if not (a["bf16"] and x.bf16 and (out_split is None or out_split.bf16)):
-            self._fail("conv3x3_split ran without bf16 operands in a bf16 forward")
-        c_in0, Cin, Cout, dil, lp, d2s = a["c_in0"], a["Cin"], a["Cout"], a["dilation"], a["linear_prefix"], \
-            a["depth_to_space"]
-        N, _, H, W = x.shape
-        ws = int(_lib.lib().mfn_conv3x3_workspace_bytes(N, Cin, H, W, Cout, 1, int(dil)))
-        before = out_split.buf.clone() if out_split is not None else None
-        self.orig["conv3x3_split"](*args, **kw)
-        torch.cuda.synchronize()
-        kern = _lib.last_kernel()
-        if out_split is not None:
-            c0 = a["out_c0"]
-            if not _groups_unchanged(out_split.buf, before, c0 // 8, (c0 + Cout - lp) // 8):
-                self._fail(f"conv3x3_split wrote outside channels [{c0}, {c0 + Cout - lp}) of its bf16 output")
-            if not _bf16_pad_is_zero(out_split):
-                self._fail("conv3x3_split: pad channels of the bf16 output are not zero")
-            del before
-
-            def got_of(n):
-                v = _split_values(out_split, n, c0, c0 + Cout - lp)
-                return torch.cat([out[n:n + 1].double(), v], dim=1) if lp else v
-        else:
-            def got_of(n):
-                return out[n:n + 1]
-        tags = (["bf16-io"] if out_split is not None else []) + (["d2s"] if d2s else []) + (["lin"] if lp else []) + \
-            (["dil>=4"] if dil >= 4 else [])
-        self._check_conv("conv3x3_split", a["packed"], a["bias"], Cout, a["leaky_slope"], dil, 1, d2s, lp,
-                         lambda n: _split_values(x, n, c_in0, c_in0 + Cin), got_of, N, Cin, H, W, ws, kern, tags,
-                         lp if out_split is not None else None)
-
-    def split_pack(self, act, src, c0):
-        if not act.bf16:
-            self._fail("SplitAct.pack into a split activation in a bf16 forward")
-            return self.orig["pack"](act, src, c0)
-        N, C, H, W = src.shape
-        before = act.buf.clone()
-        self.orig["pack"](act, src, c0)
-        torch.cuda.synchronize()
-        ok = _groups_unchanged(act.buf, before, c0 // 8, (c0 + C + 15) // 16 * 2) and _bf16_pad_is_zero(act)
-        del before
-        hi, lo = act.hi_lo()
-        ok = ok and torch.equal(hi[:, c0:c0 + C], src.detach().bfloat16().float()) and not bool(lo.any())
-        if not ok:
-            self._fail(f"SplitAct.pack of {C} channels at {c0} ({N}x{H}x{W}) is not the bf16 rounding in place")
-        self.rows.append(dict(op="SplitAct.pack", name=f"[{c0}:{c0 + C}]", kernel="split_pack<bf16>", N=N, Cin=C,
-                              Cout=C, H=H, W=W, dil=0, stride=1, ws=0, err_q=0.0, ratio=0.0 if ok else float("inf"),
-                              tags=[], split_out=True))
-
-    def report(self):
-        for r in self.rows:
-            plan = f"ws={r['ws']}" if r["ws"] else "-"
-            print(f"{self.run:8s} {r['op']:17s} {r['name']:24s} {r['kernel']:42s} N={r['N']} {r['Cin']}->{r['Cout']} "
-                  f"{r['H']}x{r['W']} d={r['dil']} s={r['stride']} {plan:12s} err/bound={r['ratio']:.3f}")
-        for tag, (name, rs) in sorted(self.controls.items()):
-            print(f"{self.run:8s} control {tag:8s} on {name}: fp32-accurate err/bound={rs['fp32']:.3g}, "
-                  f"dropped tap err/bound={rs['tap']:.3g}")
-
-    # the fp32 operators of a bf16 forward run unchecked here (their own tests check them)
-    def correlation(self, *args, **kw):
-        return self.orig["correlation"](*args, **kw)
-
-    def warp_mask(self, *args, **kw):
-        return self.orig["warp_mask"](*args, **kw)
-
-    def upsample(self, *args, **kw):
-        return self.orig["upsample"](*args, **kw)
-
-    def image_warp_concat(self, *args, **kw):
-        return self.orig["image_warp_concat"](*args, **kw)
-
-
 RUNS = {   # run: (model class, batch, H, W, image seed, through network.predict)
     "fwd": (network.MaskFlownetS, 8, 448, 1024, 51, False),
     "cascade": (network.MaskFlownet, 4, 448, 1024, 52, False),   # bench.py's cascade batch: level 2 has a split-K tail
@@ -271,9 +94,8 @@ RUNS = {   # run: (model class, batch, H, W, image seed, through network.predict
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", list(RUNS))
+@pytest.mark.usefixtures("fp64_references")
 def test_every_convolution_of_a_bf16_forward_against_float64(run, monkeypatch):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     cls, N, H, W, seed, via_predict = RUNS[run]
     t0 = time.perf_counter()
     rec = BF16Recorder(monkeypatch, run)

@@ -12,11 +12,9 @@ Ambiguous pixels (where float32 and float64 may decide differently) are excluded
 |d^2 - (alpha m^2 + beta)| <= 1e-4 (d^2 + alpha m^2 + beta), or a target within 1e-3 of a frame bound.  The oracle takes
 the target x + u as the float32 sum the rule defines; everything after it is float64.
 """
-import contextlib
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -25,10 +23,12 @@ import torch
 from maskflownet_b200 import MaskflowError, _lib, network, ops
 from maskflownet_b200.video import VideoFlowPredictor
 
+from launchcheck.bidirectional import ALPHA, AMBIGUOUS_MAX, BETA, consistency_ref
+from launchcheck.emu import build, ptr
+from launchcheck.inputs import _deterministic
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-ALPHA, BETA = 0.01, 0.5
-AMBIGUOUS_MAX = 1e-3          # share of the compared pixels that may be excluded as ambiguous
 # DESIGN.md section 2, network level: 2e-3 px on flows of about 12 px, i.e. 1e-4 of the x20 flow scale.  A forward's
 # rounding error grows with its activations, so flows larger than 12 px (random-init weights) scale the bound with them.
 FLOW_TOL, FLOW_TOL_AT_PX = 1e-4 * 20.0, 12.0
@@ -39,49 +39,8 @@ def _flow_tol(*refs):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# float64 restatement of the rule (include/maskflow_b200.h, mfn_flow_consistency)
+# the comparison with the float64 restatement of the rule (launchcheck/bidirectional.py)
 # ---------------------------------------------------------------------------------------------------------------
-def _lerp(p, q, w):
-    return p * (1.0 - w) + q * w
-
-
-def _one_direction(flow, other, alpha, beta):
-    """occ (N,H,W) bool and ambiguous (N,H,W) bool for the pixels of `flow` against `other`.  The target x + u is the
-    float32 sum, as the rule defines it (one exactly specified rounding: where the other flow is steep, the bilinear
-    sample moves with the target's last bit); everything after it is float64."""
-    N, H, W, _ = flow.shape
-    y, x = np.mgrid[0:H, 0:W]
-    with np.errstate(invalid="ignore", over="ignore"):
-        qx = (x.astype(np.float32) + flow[..., 0]).astype(np.float64)
-        qy = (y.astype(np.float32) + flow[..., 1]).astype(np.float64)
-    f = flow.astype(np.float64)
-    g = other.astype(np.float64)
-    with np.errstate(invalid="ignore", over="ignore"):
-        inside = (qx >= 0) & (qx <= W - 1) & (qy >= 0) & (qy <= H - 1)
-        sx, sy = np.where(inside, qx, 0.0), np.where(inside, qy, 0.0)
-        x0, y0 = np.floor(sx).astype(np.int64), np.floor(sy).astype(np.int64)
-        x1, y1 = np.minimum(x0 + 1, W - 1), np.minimum(y0 + 1, H - 1)
-        wx, wy = sx - x0, sy - y0
-        n = np.arange(N)[:, None, None]
-        a, b, c, d = g[n, y0, x0], g[n, y0, x1], g[n, y1, x0], g[n, y1, x1]
-        bu = _lerp(_lerp(a[..., 0], b[..., 0], wx), _lerp(c[..., 0], d[..., 0], wx), wy)
-        bv = _lerp(_lerp(a[..., 1], b[..., 1], wx), _lerp(c[..., 1], d[..., 1], wx), wy)
-        u, v = f[..., 0], f[..., 1]
-        d2 = (u + bu) ** 2 + (v + bv) ** 2
-        rhs = alpha * (u * u + v * v + bu * bu + bv * bv) + beta
-        occ = ~inside | ~(d2 <= rhs) | ~np.isfinite(rhs)
-        near_rule = inside & (np.abs(d2 - rhs) <= 1e-4 * (d2 + rhs))
-        near_bound = np.minimum.reduce([np.abs(qx), np.abs(qx - (W - 1)), np.abs(qy), np.abs(qy - (H - 1))]) <= 1e-3
-    return occ, near_rule | near_bound
-
-
-def consistency_ref(flow_fw, flow_bw, alpha=ALPHA, beta=BETA):
-    """(occ_fw, occ_bw, ambiguous_fw, ambiguous_bw) of (N,H,W,2) float32 flows."""
-    occ_fw, amb_fw = _one_direction(flow_fw, flow_bw, alpha, beta)
-    occ_bw, amb_bw = _one_direction(flow_bw, flow_fw, alpha, beta)
-    return occ_fw, occ_bw, amb_fw, amb_bw
-
-
 def _compare(got_fw, got_bw, flow_fw, flow_bw, alpha=ALPHA, beta=BETA):
     """Masks against the oracle outside the ambiguous pixels; returns (excluded, compared) pixel counts."""
     occ_fw, occ_bw, amb_fw, amb_bw = consistency_ref(flow_fw, flow_bw, alpha, beta)
@@ -141,17 +100,9 @@ def _known_answers(consistency):
 # ---------------------------------------------------------------------------------------------------------------
 # CPU: the kernel source on the host
 # ---------------------------------------------------------------------------------------------------------------
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libconsistency_emu.so")
-    src = os.path.join(HERE, "host_emu", "consistency_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "consistency_emu")
     L.emu_flow_consistency.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_float] * 2
     return L
 
@@ -162,7 +113,7 @@ def _emu_consistency(emu, flow_fw, flow_bw, alpha=ALPHA, beta=BETA):
     N, H, W, _ = fw.shape
     occ_fw = np.full((N, H, W), 7, np.uint8)
     occ_bw = np.full((N, H, W), 7, np.uint8)
-    emu.emu_flow_consistency(_ptr(fw), _ptr(bw), _ptr(occ_fw), _ptr(occ_bw), N, H, W, alpha, beta)
+    emu.emu_flow_consistency(ptr(fw), ptr(bw), ptr(occ_fw), ptr(occ_bw), N, H, W, alpha, beta)
     return occ_fw, occ_bw
 
 
@@ -272,16 +223,6 @@ def test_flow_consistency_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------
 # GPU: predict_bidirectional
 # ---------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
 def _model(cls):
     torch.manual_seed(7)
     return cls().cuda().eval()

@@ -11,9 +11,9 @@ to 1088x1920) the dispatch differs from every shape test_bench_shapes.py and tes
     sample 14 on its entries lie past 2^32 bytes.
 test_split_plans_of_the_bidirectional_shapes pins those plans on the CPU (mfn_conv3x3_workspace_bytes is host
 arithmetic).  test_every_launch_of_a_bidirectional_forward_against_float64 runs predict_bidirectional through
-ServingRecorder (test_serving_shapes.py: the float64 recorder of test_bench_shapes.py, its bounds and controls, and
+ServingRecorder (launchcheck.recorders: the float64 recorder of test_bench_shapes.py, its bounds and controls, and
 pre- / post-processing against oracle/prepost_ref), extended here with:
-  * ops.flow_consistency against test_bidirectional.consistency_ref outside the ambiguous pixels;
+  * ops.flow_consistency against launchcheck.bidirectional.consistency_ref outside the ambiguous pixels;
   * the wiring, bit for bit, which per-launch judging cannot see (each launch is judged on the inputs it read): the
     first pyramid launch reads the ops.preprocess buffer in place; every S-head correlation reads the pyramid output as
     its first operand, and at level 6 its halves swapped as its second; every S-head warp warps the swapped pyramid
@@ -29,7 +29,7 @@ pre- / post-processing against oracle/prepost_ref), extended here with:
     decisions near the threshold and at the frame's edges: about 0.3 % of them at 1080p for MaskFlownet-S, 0.05 % for
     the cascade, whose flows leave almost every pixel occluded.  A share of the pixels (a multiple of AMBIGUOUS_MAX)
     would ask more of this control than such flows give; the count it is held to is what the comparison could hide.
-The flow heads are scaled by test_unsup_step_launches.FLOW_HEAD_SCALE, so that the occluded share of each direction lies
+The flow heads are scaled by launchcheck.inputs.FLOW_HEAD_SCALE, so that the occluded share of each direction lies
 strictly inside (0, 1) and both decisions are reached.  hd8 runs once more in bf16 mode under BF16Recorder
 (test_bf16_mode.py), and VideoFlowPredictor(bidirectional=True) must replay its eager chain bit for bit at batch 8 on a
 9-frame 1080p clip.
@@ -48,12 +48,13 @@ import torch.nn.functional as tF
 from maskflownet_b200 import _lib, network, ops
 from maskflownet_b200.video import VideoFlowPredictor
 from oracle import torch_ref
-from test_bench_shapes import (CONTROL_MARGIN, EPS_Q, EPS_S, Recorder, _expected_convs, _images_u8, _named_model,
-                               activate, channel_slopes, conv_terms, judge, split_storage_term)
-from test_bf16_mode import BF16Recorder
-from test_bidirectional import AMBIGUOUS_MAX, consistency_ref
-from test_serving_shapes import ServingRecorder, _cover_tiny, _cover_tiny_cascade, _deterministic, _same
-from test_unsup_step_launches import FLOW_HEAD_SCALE
+
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.bidirectional import AMBIGUOUS_MAX, consistency_ref
+from launchcheck.bounds import (CONTROL_MARGIN, EPS_Q, EPS_S, _expected_convs, activate, channel_slopes, conv_terms,
+                                judge, split_storage_term)
+from launchcheck.inputs import _clip, _deterministic, _images_u8, _same, _scaled_model
+from launchcheck.recorders import BF16Recorder, Recorder, ServingRecorder, _cover_tiny, _cover_tiny_cascade
 
 HD_CASCADE_PAIRS = 8
 
@@ -326,21 +327,6 @@ SHAPES = {   # run: (model class, pairs, H, W, image seed, coverage)
 }
 
 
-def _scaled_model(cls):
-    model = _named_model(cls).eval()
-    with torch.no_grad():
-        for k, p in model.named_parameters():
-            if "pred_flow" in k or "dc_conv7" in k:
-                p.mul_(FLOW_HEAD_SCALE)
-    return model
-
-
-def _clip(seed, T, H, W):
-    """T uint8 frames (T,3,H,W) on the device: one seeded image moving by (2, -3) px per frame."""
-    base = _images_u8(seed=seed, n=1, h=H, w=W)[0][0]
-    return torch.stack([torch.roll(base, shifts=(2 * t, -3 * t), dims=(1, 2)) for t in range(T)]).contiguous()
-
-
 def _inputs(run):
     cls, n, H, W, seed, _ = SHAPES[run]
     if run == "clip":
@@ -351,9 +337,8 @@ def _inputs(run):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", list(SHAPES))
+@pytest.mark.usefixtures("fp64_references")
 def test_every_launch_of_a_bidirectional_forward_against_float64(run, monkeypatch):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     cls, n, H, W, seed, cover = SHAPES[run]
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
@@ -408,10 +393,9 @@ def test_every_launch_of_a_bidirectional_forward_against_float64(run, monkeypatc
 
 
 @pytest.mark.gpu
+@pytest.mark.usefixtures("fp64_references")
 def test_every_convolution_of_a_bf16_bidirectional_forward_against_float64(monkeypatch):
     """hd8 in bf16 mode: every convolution meets the bf16 bound of test_bf16_mode.py and ran the one-product variant."""
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
     t0 = time.perf_counter()

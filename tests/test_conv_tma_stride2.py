@@ -12,8 +12,9 @@ import pytest
 import torch
 
 from maskflownet_b200 import _lib, network, ops
-from test_conv_tma_input import check, feat, run_both, weights
-from test_serving_shapes import _deterministic, _same
+
+from launchcheck.conv_tma import check, feat, run_both, weights
+from launchcheck.inputs import _deterministic, _same
 
 # (N, Cin, Cout, H, W): conv1a / conv2a / conv3a at the benchmark's size (both images, batch 8), and the cascade's conv1x
 # (its 4-channel input, batch 4, one image per pyramid pass)

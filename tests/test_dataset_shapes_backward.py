@@ -9,7 +9,7 @@ The loss sees the mask after the geometry augmentation: fractional, and for KITT
 way PipelineFlownet._train_batch does -- uint8 frames and a flow label at the dataset's size, augment.geometry_augment
 with fixed draws, ColorAugmentation with the reference's arguments for the dataset, network.centralize, the model in train
 mode, losses.multiscale_epe(eps=1e-8, q) and its backward -- and checks every launch while it happens with the recorders
-of test_bench_shapes.py (forward) and test_bench_shapes_backward.py (backward), bounds and controls included.
+Recorder (forward) and BackwardRecorder (backward) of launchcheck.recorders, bounds and controls included.
 
 The KITTI runs also place exact zeros: after the forward the label of a patch is set to ops.upsample(preds[-1], 4), which
 the loss kernel's own up-sampling reproduces bit for bit (asserted), so there d = 0 at scale 4, s = eps and the q-gradient's
@@ -22,8 +22,11 @@ import pytest
 import torch
 
 from maskflownet_b200 import augment, losses, network
-from test_bench_shapes import Recorder, _images_u8, _named_model
-from test_bench_shapes_backward import CONTROL_MARGIN, BackwardRecorder
+
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.bounds import CONTROL_MARGIN
+from launchcheck.inputs import _images_u8, _named_model
+from launchcheck.recorders import BackwardRecorder, Recorder
 
 EPS = 1e-8
 # The q-gradient's bound is vacuous at an element where the box of the kernel's fp32 d leaves it no tighter than the
@@ -81,9 +84,8 @@ def _frames(dataset, N, seed):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", list(RUNS))
+@pytest.mark.usefixtures("fp64_references")
 def test_every_launch_of_a_dataset_training_step_against_float64(run, monkeypatch):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     dataset, cls, N, q, det, seed = RUNS[run]
     orig, target, geo_args, col_args = DATASETS[dataset]
     torch.cuda.synchronize()

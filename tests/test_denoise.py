@@ -18,11 +18,9 @@ purpose; on the GPU at most FLIPPED = 1e-5 of the values may differ by more than
 on the host, which evaluates the kernel source without contraction, none may.  The noise estimate is an exact integer
 sum and one float64 expression: bit-identical.
 """
-import contextlib
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -32,6 +30,9 @@ from scipy.ndimage import binary_dilation, binary_erosion, gaussian_filter, map_
 from maskflownet_b200 import MaskflowError, _lib, network, ops
 from maskflownet_b200.video import VideoDenoiser, VideoFlowPredictor
 from oracle import denoise_ref as R
+
+from launchcheck.emu import build, ptr
+from launchcheck.inputs import _deterministic
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -78,17 +79,9 @@ HOST_SHAPES = [(1, 1, 257), (1, 257, 1), (3, 37, 53), (2, 20, 40)]
 # ---------------------------------------------------------------------------------------------------------------
 # the host build and the two ways to run the kernels
 # ---------------------------------------------------------------------------------------------------------------
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libdenoise_emu.so")
-    src = os.path.join(HERE, "host_emu", "denoise_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out,
-                    src], check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "denoise_emu")
     v, i, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
     L.emu_denoise_frames.argtypes = [v] * 4 + [i] * 9 + [f] * 4
     L.emu_noise_sigma.argtypes = [v] * 3 + [i] * 3
@@ -103,7 +96,7 @@ def _host_ops(L):
         n = t_hi - t0 + 1 if n is None else n
         out = np.zeros((n, H, W, 3), np.uint8)
         frames, fw, bw = (np.ascontiguousarray(a) for a in (frames, fw, bw))
-        L.emu_denoise_frames(_ptr(frames), _ptr(fw), _ptr(bw), _ptr(out), S, H, W, t0, n, t_lo, t_hi, radius, patch,
+        L.emu_denoise_frames(ptr(frames), ptr(fw), ptr(bw), ptr(out), S, H, W, t0, n, t_lo, t_hi, radius, patch,
                              sigma, h, alpha, beta)
         return out
 
@@ -111,7 +104,7 @@ def _host_ops(L):
         frames = np.ascontiguousarray(frames)
         F, H, W, _ = frames.shape
         s, S = np.zeros(F), np.zeros(F, np.int64)
-        L.emu_noise_sigma(_ptr(frames), _ptr(s), _ptr(S), F, H, W)
+        L.emu_noise_sigma(ptr(frames), ptr(s), ptr(S), F, H, W)
         return s, S
     return denoise, noise
 
@@ -483,16 +476,6 @@ def test_ops_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------
 # GPU: the eager chain and the stream
 # ---------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
 def _model(cls):
     torch.manual_seed(7)
     return cls().cuda().eval()

@@ -23,6 +23,9 @@ import torch
 from maskflownet_b200 import _lib, ops
 from oracle import torch_ref
 
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.emu import build, ptr
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
@@ -38,20 +41,12 @@ def det_mode(on=True, warn_only=False):
         torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
 
 
-def _ptr(a):
-    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
-
-
 # ---------------------------------------------------------------------------------------------------------------
 # CPU: the kernel source on the host
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libdet_emu.so")
-    src = os.path.join(HERE, "host_emu", "det_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "det_emu")
     L.emu_det_bits.argtypes = [ctypes.c_longlong]
     L.emu_det_scale.argtypes = [ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]
     L.emu_bilinear_sampler_backward_det.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_int] * 6 + [ctypes.c_void_p]
@@ -99,8 +94,8 @@ def _run_sampler_det(emu, go, data, grid, order):
     H, W = data.shape[2:]
     gd = np.zeros(data.shape, np.float32)
     gg = np.full((N, 2, OH, OW), np.nan, np.float32)
-    emu.emu_bilinear_sampler_backward_det(_ptr(go), _ptr(data), _ptr(grid), _ptr(gd), _ptr(gg), N, C, H, W, OH, OW,
-                                          _ptr(np.ascontiguousarray(order, np.int64)))
+    emu.emu_bilinear_sampler_backward_det(ptr(go), ptr(data), ptr(grid), ptr(gd), ptr(gg), N, C, H, W, OH, OW,
+                                          ptr(np.ascontiguousarray(order, np.int64)))
     return gd, gg
 
 
@@ -173,9 +168,9 @@ def test_k4_bound_pass_on_host(emu):
     N, F, HW = 2, 5, 37
     g = rng.standard_normal((N, F, HW)).astype(np.float32)
     want = np.abs(g).sum(axis=1, dtype=np.float64).max()
-    assert abs(emu.emu_pixel_abs_sum_max(_ptr(g), N, F, HW) - want) <= 1e-6 * want
+    assert abs(emu.emu_pixel_abs_sum_max(ptr(g), N, F, HW) - want) <= 1e-6 * want
     g[1, 3, 7] = np.nan
-    assert np.isnan(emu.emu_pixel_abs_sum_max(_ptr(g), N, F, HW))
+    assert np.isnan(emu.emu_pixel_abs_sum_max(ptr(g), N, F, HW))
 
 
 @pytest.mark.parametrize("layout", ["weight_partials", "plane_slices"])
@@ -197,7 +192,7 @@ def test_ordered_sum_is_order_independent(emu, layout):
     want = (base + want).astype(np.float32) if acc else want
     for seed in range(3):
         out = base.copy()
-        emu.emu_ordered_sum(_ptr(part), nparts, ps, es, _ptr(out), n, acc, _ptr(np.random.default_rng(seed).permutation(n)))
+        emu.emu_ordered_sum(ptr(part), nparts, ps, es, ptr(out), n, acc, ptr(np.random.default_rng(seed).permutation(n)))
         assert np.array_equal(out, want)
 
 
@@ -285,6 +280,7 @@ def _warp_mask_grads(arrs, go, gflow, border):
 @pytest.mark.gpu
 @pytest.mark.parametrize("N,C,F,H,W", [(2, 12, 12, 8, 12), (8, 32, 32, 96, 128)])   # + BASELINE configs[2] level 2
 @pytest.mark.parametrize("border", [0, 1])
+@pytest.mark.usefixtures("fp64_references")
 def test_warp_mask_backward_det(N, C, F, H, W, border):
     # the reference in fp32, like tests/test_ops_gpu.py: it rounds the sample positions as the kernels do, which matters at
     # the discontinuous MXNET15 border (a position just below 0 reads nothing, just above it reads pixel 0)

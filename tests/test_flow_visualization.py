@@ -9,7 +9,6 @@ command line on a small video and an image pair.
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,13 +18,12 @@ from maskflownet_b200 import MaskflowError, network, ops
 from maskflownet_b200.video import VideoFlowPredictor
 from oracle import flowvis_ref
 
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.emu import build, ptr
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 WHITE = (255, 255, 255)
-
-
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
 
 
 def _random_flow(rng, N, H, W, scale=5.0):
@@ -47,11 +45,7 @@ def _check_against_oracle(rgb, rad_max, flow, max_radius, bgr):
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libflowvis_emu.so")
-    src = os.path.join(HERE, "host_emu", "flowvis_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "flowvis_emu")
     L.emu_flow_to_color.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int] * 3 + [ctypes.c_float, ctypes.c_int]
     L.emu_wheel_taps.argtypes = [ctypes.c_float, ctypes.c_float] + [ctypes.c_void_p] * 3
     return L
@@ -62,7 +56,7 @@ def _emu_color(emu, flow, max_radius=None, bgr=False):
     N, H, W, _ = flow.shape
     rgb = np.full((N, H, W, 3), 7, np.uint8)
     rad = np.full(N, np.nan, np.float32)
-    emu.emu_flow_to_color(_ptr(flow), _ptr(rgb), _ptr(rad), N, H, W, 0.0 if max_radius is None else max_radius, int(bgr))
+    emu.emu_flow_to_color(ptr(flow), ptr(rgb), ptr(rad), N, H, W, 0.0 if max_radius is None else max_radius, int(bgr))
     return rgb, rad
 
 
@@ -180,12 +174,11 @@ def _frames(n, H=100, W=150, seed=4):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cls,max_radius,bgr", [(network.MaskFlownetS, None, False), (network.MaskFlownet, 8.0, True)])
+@pytest.mark.usefixtures("fp64_references")
 def test_video_predictor_graph_equals_eager_chain(cls, max_radius, bgr):
     """11 frames at batch 4: two full batches and one of 2 pairs.  Each result equals, bit for bit, network.predict +
     ops.flow_to_color run eagerly on the same 4-pair batch (the last one padded with the last frame), since the
     convolutions' split-K plan depends on the batch."""
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     model = _model(cls)
     frames = _frames(11)
     B, resize = 4, (128, 192)

@@ -11,8 +11,6 @@ fractional parts in [0.2, 0.8] (flows = multiples of 16 pixels + that fraction: 
 taps are multiples of 1/4), and displacements of up to 32 pixels so that samples leave the image.
 """
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -22,11 +20,8 @@ import torch.nn.functional as tF
 from maskflownet_b200 import _lib
 from oracle import torch_ref
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _ptr(a):
-    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.emu import build, ptr
 
 
 def _positions(rng, shape, lo, hi):
@@ -50,11 +45,7 @@ def _rel_err(got, want):
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libimage_warp_bwd_emu.so")
-    src = os.path.join(HERE, "host_emu", "image_warp_bwd_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "image_warp_bwd_emu")
     L.emu_image_warp_concat_backward.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int] * 4 + [ctypes.c_float]
     return L
 
@@ -73,14 +64,14 @@ def test_kernel_source_bilinear_sampler_backward_on_host(emu):
         torch.from_numpy(go).double())
     base = rng.standard_normal(data.shape).astype(np.float32)                           # accumulated into
     gd, gg = base.copy(), np.full_like(grid, np.nan)
-    emu.emu_bilinear_sampler_backward(_ptr(go), _ptr(data), _ptr(grid), _ptr(gd), _ptr(gg), N, C, H, W, OH, OW)
+    emu.emu_bilinear_sampler_backward(ptr(go), ptr(data), ptr(grid), ptr(gd), ptr(gg), N, C, H, W, OH, OW)
     assert _rel_err(gd - base, d.grad.numpy()) < 2e-5
     assert _rel_err(gg, g.grad.numpy()) < 2e-5
     gg2 = np.full_like(grid, np.nan)                                                    # grid only, data only
-    emu.emu_bilinear_sampler_backward(_ptr(go), _ptr(data), _ptr(grid), None, _ptr(gg2), N, C, H, W, OH, OW)
+    emu.emu_bilinear_sampler_backward(ptr(go), ptr(data), ptr(grid), None, ptr(gg2), N, C, H, W, OH, OW)
     assert np.array_equal(gg, gg2)
     gd2 = np.zeros_like(data)
-    emu.emu_bilinear_sampler_backward(_ptr(go), _ptr(data), _ptr(grid), _ptr(gd2), None, N, C, H, W, OH, OW)
+    emu.emu_bilinear_sampler_backward(ptr(go), ptr(data), ptr(grid), ptr(gd2), None, N, C, H, W, OH, OW)
     assert _rel_err(gd2, d.grad.numpy()) < 2e-5
 
 
@@ -93,7 +84,7 @@ def test_kernel_source_grid_generator_backward_on_host(emu):
     gg = rng.standard_normal((N, 2, H, W)).astype(np.float32)
     grid.backward(torch.from_numpy(gg).double())
     gf = np.full_like(gg, np.nan)
-    emu.emu_grid_generator_warp_backward(_ptr(gg), _ptr(gf), N, H, W)
+    emu.emu_grid_generator_warp_backward(ptr(gg), ptr(gf), N, H, W)
     assert _rel_err(gf, flow.grad.numpy()) < 1e-6
 
 
@@ -120,7 +111,7 @@ def test_kernel_source_image_warp_concat_backward_on_host(emu):
     assert ((pos[:, 0] < 0) | (pos[:, 0] > H - 1) | (pos[:, 1] < 0) | (pos[:, 1] > W - 1)).mean() > 0.2
     base = rng.standard_normal(im2.shape).astype(np.float32)
     gi2, gfu, gmu = base.copy(), np.full((N, 2, H, W), np.nan, np.float32), np.full((N, 1, H, W), np.nan, np.float32)
-    emu.emu_image_warp_concat_backward(_ptr(g40), _ptr(im2), _ptr(fq), _ptr(mq), _ptr(gi2), _ptr(gfu), _ptr(gmu),
+    emu.emu_image_warp_concat_backward(ptr(g40), ptr(im2), ptr(fq), ptr(mq), ptr(gi2), ptr(gfu), ptr(gmu),
                                        N, Ci, H, W, scale)
     assert _rel_err(gi2 - base, want_i2) < 2e-5
     assert _rel_err(gfu, want_fu) < 2e-5
@@ -128,7 +119,7 @@ def test_kernel_source_image_warp_concat_backward_on_host(emu):
     for which in range(3):                       # each output alone gives the same numbers
         outs = [None, None, None]
         outs[which] = np.zeros_like((gi2, gfu, gmu)[which])
-        emu.emu_image_warp_concat_backward(_ptr(g40), _ptr(im2), _ptr(fq), _ptr(mq), *[_ptr(o) for o in outs], N, Ci, H, W,
+        emu.emu_image_warp_concat_backward(ptr(g40), ptr(im2), ptr(fq), ptr(mq), *[ptr(o) for o in outs], N, Ci, H, W,
                                            scale)
         want = (gi2 - base, gfu, gmu)[which]
         assert np.array_equal(outs[which], want) if which else _rel_err(outs[0], want) < 1e-6
@@ -284,12 +275,12 @@ def _reference_image_warp_concat(im1, im2, flow_q, mask_q, scale=20.0, want_c30=
 
 
 @pytest.mark.gpu
+@pytest.mark.usefixtures("fp64_references")
 def test_cascade_training_step_with_trainable_head(monkeypatch):
     """One MaskFlownet (cascade) training step with the S head trainable: every head parameter gets a finite, non-zero
     gradient through K5's backward, and the loss and all gradients equal the same step with K5 replaced by the torch_ref
     composition up to the criterion of the tensor-core training-step test (a swapped y/x or a missing x20 is O(1))."""
     from maskflownet_b200 import losses, network, ops
-    monkeypatch.setattr(torch.backends.cudnn, "allow_tf32", False)
     torch.manual_seed(3)
     model = network.MaskFlownet().cuda().train()
     g = torch.Generator().manual_seed(5)

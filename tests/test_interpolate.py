@@ -21,11 +21,9 @@ A value within that of a rounding tie (k + 1/2), or a weight sum within dW of 2^
 are excluded and counted; every other value may differ by at most 1.  A hole's blend fmaf(t, I1, fl((1-t) I0)) is computed here exactly as the kernel rounds it, and
 excluded where it lies on the other side of a tie from the exact blend.
 """
-import contextlib
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -35,51 +33,13 @@ from maskflownet_b200 import MaskflowError, _lib, network, ops
 from maskflownet_b200.video import VideoFlowPredictor
 from oracle import interp_ref
 
+from launchcheck.emu import build, ptr
+from launchcheck.inputs import _deterministic
+from launchcheck.interpolate import EXCLUDED_MAX, _check, _mismatch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 TIMES = (1e-3, 0.5, 0.999)
-EXCLUDED_MAX = 1e-3           # share of the compared values that may be excluded as near a rounding tie
-DB, U = 2.0 ** -23, 2.0 ** -24
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# the comparison against the oracle
-# ---------------------------------------------------------------------------------------------------------------
-def _ambiguous(ref, H, W, img0, img1, times):
-    """(N,T,H,W,3) bool: values whose rounding the kernel's arithmetic may decide the other way (module docstring), and
-    the part of them where the hole decision itself may go the other way."""
-    s_w = 61 - int(2 * H * W).bit_length()
-    s_c = s_w - 8
-    Wo, n, wnear = ref["wsum"], ref["count"], ref["wnear"]
-    dW = DB * wnear + 3 * U * Wo + n * 2.0 ** -(s_w + 1)
-    with np.errstate(divide="ignore", invalid="ignore"):
-        E = (255 * (DB * wnear + 4 * U * Wo) + n * 2.0 ** -s_c) / (Wo - dW) + 2.0 ** -16
-    E = np.where(Wo - dW > 0, E, np.inf)[..., None]
-    t = np.asarray(times, np.float32)[None, :, None, None, None]
-    i0, i1 = img0[:, None].astype(np.float32), img1[:, None].astype(np.float32)
-    blend32 = (t.astype(np.float64) * i1 + (np.float32(1) - t) * i0).astype(np.float32)   # the kernel's fmaf, exactly
-    v = ref["value"]
-    hole = ref["hole"][..., None]
-    near_tie = np.where(hole, np.rint(blend32) != np.rint(v), np.abs(v - (np.floor(v) + 0.5)) <= E)
-    near_hole = (np.abs(Wo - interp_ref.HOLE) <= dW)[..., None]
-    return near_tie | near_hole, np.broadcast_to(near_hole, near_tie.shape)
-
-
-def _mismatch(got, ref, img0, img1, times):
-    """(values that differ outside the ambiguous ones, values excluded, values compared, max |got - ref| outside the
-    values whose hole decision is ambiguous: there one side is the blend and the other the splatted colour)."""
-    want = ref["frames"]
-    assert got.shape == want.shape and got.dtype == np.uint8, (got.shape, want.shape, got.dtype)
-    amb, near_hole = _ambiguous(ref, img0.shape[1], img0.shape[2], img0, img1, times)
-    diff = np.abs(got.astype(np.int64) - want)
-    return int(((diff != 0) & ~amb).sum()), int(amb.sum()), amb.size, int(diff[~near_hole].max(initial=0))
-
-
-def _check(got, ref, img0, img1, times, what=""):
-    bad, excl, total, dmax = _mismatch(got, ref, img0, img1, times)
-    assert bad == 0, f"{what}: {bad} values differ from the oracle outside the {excl} ambiguous ones"
-    assert dmax <= 1, f"{what}: max |got - ref| = {dmax}"
-    return excl, total
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -114,17 +74,9 @@ def _case(rng, N, H, W, occ_kind="random"):
     return img0, img1, flows[0], flows[1], occ[0], occ[1]
 
 
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libinterp_emu.so")
-    src = os.path.join(HERE, "host_emu", "interp_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out,
-                    src], check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "interp_emu")
     L.emu_interpolate_frames.argtypes = [ctypes.c_void_p] * 7 + [ctypes.c_int] * 3 + [ctypes.c_void_p, ctypes.c_int,
                                                                                      ctypes.c_float] + [ctypes.c_void_p] * 2
     L.emu_interp_weight_shift.argtypes = [ctypes.c_int, ctypes.c_int]
@@ -137,8 +89,8 @@ def _emu_run(emu, img0, img1, ffw, fbw, ofw, obw, times, ow=0.01, order=None, wa
     ts = np.asarray(times, np.float32)
     out = np.full((N, len(ts), H, W, 3), 7, np.uint8)
     acc = np.zeros((N, H, W, 4), np.int64) if want_acc else None
-    emu.emu_interpolate_frames(*(_ptr(v) for v in a), _ptr(out), N, H, W, _ptr(ts), len(ts), ow,
-                               None if order is None else _ptr(order), None if acc is None else _ptr(acc))
+    emu.emu_interpolate_frames(*(ptr(v) for v in a), ptr(out), N, H, W, ptr(ts), len(ts), ow,
+                               None if order is None else ptr(order), None if acc is None else ptr(acc))
     return (out, acc) if want_acc else out
 
 
@@ -485,16 +437,6 @@ def test_synthetic_scene_from_the_kernel():
 # ---------------------------------------------------------------------------------------------------------------
 # GPU: the network and the video predictor
 # ---------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
 def _model(cls):
     torch.manual_seed(7)
     return cls().cuda().eval()

@@ -10,11 +10,9 @@ VideoMotionSegmenter bit for bit against network.segment_motion, bf16 and the co
 Tolerances.  Labels, count, dropped, area, box, centroid and peak are exact.  dx, dy are 64-bit fixed point at scale 2^S
 (include/maskflow_b200.h): within 2^-(S+1) + 2^-50 (1 + |mean|) of the oracle's exact mean, NaN in the same places.
 """
-import contextlib
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -26,38 +24,13 @@ from maskflownet_b200.video import MotionFrame, VideoFlowPredictor, VideoMotionS
 from oracle import motionseg_ref as R
 from oracle import stabilize_ref as SR
 
+from launchcheck.emu import build
+from launchcheck.inputs import _deterministic
+from launchcheck.motion_segment import _check, _mismatch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 EIGHT = np.ones((3, 3), int)
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# comparisons against the oracle
-# ---------------------------------------------------------------------------------------------------------------
-def _mismatch(got, ref, H, W):
-    """A description of the first difference between two results (labels, objects, count, dropped), or None."""
-    (gl, go, gc, gd), (rl, ro, rc, rd) = got, ref
-    gl, go, gc, gd = (np.asarray(v) for v in (gl, go, gc, gd))
-    if not np.array_equal(gc, rc) or not np.array_equal(gd, rd):
-        return f"count {gc} != {rc} or dropped {gd} != {rd}"
-    bad = np.flatnonzero((gl != rl).reshape(len(gl), -1).any(1))
-    if len(bad):
-        return f"labels differ in frames {bad.tolist()}: {int((gl != rl).sum())} pixels"
-    if not np.array_equal(go[..., :8], ro[..., :8]):
-        return f"area/box/centroid/peak differ by {np.abs(go[..., :8] - ro[..., :8]).max()}"
-    gn, rn = np.isnan(go[..., 8:]), np.isnan(ro[..., 8:])
-    if not np.array_equal(gn, rn):
-        return "dx/dy NaN pattern differs"
-    tol = 2.0 ** -(R.scale_bits(H, W) + 1) + 2.0 ** -50 * (1 + np.abs(np.nan_to_num(ro[..., 8:])))
-    err = np.abs(np.nan_to_num(go[..., 8:]) - np.nan_to_num(ro[..., 8:]))
-    if (err > tol).any():
-        return f"dx/dy differ by {err.max()} > {tol.max()}"
-    return None
-
-
-def _check(got, ref, H, W, what=""):
-    m = _mismatch(got, ref, H, W)
-    assert m is None, f"{what}: {m}"
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -248,11 +221,7 @@ def _ptr(a):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libmotionseg_emu.so")
-    src = os.path.join(HERE, "host_emu", "motionseg_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out,
-                    src], check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "motionseg_emu")
     v, i = ctypes.c_void_p, ctypes.c_int
     L.emu_motion_segment.argtypes = [v] * 10 + [i] * 3 + [ctypes.c_float] * 2 + [i, i, ctypes.c_ulonglong]
     L.emu_union_find.argtypes = [v, v, i, i, i, ctypes.c_ulonglong]
@@ -606,16 +575,6 @@ def test_ops_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------
 # GPU: the network and the video segmenter
 # ---------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
 def _model(cls):
     torch.manual_seed(7)
     return cls().cuda().eval()

@@ -1,42 +1,26 @@
 """GPU tests of the product model graph: against the golden fixture from the reference's own graph, against the oracle
 network on fresh inputs, the cascade, a training step, and the reference's operator call style through the mx shim."""
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("fp64_references")]
 
 from maskflownet_b200 import _lib, mx, network, ops  # noqa: E402
 from oracle import network_ref  # noqa: E402
 
+from launchcheck import fp64_references  # noqa: E402,F401
+from launchcheck.inputs import _named_model, seeded_images  # noqa: E402
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(ROOT, "tests", "golden")
-sys.path.insert(0, G)
-from make_golden import named_init, seeded_images  # noqa: E402
-
-
-@pytest.fixture(autouse=True)
-def _fp32():
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-
-
-def _named_model(cls=network.MaskFlownetS):
-    m = cls()
-    with torch.no_grad():
-        for k, p in m.named_parameters():
-            p.copy_(named_init(k.replace("MaskFlownet_S.", ""), p.shape) if cls is network.MaskFlownetS
-                    else named_init(k, p.shape))
-    return m.cuda().eval()
 
 
 def test_product_graph_matches_reference_graph_fixture():
     d = np.load(os.path.join(G, "net_ref_graph.npz"))
-    model = _named_model()
+    model = _named_model(network.MaskFlownetS).eval()
     im1, im2 = seeded_images()
     n0 = _lib.launch_count()
     with torch.no_grad():
@@ -51,7 +35,7 @@ def test_product_graph_matches_reference_graph_fixture():
 
 
 def test_product_graph_matches_oracle_network_batch2():
-    model = _named_model()
+    model = _named_model(network.MaskFlownetS).eval()
     a1, a2 = seeded_images(seed=5, n=2, h=64, w=192)
     params = {k: v.detach().cpu() for k, v in model.named_parameters()}
     with torch.no_grad():
@@ -62,7 +46,7 @@ def test_product_graph_matches_oracle_network_batch2():
 
 
 def test_predict_flow_pipeline():
-    model = _named_model()
+    model = _named_model(network.MaskFlownetS).eval()
     rng = np.random.default_rng(0)
     u1 = torch.from_numpy(rng.integers(0, 256, (1, 3, 64, 128), dtype=np.uint8))
     u2 = torch.from_numpy(rng.integers(0, 256, (1, 3, 64, 128), dtype=np.uint8))
@@ -78,7 +62,7 @@ def test_cascade_matches_reference_graph_fixture():
     through the shim with the oracle's operators (tests/golden/net_ref_graph_cascade.npz): pins the dual pyramid, the md=2
     correlations, deform6 and the c2s quirk (:306).  Bound: 1e-4 relative to the flow scale (x20) = 2e-3 px."""
     d = np.load(os.path.join(G, "net_ref_graph_cascade.npz"))
-    model = _named_model(network.MaskFlownet)
+    model = _named_model(network.MaskFlownet).eval()
     assert sum(p.numel() for p in model.parameters()) == int(d["n_params"])
     im1, im2 = seeded_images()
     with torch.no_grad():
@@ -92,7 +76,7 @@ def test_cascade_matches_reference_graph_fixture():
 
 
 def test_cascade_matches_oracle_network_fresh_inputs():
-    model = _named_model(network.MaskFlownet)
+    model = _named_model(network.MaskFlownet).eval()
     a1, a2 = seeded_images(seed=11, n=2, h=64, w=128)
     params = {k: v.detach().cpu() for k, v in model.named_parameters()}
     with torch.no_grad():
@@ -114,7 +98,7 @@ def test_cascade_forward_runs_and_uses_md2_kernels():
 
 
 def test_training_step_gradients_flow_through_cuda_backward():
-    model = _named_model().train()
+    model = _named_model(network.MaskFlownetS).train()
     a1, a2 = seeded_images(seed=9, n=2, h=64, w=128)
     preds = model(a1.cuda(), a2.cuda())[0]
     loss = sum(w * p.square().mean() for w, p in zip((.005, .01, .02, .08, .32), preds))
@@ -188,7 +172,7 @@ def test_predict_any_size_matches_oracle_pipeline():
     """network.predict (PipelineFlownet.predict: resize to x64, forward, Upsample(4), resize back, flip) on a 50x100 pair
     against the oracle network + oracle pre/post-processing."""
     from oracle import prepost_ref
-    model = _named_model()
+    model = _named_model(network.MaskFlownetS).eval()
     rng = np.random.default_rng(3)
     u1 = rng.integers(0, 256, (1, 3, 50, 100), dtype=np.uint8)
     u2 = rng.integers(0, 256, (1, 3, 50, 100), dtype=np.uint8)
@@ -207,7 +191,7 @@ def test_predict_any_size_matches_oracle_pipeline():
 def test_fused_heads_equal_separate_heads(cls):
     """fuse_heads (pred_flow / pred_mask partial sums computed by conv{L}_4's launch through the linear-prefix epilogue, plus a
     32-channel tail convolution) == the separate 3-output head convolution over the whole block output."""
-    model = _named_model(cls)
+    model = _named_model(cls).eval()
     a1, a2 = seeded_images(seed=13, n=2, h=64, w=128)
     with torch.no_grad():
         model.fuse_heads = True

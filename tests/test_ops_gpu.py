@@ -11,6 +11,8 @@ pytestmark = pytest.mark.gpu
 
 from maskflownet_b200 import ops, _lib  # noqa: E402
 
+from launchcheck import tf32  # noqa: E402
+
 DEV = "cuda"
 
 
@@ -384,10 +386,9 @@ def test_conv3x3_tensor_core_matches_fp32(N, Cin, Cout, H, W):
     scale = max(1.0, float(np.abs(ref).max()))
     assert np.abs(got - ref).max() <= 1e-4 * scale, np.abs(got - ref).max()
     # for context: error of a TF32 convolution (what "allow_tf32" would do) is two orders of magnitude larger
-    torch.backends.cudnn.allow_tf32 = True
-    tf32 = torch.nn.functional.leaky_relu(torch.nn.functional.conv2d(cu(x), cu(w), cu(b), padding=1), 0.1).cpu().numpy()
-    torch.backends.cudnn.allow_tf32 = False
-    assert np.abs(got - ref).max() <= max(0.5 * np.abs(tf32 - ref).max(), 2e-5 * scale)
+    with tf32(True):
+        got_tf32 = torch.nn.functional.leaky_relu(torch.nn.functional.conv2d(cu(x), cu(w), cu(b), padding=1), 0.1)
+    assert np.abs(got - ref).max() <= max(0.5 * np.abs(got_tf32.cpu().numpy() - ref).max(), 2e-5 * scale)
 
 
 @pytest.mark.parametrize("dil", [2, 4, 8, 16])

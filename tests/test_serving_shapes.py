@@ -11,7 +11,7 @@ tools/predict_new_data.py run other shapes -- one pair at a time, KITTI frames (
   * the 1x1 correlation has every displacement but the centre outside the image, and the dilation-16 context layer on
     a 16x16 level 2 has every off-centre tap outside: its TMA boxes lie wholly out of bounds.
 test_split_plans_of_the_serving_shapes pins those plans on the CPU (mfn_conv3x3_workspace_bytes is host arithmetic).
-test_every_launch_of_a_serving_forward_against_float64 runs five forwards through the recorder of test_bench_shapes.py,
+test_every_launch_of_a_serving_forward_against_float64 runs five forwards through launchcheck's ServingRecorder,
 with its bound and controls, and asserts that each run reached the path it is there for.  Controls added here, each to
 be rejected by CONTROL_MARGIN: replicate padding instead of zero padding (the dilation-16 layer, the 1x1 correlation:
 an out-of-bounds box that read the image), the last 16-channel chunk dropped on a split-every-tile launch (a lost
@@ -26,19 +26,19 @@ writing it shows up as a non-finite or different flow.
 
 Not checked here: the backward at these shapes, frames larger than 1088x1920.
 """
-import contextlib
 import time
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as tF
 
-from maskflownet_b200 import _lib, network, ops
-from oracle import torch_ref
-from test_bench_shapes import (CONTROL_MARGIN, EPS_Q, EPS_S, Recorder, _expected_convs, _images_u8, _named_model,
-                               _warp_conv, activate, channel_slopes, conv_terms, judge, split_storage_term)
-from make_golden import named_init  # noqa: E402  (tests/golden, on the path test_bench_shapes sets)
+from maskflownet_b200 import _lib, network
+
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.bounds import (CONTROL_MARGIN, EPS_Q, EPS_S, _expected_convs, channel_slopes, conv_terms, judge,
+                                split_storage_term)
+from launchcheck.inputs import _deterministic, _images_u8, _named_model, _same, named_init
+from launchcheck.recorders import Recorder, ServingRecorder, _cover_tiny, _cover_tiny_cascade
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -112,189 +112,8 @@ def test_split_output_storage_term_covers_a_bias_dominated_output():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# GPU: the recorder with this file's controls
-# ------------------------------------------------------------------------------------------------------------------
-def _corr_replicate(f1, f2, md):
-    """torch_ref.correlation with f2 padded by replicating its border instead of by zeros (a near miss)."""
-    H, W = f1.shape[2:]
-    p = tF.pad(f2, (md,) * 4, mode="replicate")
-    return torch.stack([(f1 * p[:, :, md + dy:md + dy + H, md + dx:md + dx + W]).sum(dim=1) / f1.shape[1]
-                        for dy in range(-md, md + 1) for dx in range(-md, md + 1)], dim=1)
-
-
-def _row(op, name, kernel, shape, ratio, **kw):
-    N, C, H, W = shape
-    r = dict(op=op, name=name, kernel=kernel, N=N, Cin=C, Cout=C, H=H, W=W, dil=0, stride=1, ws=0, err_q=0.0,
-             ratio=ratio, tags=[], split_out=False, split_all=False)
-    r.update(kw)
-    return r
-
-
-class ServingRecorder(Recorder):
-    """test_bench_shapes.Recorder plus: where each launch's split-K plan splits every tile, the controls of this file
-    (self.extra: tag -> (layer, err/bound)) and the warp_mma_kernel controls (in self.controls, the base's format), and
-    ops.preprocess / ops.postprocess against oracle/prepost_ref."""
-
-    def __init__(self, monkeypatch, run):
-        super().__init__(monkeypatch, run)
-        self.extra = {}
-        for name in ("preprocess", "postprocess"):
-            self.orig[name] = getattr(ops, name)
-            monkeypatch.setattr(ops, name, getattr(self, name))
-
-    # ---- convolutions ---------------------------------------------------------------------------------------------
-    def _check_conv(self, op, packed, bias, Cout, slope, dil, stride, d2s, lp, x_of, got_of, N, Cin, H, W, ws, kern,
-                    tags, store_from=None):
-        OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
-        # the base controls drop tap (0, 0): they say something only where that tap reads inside the image for some
-        # output pixel, so launches where it never does (1x1 levels) leave them to a later launch of the same kind
-        reach = (OH - 1) * stride >= dil and (OW - 1) * stride >= dil
-        super()._check_conv(op, packed, bias, Cout, slope, dil, stride, d2s, lp, x_of, got_of, N, Cin, H, W, ws, kern,
-                            tags if reach else [], store_from)
-        row = self.rows[-1]
-        row["tags"], row["split_out"] = tags, "split" in tags
-        row["split_all"] = ws > 0 and ws % (4 * N * Cout * OH * OW) == 0     # the workspace holds k whole outputs
-        want = []
-        # (on an image wider and taller than 4 px: below that the correlation's last channels, the last chunk of the
-        # first dense-block layer, lie wholly outside and are zero)
-        if op == "conv3x3_split" and row["split_all"] and not d2s and Cin > 16 and min(H, W) > 4 and \
-                "chunk" not in self.extra:
-            want.append("chunk")
-        if not d2s and dil > 1 and dil >= max(H, W) and "pad" not in self.extra:
-            want.append("pad")
-        if want:
-            self._conv_controls(want, packed, bias, Cout, slope, dil, stride, lp, x_of(0), store_from)
-
-    def _conv_controls(self, tags, packed, bias, Cout, slope, dil, stride, lp, x, store_from):
-        w = self.packs[packed.data_ptr()][0].double()
-        b = bias.detach().double().view(1, -1, 1, 1) if bias is not None else None
-        name = self.names.get(packed.data_ptr(), "?")
-        sl = channel_slopes(Cout, slope, lp, w.device)
-        with torch.no_grad():
-            pre, Q, S = conv_terms(x, w, b.view(-1) if b is not None else None, stride, dil)
-            bound = EPS_Q * Q + EPS_S * S + split_storage_term(pre, store_from)
-            for tag in tags:
-                if tag == "chunk":      # the input channels of the last 16-channel chunk dropped
-                    wd = w.clone()
-                    wd[:, (w.shape[1] - 1) // 16 * 16:] = 0
-                    alt = tF.conv2d(x, wd, stride=stride, padding=dil, dilation=dil)
-                else:                   # the padding replicates the border instead of reading zeros
-                    alt = tF.conv2d(tF.pad(x, (dil,) * 4, mode="replicate"), w, stride=stride, dilation=dil)
-                if b is not None:
-                    alt = alt + b
-                self.extra[tag] = (name, judge(activate(alt, sl), pre, sl, bound, Q)[0])
-
-    # ---- correlation: replicate padding at 1x1 --------------------------------------------------------------------
-    def correlation(self, *args, **kw):
-        res = super().correlation(*args, **kw)
-        a = self._bind("correlation", args, kw)
-        d1, d2, md, slope = a["data1"], a["data2"], a["max_displacement"], a["leaky_slope"]
-        N, C, H, W = d1.shape
-        if (H, W) == (1, 1) and "corr_pad" not in self.extra:
-            with torch.no_grad():
-                f1, f2 = d1[:1].detach().double(), d2[:1].detach().double()
-                pre = torch_ref.correlation(f1, f2, md)
-                Q = (torch_ref.correlation(f1 * f1, f2 * f2, md) * C).sqrt() / C
-                S = torch_ref.correlation(f1.abs(), f2.abs(), md)
-                sl = channel_slopes(pre.shape[1], slope, 0, d1.device)
-                r = judge(activate(_corr_replicate(f1, f2, md), sl), pre, sl, EPS_Q * Q + EPS_S * S, Q)[0]
-            self.extra["corr_pad"] = (f"correlation md={md} C={C} 1x1", r)
-        return res
-
-    # ---- warp: the warp_mma_kernel controls -----------------------------------------------------------------------
-    def warp_mask(self, *args, **kw):
-        res = super().warp_mask(*args, **kw)
-        if self.rows[-1]["kernel"].startswith("warp_mma_kernel") and "warp_mma" not in self.controls:
-            a = self._bind("warp_mask", args, kw)
-            _, fup, mup = res
-            x, fc, mc, w, b, t = (a[k] for k in ("x", "flow_coarse", "mask_coarse", "weight", "bias", "tradeoff"))
-            scale, stride, border = a["scale"], a["stride"], a["border_mode"]
-            with torch.no_grad():
-                xn, fn, wd = x[:1].detach().double(), fup[:1].detach(), w.detach().double()
-                sig = torch.sigmoid(mup[:1].detach().double()) if mc is not None else 1.0
-                bb = b.detach().double().view(1, -1, 1, 1) if b is not None else 0.0
-                tn = t[:1].detach().double() if t is not None else 0.0
-
-                def pre_of(xx, ww):
-                    return (_warp_conv(xx, fn, ww, scale, stride, border) + bb) * sig + tn
-                pre = pre_of(xn, wd)
-                Q = _warp_conv(xn * xn, fn, wd * wd, scale, stride, border).sqrt() * sig
-                S = (_warp_conv(xn.abs(), fn, wd.abs(), scale, stride, border) +
-                     (b.detach().double().abs().view(1, -1, 1, 1) if b is not None else 0.0)) * sig
-                S = S + (tn.abs() if t is not None else 0.0)
-                bound = EPS_Q * Q + EPS_S * S
-                sl = channel_slopes(w.shape[0], a["leaky_slope"], 0, x.device)
-                bf = lambda v: v.to(torch.bfloat16).double()  # noqa: E731
-                w_drop = wd.clone()
-                w_drop[:, :, 1, 1] = 0      # the centre tap: at 2x2 the corner taps may all fall outside
-                self.controls["warp_mma"] = (
-                    f"warp_mask {x.shape[2]}x{x.shape[3]} F={w.shape[0]}",
-                    {"bf16": judge(activate(pre_of(bf(xn), bf(wd)), sl), pre, sl, bound, Q)[0],
-                     "tap": judge(activate(pre_of(xn, w_drop), sl), pre, sl, bound, Q)[0]})
-        return res
-
-    # ---- pre / post-processing against the oracle (tolerances of test_ops_gpu's oracle test) ----------------------
-    def preprocess(self, img1, img2, out_hw=None):
-        from oracle import prepost_ref
-        res = self.orig["preprocess"](img1, img2, out_hw)
-        torch.cuda.synchronize()
-        kern = _lib.last_kernel()
-        ra, rb, rm = prepost_ref.preprocess(img1.cpu().numpy(), img2.cpu().numpy(), out_hw)
-        o1, o2, m = (t.cpu().numpy() for t in res)
-        r = max(np.abs(m - rm).max() / 2e-6, np.abs(o1 - ra).max() / 1e-5, np.abs(o2 - rb).max() / 1e-5)
-        if r > 1.0:
-            self._fail(f"preprocess {tuple(img1.shape)} -> {out_hw}: err/tolerance {r:.3g}")
-        self.rows.append(_row("preprocess", f"-> {o1.shape[2]}x{o1.shape[3]}", kern, tuple(img1.shape), float(r)))
-        return res
-
-    def postprocess(self, pred, H, W, flip_channels=True, is_flow=True):
-        from oracle import prepost_ref
-        res = self.orig["postprocess"](pred, H, W, flip_channels, is_flow)
-        torch.cuda.synchronize()
-        kern = _lib.last_kernel()
-        ref = prepost_ref.postprocess(pred.detach().cpu().numpy(), H, W, flip_channels, is_flow)
-        r = float(np.abs(res.cpu().numpy() - ref).max()) / (1e-4 if is_flow else 1e-5)
-        if r > 1.0:
-            self._fail(f"postprocess {tuple(pred.shape)} -> {H}x{W} (flow {is_flow}): err/tolerance {r:.3g}")
-        self.rows.append(_row("postprocess", "flow" if is_flow else "mask", kern, tuple(pred.shape), r, H=H, W=W))
-        return res
-
-    def report(self):
-        super().report()
-        for tag, (name, r) in sorted(self.extra.items()):
-            print(f"{self.run:8s} control {tag:8s} on {name}: err/bound={r:.3g}")
-        worst = {}
-        for r in self.rows:
-            key = (r["op"], r["kernel"].split("<")[0])
-            worst[key] = max(worst.get(key, 0.0), r["ratio"])
-        for (op, kern), v in sorted(worst.items()):
-            print(f"{self.run:8s} worst {op:17s} {kern:30s} err/bound={v:.3f}")
-
-
-# ------------------------------------------------------------------------------------------------------------------
 # GPU: the five serving forwards
 # ------------------------------------------------------------------------------------------------------------------
-def _cover_tiny(rec, convs):
-    warps = {(r["H"], r["W"], r["kernel"]) for r in rec.rows if r["op"] == "warp_mask"}
-    assert (2, 2, "warp_mma_kernel") in warps, warps                      # level 5
-    assert (4, 4, "warp_lin_kernel") in warps, warps                      # level 4, the through-linearity minimum
-    corr = {(r["H"], r["Cin"]): r["kernel"] for r in rec.rows if r["op"] == "correlation"}
-    assert (1, 196) in corr and (2, 128) in corr, corr
-    assert {c for (_, c), k in corr.items() if k.startswith("corr_rb_kernel")} == {196, 128, 96, 64}, corr
-    assert any(r["op"] == "conv3x3_split" and r["dil"] == 16 and (r["H"], r["W"]) == (16, 16) for r in convs)
-    split_levels = {r["H"] for r in convs if r["op"] == "conv3x3_split" and r["split_all"]}
-    assert {1, 2, 4, 8, 16} <= split_levels, split_levels                 # a reduce launch at every decoder level
-    assert {"chunk", "pad", "corr_pad"} <= set(rec.extra) and "warp_mma" in rec.controls
-
-
-def _cover_tiny_cascade(rec, convs):
-    assert any(r["op"] == "warp_mask" and r["kernel"].startswith("deform_fwd_kernel") and r["Cout"] == 196 and
-               (r["H"], r["W"]) == (1, 1) for r in rec.rows)
-    assert any(r["op"] == "correlation" and r["name"] == "md=2" and (r["H"], r["W"]) == (1, 1) for r in rec.rows)
-    assert any(r["op"] == "image_warp_concat" and (r["H"], r["W"]) == (64, 64) for r in rec.rows)
-    assert "warp_mma" in rec.controls and "corr_pad" in rec.extra
-
-
 def _cover_single(rec, convs):
     for h in (56, 28):      # levels 3 and 4
         split = [r for r in convs if r["op"] == "conv3x3_split" and r["H"] == h and r["ws"] > 0]
@@ -340,9 +159,8 @@ SERVING = {   # run: (model class, batch, input H, W, image seed, through networ
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", list(SERVING))
+@pytest.mark.usefixtures("fp64_references")
 def test_every_launch_of_a_serving_forward_against_float64(run, monkeypatch):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     cls, N, H, W, seed, via_predict, cover = SERVING[run]
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
@@ -377,23 +195,6 @@ def test_every_launch_of_a_serving_forward_against_float64(run, monkeypatch):
 # ------------------------------------------------------------------------------------------------------------------
 # GPU: the serving paths against eager, bit for bit
 # ------------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
-def _same(got, ref, what):
-    assert bool(torch.isfinite(ref).all()), f"{what}: the eager flow is not finite"
-    d = (got.float() - ref.float()).abs()
-    assert torch.equal(got, ref), f"{what}: max |diff| {float(d.nan_to_num(float('inf')).max()):.3g} at " \
-                                  f"{np.unravel_index(int(d.nan_to_num(float('inf')).argmax()), tuple(d.shape))}"
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("arch,N,conv,deform", [("S", 8, "conv5_1", "deform4"), ("cascade", 4, "conv4_1", "deform3")])
 def test_flow_predictor_graph_equals_eager_at_the_benchmark_shape(arch, N, conv, deform):

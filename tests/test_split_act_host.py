@@ -3,22 +3,16 @@ numpy restatement of the format: for every fp32 value v, hi = bf16 round-to-near
 (N, 2, Cg, H, W, 8) bf16 with zero pad channels; partial 8- and 16-channel groups, NaN / inf / overflow, a slice that
 starts inside a larger buffer and a batch stride wider than the tensor.  No GPU."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+from launchcheck.emu import build
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libsplit_act_emu.so")
-    src = os.path.join(HERE, "host_emu", "split_act_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "split_act_emu")
     L.emu_split_pack.argtypes = [ctypes.c_void_p, ctypes.c_longlong] + [ctypes.c_int] * 4 + [ctypes.c_void_p] + \
         [ctypes.c_int] * 2
     L.emu_split_pack.restype = None

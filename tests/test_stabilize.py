@@ -13,11 +13,9 @@ within 1e-5 px plus one float32 ulp of the value, NaN in the same places.  The w
 the same order; the kernel's fused multiply-adds may move a value across a rounding tie, so values may differ by 1, and at
 least 99.9 % must be exact.
 """
-import contextlib
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -27,44 +25,12 @@ from maskflownet_b200 import MaskflowError, _lib, camera, network, ops
 from maskflownet_b200.video import VideoFlowPredictor, VideoStabilizer
 from oracle import stabilize_ref as R
 
+from launchcheck.emu import build, ptr
+from launchcheck.inputs import _deterministic
+from launchcheck.stabilize import CORNER_TOL, WARP_EXACT, _check_fit, _check_warp, _fit_mismatch, _warp_mismatch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-CORNER_TOL, RES_TOL, WARP_EXACT = 1e-6, 1e-5, 0.999
-
-
-# ---------------------------------------------------------------------------------------------------------------
-# comparisons against the oracle
-# ---------------------------------------------------------------------------------------------------------------
-def _fit_mismatch(got, ref, H, W):
-    """(max corner distance in px, ok flags differ, residual values outside tolerance or NaN pattern differs)."""
-    (ga, gok, gres), (ra, rok, rres) = got, ref
-    d = float(np.abs(R.corners(ga, H, W) - R.corners(ra, H, W)).max(initial=0.0))
-    okbad = not np.array_equal(np.asarray(gok, bool), np.asarray(rok, bool))
-    resbad = 0
-    if gres is not None:
-        gn, rn = np.isnan(gres), np.isnan(rres)
-        tol = RES_TOL + np.spacing(np.abs(np.nan_to_num(rres)).astype(np.float32))
-        resbad = int((gn != rn).sum() + ((np.abs(np.nan_to_num(gres) - np.nan_to_num(rres)) > tol) & ~gn & ~rn).sum())
-    return d, okbad, resbad
-
-
-def _check_fit(got, ref, H, W, what=""):
-    d, okbad, resbad = _fit_mismatch(got, ref, H, W)
-    assert not okbad, f"{what}: ok {got[1]} != {ref[1]}"
-    assert d <= CORNER_TOL, f"{what}: corners differ by {d} px"
-    assert resbad == 0, f"{what}: {resbad} residual values differ"
-    return d
-
-
-def _warp_mismatch(got, ref):
-    diff = np.abs(got.astype(np.int64) - ref)
-    return int(diff.max(initial=0)), float((diff == 0).mean()) if diff.size else 1.0
-
-
-def _check_warp(got, ref, what=""):
-    dmax, exact = _warp_mismatch(got, ref)
-    assert dmax <= 1 and exact >= WARP_EXACT, f"{what}: max |diff| {dmax}, exact {exact:.5f}"
-    return exact
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -118,17 +84,9 @@ HOST_SHAPES = [(2, 37, 53), (1, 1, 40), (1, 40, 1), (2, 64, 96), (1, 3, 3)]
 # ---------------------------------------------------------------------------------------------------------------
 # the host build
 # ---------------------------------------------------------------------------------------------------------------
-def _ptr(a):
-    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libstabilize_emu.so")
-    src = os.path.join(HERE, "host_emu", "stabilize_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out,
-                    src], check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "stabilize_emu")
     v, i = ctypes.c_void_p, ctypes.c_int
     L.emu_affine_motion.argtypes = [v] * 4 + [i] * 4 + [ctypes.c_float]
     L.emu_warp_frames_affine.argtypes = [v] * 3 + [i] * 3
@@ -143,14 +101,14 @@ def _host_ops(L):
         A = np.zeros((N, 2, 3))
         ok = np.zeros(N, np.uint8)
         res = np.zeros((N, H, W), np.float32)
-        L.emu_affine_motion(_ptr(flow), _ptr(A), _ptr(ok), _ptr(res), N, H, W, iterations, sigma)
+        L.emu_affine_motion(ptr(flow), ptr(A), ptr(ok), ptr(res), N, H, W, iterations, sigma)
         return A, ok.astype(bool), res
 
     def warp(src, M):
         src = np.ascontiguousarray(src, np.uint8)
         M = np.ascontiguousarray(M, np.float64)
         out = np.zeros_like(src)
-        L.emu_warp_frames_affine(_ptr(src), _ptr(M), _ptr(out), *src.shape[:3])
+        L.emu_warp_frames_affine(ptr(src), ptr(M), ptr(out), *src.shape[:3])
         return out
 
     return fit, warp
@@ -597,16 +555,6 @@ def test_ops_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------
 # GPU: the network and the video stabiliser
 # ---------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
 def _model(cls):
     torch.manual_seed(7)
     return cls().cuda().eval()

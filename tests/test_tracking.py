@@ -13,11 +13,9 @@ is excluded and counted; at most EXCLUDED_MAX of the compared slots may be.  Eve
 TRACKED position must lie within its bound of the oracle's.  The seeding starts from the kernel's own state after the
 advance, so its births and dropped counts are compared exactly.
 """
-import contextlib
 import ctypes
 import importlib.util
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -27,26 +25,20 @@ from maskflownet_b200 import MaskflowError, _lib, network, ops
 from maskflownet_b200.video import TrackFrame, VideoTracker, collect_tracks, track_frames
 from oracle import track_ref as R
 
+from launchcheck.emu import build, ptr
+from launchcheck.inputs import _deterministic
+from launchcheck.tracking import CONSTS, Tally, _compare_advance, _compare_seed
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-EXCLUDED_MAX = 1e-3
-CONSTS = dict(alpha=0.01, beta=0.5, boundary=(0.01, 0.002))
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # the host build
 # ---------------------------------------------------------------------------------------------------------------
-def _ptr(a):
-    return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libtrack_emu.so")
-    src = os.path.join(HERE, "host_emu", "track_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out,
-                    src], check=True)
-    L = ctypes.CDLL(out)
+    L = build(tmp_path_factory, "track_emu")
     v, i, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
     L.emu_track_texture.argtypes = [v, v, v, i, i, i, i]
     L.emu_track_advance.argtypes = [v] * 5 + [i] * 4 + [f] * 4
@@ -74,18 +66,18 @@ class HostTracker:
     def texture(self, frame):
         lam = np.zeros((1, self.Gy, self.Gx))
         lmax = np.zeros(1)
-        self.L.emu_track_texture(_ptr(np.ascontiguousarray(frame[None])), _ptr(lam), _ptr(lmax), 1, self.H, self.W, self.h)
+        self.L.emu_track_texture(ptr(np.ascontiguousarray(frame[None])), ptr(lam), ptr(lmax), 1, self.H, self.W, self.h)
         return lam[0], lmax
 
     def advance(self, ffw, fbw):
         ab, bb = self.boundary
-        self.L.emu_track_advance(_ptr(np.ascontiguousarray(ffw)), _ptr(np.ascontiguousarray(fbw)), _ptr(self.pos),
-                                 _ptr(self.status), _ptr(self.cells), self.K, self.H, self.W, self.h, self.alpha,
+        self.L.emu_track_advance(ptr(np.ascontiguousarray(ffw)), ptr(np.ascontiguousarray(fbw)), ptr(self.pos),
+                                 ptr(self.status), ptr(self.cells), self.K, self.H, self.W, self.h, self.alpha,
                                  self.beta, ab, bb)
 
     def seed(self, lam, lmax):
-        self.L.emu_track_seed(_ptr(np.ascontiguousarray(lam)), _ptr(lmax), _ptr(self.q) if self.M else None, self.M,
-                              _ptr(self.pos), _ptr(self.status), _ptr(self.cells), _ptr(self.frame), _ptr(self.dropped),
+        self.L.emu_track_seed(ptr(np.ascontiguousarray(lam)), ptr(lmax), ptr(self.q) if self.M else None, self.M,
+                              ptr(self.pos), ptr(self.status), ptr(self.cells), ptr(self.frame), ptr(self.dropped),
                               self.K, self.H, self.W, self.h, self.tau)
         return self.pos.copy(), self.status.copy(), int(self.dropped[0])
 
@@ -130,39 +122,6 @@ def _texture_np(tr, frame):
 # ---------------------------------------------------------------------------------------------------------------
 # the comparison against the oracle, one frame at a time from the kernel's own previous state
 # ---------------------------------------------------------------------------------------------------------------
-class Tally:
-    def __init__(self):
-        self.excluded = self.compared = 0
-
-    def check(self):
-        print(f"excluded {self.excluded} of {self.compared} slot decisions")
-        assert self.excluded <= EXCLUDED_MAX * max(self.compared, 1), (self.excluded, self.compared)
-
-
-def _compare_advance(prev_pos, prev_status, adv_pos, adv_status, ffw, fbw, tally, control=None, what=""):
-    """Mismatching slots outside the exclusions (0 for the kernel against its own rule)."""
-    ref = R.advance(prev_pos, prev_status, ffw, fbw, **CONSTS, control=control)
-    live = (prev_status == R.TRACKED) | (prev_status == R.BORN)
-    amb = ref["amb"]
-    bad = (adv_status != ref["status"]) & ~amb
-    both = (adv_status == R.TRACKED) & (ref["status"] == R.TRACKED)
-    dev = np.abs(adv_pos.astype(np.float64) - ref["pos"]).max(-1)
-    bad |= both & ~(dev <= ref["eq"])
-    bad |= ~both & (adv_status != R.TRACKED) & ~np.all(np.isnan(adv_pos), -1)
-    if tally is not None:
-        tally.excluded += int((amb & live).sum())
-        tally.compared += int(live.sum())
-    return int(bad.sum())
-
-
-def _compare_seed(adv_pos, adv_status, lam, lmax, q, k, h, tau, H, W, xy, st, dropped, control=None):
-    """Mismatching slots and dropped counts of the seeding of frame k against the oracle from the state after the advance
-    (exact: no exclusion)."""
-    rp, rs, rd = R.seed(adv_pos, adv_status, lam, lmax, q, k, h, tau, H, W, control)
-    same = (rs == st) & ((rp == xy) | (np.isnan(rp) & np.isnan(xy))).all(-1)
-    return int((~same).sum()) + int(rd != dropped)
-
-
 def _run_chain(tr, frames, ffw, fbw, tally=None, control=None):
     """Runs a tracker over the frames; checks every advance (with exclusions) and every seeding (exact) against the
     oracle from the tracker's previous state.  Returns (xy (T,K,2), status (T,K), dropped (T,), mismatches)."""
@@ -698,16 +657,6 @@ def test_ops_argument_errors():
 # ---------------------------------------------------------------------------------------------------------------
 # GPU: the network and the video tracker
 # ---------------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def _deterministic():
-    prev, prev_warn = torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled()
-    torch.use_deterministic_algorithms(True)
-    try:
-        yield
-    finally:
-        torch.use_deterministic_algorithms(prev, warn_only=prev_warn)
-
-
 def _model(cls):
     torch.manual_seed(7)
     return cls().cuda().eval()

@@ -9,7 +9,6 @@ against the oracle.
 """
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -17,18 +16,17 @@ import torch
 
 from oracle import augment_ref
 
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.emu import build, ptr
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 FIX = os.path.join(HERE, "golden", "aug_ref_graph.npz")
 GEO_NAMES = ["rotation", "aspect_ratio", "scale", "tx_unit", "tx_range", "ty_unit", "ty_range", "rel_rotation", "rel_scale",
              "rel_translation"]
 
 
-@pytest.fixture(autouse=True)
-def _fp32():
-    # cuDNN / cuBLAS references in fp32 (torch's default lets cuDNN convolutions use TF32: 1e-3 relative error)
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
+# cuDNN / cuBLAS references in fp32 (torch's default lets cuDNN convolutions use TF32: 1e-3 relative error)
+pytestmark = pytest.mark.usefixtures("fp64_references")
 
 
 @pytest.fixture(scope="module")
@@ -132,26 +130,14 @@ def test_host_sampling_ranges_and_determinism():
 # ---------------------------------------------------------------------------------------------------------------
 # the kernel source compiled for the host (no GPU in the development container)
 # ---------------------------------------------------------------------------------------------------------------
-def _build_emu(tmp_path_factory, name):
-    out = str(tmp_path_factory.mktemp("emu") / f"lib{name}.so")
-    src = os.path.join(HERE, "host_emu", name + ".cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    return ctypes.CDLL(out)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return _build_emu(tmp_path_factory, "augment_emu")
+    return build(tmp_path_factory, "augment_emu")
 
 
 @pytest.fixture(scope="module")
 def emu_loss(tmp_path_factory):
-    return _build_emu(tmp_path_factory, "loss_emu")
-
-
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
+    return build(tmp_path_factory, "loss_emu")
 
 
 def emu_geometry(emu, img1, img2, flow, mask, P, target):
@@ -160,9 +146,9 @@ def emu_geometry(emu, img1, img2, flow, mask, P, target):
     o1, o2 = np.zeros((N, 3, TH, TW), np.float32), np.zeros((N, 3, TH, TW), np.float32)
     of, om = np.zeros((N, 2, TH, TW), np.float32), np.zeros((N, 1, TH, TW), np.float32)
     arrs = [np.ascontiguousarray(a) for a in (img1, img2, flow, mask, P)]
-    emu.emu_geometry_augment(_ptr(arrs[0]), _ptr(arrs[1]), int(img1.dtype == np.uint8), _ptr(arrs[2]), _ptr(arrs[3]),
-                             int(mask.shape[2:] == (1, 1) and (H, W) != (1, 1)), _ptr(arrs[4]), _ptr(o1), _ptr(o2), _ptr(of),
-                             _ptr(om), N, H, W, TH, TW)
+    emu.emu_geometry_augment(ptr(arrs[0]), ptr(arrs[1]), int(img1.dtype == np.uint8), ptr(arrs[2]), ptr(arrs[3]),
+                             int(mask.shape[2:] == (1, 1) and (H, W) != (1, 1)), ptr(arrs[4]), ptr(o1), ptr(o2), ptr(of),
+                             ptr(om), N, H, W, TH, TW)
     return o1, o2, of, om
 
 
@@ -223,11 +209,11 @@ def test_kernel_source_color_on_host(emu, fx):
     ws = np.zeros((2, N, 64, 3), np.float32)
     for k, (img, nz) in enumerate(((i1, n1), (i2, n2))):
         pre = np.zeros_like(img)
-        emu.emu_color_pre_mean(_ptr(img), _ptr(nz), _ptr(P), ctypes.c_float(sigma), ctypes.c_longlong(0), k, _ptr(pre), N, H, W)
+        emu.emu_color_pre_mean(ptr(img), ptr(nz), ptr(P), ctypes.c_float(sigma), ctypes.c_longlong(0), k, ptr(pre), N, H, W)
         ws[k, :, 0, :] = pre.sum(axis=(2, 3), dtype=np.float64)
     o1, o2 = np.zeros_like(i1), np.zeros_like(i2)
-    emu.emu_color_apply(_ptr(i1), _ptr(i2), _ptr(P), _ptr(n1), _ptr(n2), ctypes.c_float(sigma), ctypes.c_longlong(0), _ptr(ws),
-                        _ptr(o1), _ptr(o2), N, H, W, 1)
+    emu.emu_color_apply(ptr(i1), ptr(i2), ptr(P), ptr(n1), ptr(n2), ctypes.c_float(sigma), ctypes.c_longlong(0), ptr(ws),
+                        ptr(o1), ptr(o2), N, H, W, 1)
     assert np.abs(o1 - fx["col_img1"]).max() < 2e-5 and np.abs(o2 - fx["col_img2"]).max() < 2e-5
 
 
@@ -237,7 +223,7 @@ def test_kernel_source_philox_noise_on_host(emu):
     img = np.zeros((N, 3, H, W), np.float32)
     for image in (0, 1):
         pre = np.zeros_like(img)
-        emu.emu_color_pre_mean(_ptr(img), None, _ptr(P), ctypes.c_float(1.0), ctypes.c_longlong(seed), image, _ptr(pre), N, H, W)
+        emu.emu_color_pre_mean(ptr(img), None, ptr(P), ctypes.c_float(1.0), ctypes.c_longlong(seed), image, ptr(pre), N, H, W)
         want = augment_ref.philox_normal(N, H, W, seed, image)
         assert np.abs(pre - want).max() < 2e-5
     z = augment_ref.philox_normal(8, 64, 64, 99, 0)
@@ -357,12 +343,12 @@ def test_kernel_source_multiscale_epe_on_host(emu_loss, q):
     sa, wa = (ctypes.c_int * n)(*scales), (ctypes.c_float * n)(*weights)
     loss, msum = np.zeros(N, np.float32), np.zeros(N, np.float32)
     qf = ctypes.c_float(-1.0 if q is None else q)
-    emu_loss.emu_epe_forward(_ptr(flow), _ptr(mask), pa, sa, wa, n, ctypes.c_float(eps), qf, _ptr(loss), _ptr(msum), N, H, W)
+    emu_loss.emu_epe_forward(ptr(flow), ptr(mask), pa, sa, wa, n, ctypes.c_float(eps), qf, ptr(loss), ptr(msum), N, H, W)
     assert np.abs(loss - want_loss).max() < 1e-5 * max(1.0, np.abs(want_loss).max())
     assert np.abs(msum - mask.sum(axis=(1, 2, 3))).max() < 0.5
     grads = [np.full_like(p, np.nan) for p in preds]
     ga = (ctypes.c_void_p * n)(*[g.ctypes.data for g in grads])
-    emu_loss.emu_epe_backward(_ptr(flow), _ptr(mask), pa, sa, wa, n, ctypes.c_float(eps), qf, _ptr(gl), _ptr(msum), ga, N, H, W)
+    emu_loss.emu_epe_backward(ptr(flow), ptr(mask), pa, sa, wa, n, ctypes.c_float(eps), qf, ptr(gl), ptr(msum), ga, N, H, W)
     for g, w in zip(grads, want_grads):
         assert np.isfinite(g).all() and np.abs(g - w).max() < 1e-5 * max(1e-3, np.abs(w).max())
 

@@ -5,7 +5,7 @@ prediction and calls losses.unsupervised_loss, whose launches the supervised ste
 (mfn_flow_consistency), the stand-alone image warp ops.reconstruction2d (mfn_grid_generator_warp_forward +
 mfn_bilinear_sampler_forward and their backwards) on full-resolution flows, and the census and smoothness Functions.
 This file builds that step and checks every launch while it happens: the network, ops.upsample and its backward through
-the recorders of test_bench_shapes.py and test_bench_shapes_backward.py, the launches above through the wrappers below.
+Recorder and BackwardRecorder of launchcheck.recorders, the launches above through the wrappers below.
 Each wrapper runs the original, synchronises, and judges that launch alone, on the values it read, against float64.
 
 Bounds, per element (gamma_L = L u / (1 - L u), u = 2^-24, S the same sum on absolute values):
@@ -20,25 +20,22 @@ Bounds, per element (gamma_L = L u / (1 - L u), u = 2^-24, S the same sum on abs
   * bilinear sampler, position backward: the slope of the cell of the fp32 position, times (W - 1) / 2, judged by
     image_warp_flow_slopes (gamma_(C+6) S and the position terms; either cell where the position may lie on either side
     of an integer).  The data gradient is not requested: the images are data.
-  * census and smoothness: census_bounds / smoothness_bounds of test_unsup_loss.py (there E plays S's part).  The
+  * census and smoothness: census_bounds / smoothness_bounds of launchcheck.unsup_loss (there E plays S's part).  The
     smoothness gradient is judged with the signs of the second differences as the kernel evaluates them in fp32
     (kernel_signs): Upsample(4) makes most of them zero in exact arithmetic, where rounding decides the sign, and the
     float64 sign's allowance would be as large as the gradient itself, so that no control could fail it.
-  * flow_consistency: the decisions against the float64 rule of test_bidirectional.py outside its ambiguous pixels.
+  * flow_consistency: the decisions against the float64 rule of launchcheck.bidirectional outside its ambiguous pixels.
 Sensitivity (a control per new kind must fail by CONTROL_MARGIN on a real launch) and coverage (launch counts equal the
 graph's; sampled corners leave the frame on all four sides; the occluded share lies strictly inside (0, 1)) are
 asserted.  test_sampler_bounds_accept_kernel_arithmetic_and_reject_controls checks the same bounds on the CPU against
 the kernels' arithmetic (the backward compiled from its source, the forwards' fp32 order in torch).
 
-The network starts from the named weights of test_bench_shapes.py with its flow heads (pred_flow*, dc_conv7) scaled by
+The network starts from the named weights of launchcheck.inputs with its flow heads (pred_flow*, dc_conv7) scaled by
 FLOW_HEAD_SCALE: unscaled, the random heads give flows of several pixels that disagree between the two directions, so
 that 99 % of the pixels fail the consistency check and the census sees almost nothing.  Scaled, the flows stay below
 2 px, the size a fine-tuning run starting from a trained network sees on consecutive frames, and a fifth of the pixels
 (a twentieth in the cascade) pass the check.
 """
-import ctypes
-import os
-import subprocess
 import time
 
 import numpy as np
@@ -47,17 +44,18 @@ import torch
 
 from maskflownet_b200 import losses, network, ops, pipeline
 from oracle import unsup_ref
-from test_bench_shapes import Recorder, _images_u8, _named_model, _ratio
-from test_bench_shapes_backward import (CONTROL_MARGIN, U, BackwardRecorder, _gather0, gamma, image_warp_flow_slopes,
-                                        judge_bound, sampler_cell_slopes)
-from test_bidirectional import consistency_ref
-from test_unsup_loss import census_backward_control, census_bounds, smoothness_bounds
-from test_unsup_loss import ratio as unsup_ratio
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+from launchcheck import fp64_references  # noqa: F401
+from launchcheck.backward import _gather0, gamma, image_warp_flow_slopes, judge_bound, sampler_cell_slopes
+from launchcheck.bidirectional import consistency_ref
+from launchcheck.bounds import CONTROL_MARGIN, U, _ratio
+from launchcheck.emu import build, ptr
+from launchcheck.inputs import FLOW_HEAD_SCALE, _images_u8, _named_model
+from launchcheck.recorders import BackwardRecorder, Recorder
+from launchcheck.unsup_loss import census_backward_control, census_bounds, ratio as unsup_ratio, smoothness_bounds
+
 GRIDGEN_L, GRIDGEN_BWD_L = 3, 1        # f + p, __fdiv_rn, - 1 / __fdiv_rn
 SAMPLER_L = 6                          # wy * wx, then four products and sums
-FLOW_HEAD_SCALE = 1.0 / 16
 UPSAMPLE = 4                           # PipelineFlownet.scale: the last prediction is at a quarter of the resolution
 
 
@@ -358,9 +356,8 @@ NEW_CALLS = {
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("run", list(RUNS))
+@pytest.mark.usefixtures("fp64_references")
 def test_every_launch_of_the_unsupervised_step_against_float64(run, monkeypatch):
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
     cls, n, H, W, seed = RUNS[run]
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -417,17 +414,9 @@ def test_every_launch_of_the_unsupervised_step_against_float64(run, monkeypatch)
 # ------------------------------------------------------------------------------------------------------------------
 # CPU: the sampler and grid generator bounds accept the kernels' arithmetic and reject the controls
 # ------------------------------------------------------------------------------------------------------------------
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def warp_emu(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libimage_warp_bwd_emu.so")
-    src = os.path.join(HERE, "host_emu", "image_warp_bwd_emu.cpp")
-    subprocess.run(["g++", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-I", os.path.join(HERE, "host_emu"), "-o", out, src],
-                   check=True)
-    return ctypes.CDLL(out)
+    return build(tmp_path_factory, "image_warp_bwd_emu")
 
 
 def _emu_gridgen(f):
@@ -505,13 +494,13 @@ def test_sampler_bounds_accept_kernel_arithmetic_and_reject_controls(warp_emu):
     go = torch.randn((N, C, H, W), generator=g).numpy()
     gg = np.full((N, 2, H, W), np.nan, np.float32)
     grid_np, img_np = np.ascontiguousarray(grid.numpy()), np.ascontiguousarray(img.numpy())
-    warp_emu.emu_bilinear_sampler_backward(_ptr(go), _ptr(img_np), _ptr(grid_np), None, _ptr(gg), N, C, H, W, H, W)
+    warp_emu.emu_bilinear_sampler_backward(ptr(go), ptr(img_np), ptr(grid_np), None, ptr(gg), N, C, H, W, H, W)
     r, ctl, where = image_warp_flow_slopes(img, h, v, dh, dv, torch.from_numpy(go), ((H - 1) / 2, (W - 1) / 2),
                                            torch.from_numpy(gg).flip(1))
     assert r <= 1.0, where
     assert ctl >= CONTROL_MARGIN, ctl
     gf = np.full_like(gg, np.nan)
-    warp_emu.emu_grid_generator_warp_backward(_ptr(gg), _ptr(gf), N, H, W)
+    warp_emu.emu_grid_generator_warp_backward(ptr(gg), ptr(gf), N, H, W)
     gg64 = torch.from_numpy(gg).double()
     ref = gg64 / _gridgen_den(H, W, "cpu")
     assert judge_bound(torch.from_numpy(gf), ref, ref.abs(), GRIDGEN_BWD_L)[0] <= 1.0

@@ -9,15 +9,15 @@ in their own files on synthetic flows.  Here ChainRecorder replaces the ops the 
 ops.warp_frames_affine, ops.interpolate_frames, ops.flow_consistency) and network._pair_flows, which every forward of
 the chains and of network.predict_bidirectional goes through.  Each wrapper runs the original, synchronises, copies what
 the launch read and wrote to the host and judges that launch alone against the oracle on the inputs it read, with the
-judges of the kernels' own files (the forward and the masks are logged for the wiring only):
-  * affine_motion: test_stabilize._check_fit against stabilize_ref.fit (corners within 1e-6 px, residual within 1e-5 px
+judges the kernels' own files use, from launchcheck (the forward and the masks are logged for the wiring only):
+  * affine_motion: stabilize._check_fit against stabilize_ref.fit (corners within 1e-6 px, residual within 1e-5 px
     plus one float32 ulp, NaN in the same places);
-  * segment_motion: test_motion_segment._check against motionseg_ref.segment (labels, count, dropped, area, box,
+  * segment_motion: motion_segment._check against motionseg_ref.segment (labels, count, dropped, area, box,
     centroid and peak exact; dx, dy within the fixed-point bound);
-  * track_texture bit for bit against track_ref.texture; track_advance with test_tracking._compare_advance (exclusions
-    counted in a Tally, at most EXCLUDED_MAX) and track_seed with test_tracking._compare_seed (exact), both from the
+  * track_texture bit for bit against track_ref.texture; track_advance with tracking._compare_advance (exclusions
+    counted in a Tally, at most EXCLUDED_MAX) and track_seed with tracking._compare_seed (exact), both from the
     kernel's own previous state read out of the TrackState;
-  * warp_frames_affine: test_stabilize._check_warp against stabilize_ref.warp; interpolate_frames: test_interpolate._check
+  * warp_frames_affine: stabilize._check_warp against stabilize_ref.warp; interpolate_frames: interpolate._check
     against interp_ref.interpolate.
 Per-launch judging cannot see the wiring, because each launch is judged on whatever it read.  So the recorded flows,
 masks, residuals and fits are indexed by global pair p = k0 + j (the real pairs j < nb of each batch only) and the
@@ -61,15 +61,13 @@ from oracle import interp_ref
 from oracle import motionseg_ref as MR
 from oracle import stabilize_ref as SR
 from oracle import track_ref as TR
-from test_bidirectional_launches import _clip, _scaled_model
-from test_interpolate import EXCLUDED_MAX as INTERP_EXCLUDED_MAX
-from test_interpolate import _check as _check_interp
-from test_interpolate import _mismatch as _interp_mismatch
-from test_motion_segment import _check as _check_seg
-from test_motion_segment import _mismatch as _seg_mismatch
-from test_serving_shapes import _deterministic
-from test_stabilize import CORNER_TOL, WARP_EXACT, _check_fit, _check_warp, _fit_mismatch, _warp_mismatch
-from test_tracking import Tally, _compare_advance, _compare_seed
+
+from launchcheck.inputs import _clip, _deterministic, _scaled_model
+from launchcheck.interpolate import (EXCLUDED_MAX as INTERP_EXCLUDED_MAX, _check as _check_interp,
+                                     _mismatch as _interp_mismatch)
+from launchcheck.motion_segment import _check as _check_seg, _mismatch as _seg_mismatch
+from launchcheck.stabilize import CORNER_TOL, WARP_EXACT, _check_fit, _check_warp, _fit_mismatch, _warp_mismatch
+from launchcheck.tracking import Tally, _compare_advance, _compare_seed
 
 OPS = ("affine_motion", "segment_motion", "track_start", "track_texture", "track_advance", "track_seed",
        "warp_frames_affine", "interpolate_frames", "flow_consistency")
