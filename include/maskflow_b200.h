@@ -73,7 +73,8 @@ MFN_API unsigned long long mfn_launch_count(void);
  *   "conv_narrow"    default 1: 0 = every wgmma convolution takes 128-pixel tile rows (no 64-pixel rows)
  *   "conv_tma_in"    default 1: 0 = fp32 wgmma inputs are loaded per thread instead of staged by TMA
  *   "conv_dbg"       default 0: profiling switches of the wgmma convolution (2 = producers skip global loads, 4 = no
- *                    epilogue stores, 8 = no MMAs, 16 = no input path); any non-zero value makes results invalid */
+ *                    epilogue stores, 8 = no MMAs, 16 = no input path, 32 = no weight copies); any non-zero value
+ *                    makes results invalid */
 MFN_API int mfn_set_tuning(const char* key, int value);
 
 /* ---------------------------------------------------------------------------------------------------

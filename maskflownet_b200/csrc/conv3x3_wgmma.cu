@@ -222,12 +222,13 @@ __device__ __forceinline__ void decode_tile(int tile, int tilesX, int tilesY, co
     n = tile / (tilesX * tilesY);
   }
 }
-// split-activation operands on the device (SplitIO): in = 1: the input tiles come from the tensor map (groups in_g0.. of a
-// buffer of in_Cg groups per plane); in = 2: fp32 input whose raw tiles the tensor map {W, H, Cin, N} stages in shared
-// memory for the producers to convert; in = 0: fp32 input the producers load themselves.  out != null = output channels
+// split-activation operands on the device (SplitIO): in = 1: the input tiles are copied row by row from in_buf (groups
+// in_g0.. of a buffer of in_Cg groups per plane); in = 2: fp32 input whose raw tiles the tensor map {W, H, Cin, N} stages
+// in shared memory for the producers to convert; in = 0: fp32 input the producers load themselves.  out != null = output channels
 // >= the linear prefix go to channel out_c0.. of a split buffer of out_Cg groups
 struct SplitDev {
   int in, in_g0, in_Cg;
+  const unsigned char* in_buf;
   unsigned char* out;
   int out_Cg, out_c0;
 };
@@ -353,8 +354,9 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   // cut into sk.k parts over the channel chunks -- part p walks chunks [p nChunks / k, (p + 1) nChunks / k) and writes its
   // RAW partial sums (no bias, no activation) to the workspace; conv3x3_wgmma_reduce_kernel finishes that region.
   // dbg (tuning "conv_dbg", profiling only, results invalid): 2 = producers skip their global loads, 4 = no epilogue
-  // stores, 8 = no MMAs, 16 = producers skip loads, conversion and shared-memory stores (they only hand over each stage);
-  // the barrier protocol is unchanged, so each phase can be timed by removing it.
+  // stores, 8 = no MMAs, 16 = producers skip loads, conversion and shared-memory stores (they only hand over each stage),
+  // 32 = the weight loader issues no bulk copies (it only hands over each weight stage); the barrier protocol is
+  // unchanged, so each phase can be timed by removing it.
   static_assert(TERMS == 1 || TERMS == 3, "one or three products per multiply-add");
   static_assert(MT == MT_WIDE || MT == MT_NARROW, "128- or 64-pixel tile rows");
   constexpr bool FOLD_ACC = FOLD && TERMS == 3;   // the accumulator holds the [hi*hi | hi*lo] column blocks
@@ -639,8 +641,12 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           const unsigned char* src = wpack + (size_t)cb * 9 * sm.w_tile;
           for (int it = 9 * cb; it < 9 * ce; it += TPS, src += sm.w_stage) {
             if (wrapped) mbar_wait(w_empty + 8 * ws, wph ^ 1);
-            mbar_arrive_expect_tx(w_full + 8 * ws, (uint32_t)sm.w_stage);
-            bulk_g2s(s_base + (uint32_t)sm.w_off + ws * (uint32_t)sm.w_stage, src, (uint32_t)sm.w_stage, w_full + 8 * ws);
+            if (dbg & 32) {   // profiling: no weight copies, the stage holds whatever it held
+              mbar_arrive(w_full + 8 * ws);
+            } else {
+              mbar_arrive_expect_tx(w_full + 8 * ws, (uint32_t)sm.w_stage);
+              bulk_g2s(s_base + (uint32_t)sm.w_off + ws * (uint32_t)sm.w_stage, src, (uint32_t)sm.w_stage, w_full + 8 * ws);
+            }
             if (++ws == (uint32_t)WS) { ws = 0; wph ^= 1; wrapped = true; }
           }
         } else {
@@ -650,6 +656,11 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
           const unsigned char* src = wpack + (size_t)cb * 9 * gt;
           for (int it = 9 * cb; it < 9 * ce; it += TPS, src += TPS * gt) {
             if (wrapped) mbar_wait(w_empty + 8 * ws, wph ^ 1);
+            if (dbg & 32) {   // profiling: no weight copies
+              mbar_arrive(w_full + 8 * ws);
+              if (++ws == (uint32_t)WS) { ws = 0; wph ^= 1; wrapped = true; }
+              continue;
+            }
             mbar_arrive_expect_tx(w_full + 8 * ws, (uint32_t)sm.w_stage);
             const uint32_t dst = s_base + (uint32_t)sm.w_off + ws * (uint32_t)sm.w_stage;
 #pragma unroll 1
@@ -669,43 +680,50 @@ __global__ void __launch_bounds__(um::NTHREADS, 1)
   } else {
     // ============================ input producers (warps 9..11) ============================
     if (xs.in == 1) {
-      // split input (split_act.cuh): the buffer already holds the converted entries in the stage layout, so a chunk is a
-      // pure tensor copy -- hi and lo each one box {8 channels, PW pixels, nslots rows, 2 groups} (d < R), or one box of
-      // R rows per kernel row, group and plane (d >= R) -- issued by one thread.  Out-of-bounds rows / pixels read zero:
-      // the padding.
-      if (warp == 9 && lane == 0) {
+      // split input (split_act.cuh): the buffer already holds the converted entries in the stage layout, and each image
+      // row of one group and plane is one contiguous run of 16-byte entries.  So a chunk is nslots x 2 groups x P planes
+      // 1-D bulk copies of the tile row's in-image pixels, one per lane of warp 9 (at most 6 x 2 x 2 = 24).  Each lane
+      // first zeroes the entries of its row that lie outside the image (the padding; the stage may hold another tile's
+      // data there).  (A tensor copy of the same box moves one 16-byte entry per box row: that delivered a stage about
+      // as slowly as the MMAs of a narrow layer consume it.)
+      if (warp == 9) {
         uint32_t as = 0, aph = 0;
         bool wrapped = false;
+        const long long HW = (long long)H * W;
+        const int ncp = nslots * 2 * P;
+        const int pl = lane % P, kc = (lane / P) & 1, s = lane / (2 * P);   // this lane's row: plane, group, slot
+        const bool mine = lane < ncp;
+        const int ky = s / R, rr = s - ky * R;
         for (int work = blockIdx.x; work < numWork; work += gridDim.x) {
           const Work wk = decode_work(work, sk, nChunks);
           int tx, ty, n;
           decode_tile(wk.tile, tilesX, tilesY, sk, tx, ty, n);
           const int x0 = tx * MT - dil, y0 = ty * R;
-          const int gb = n * P * xs.in_Cg + xs.in_g0;
+          const int xa = x0 > 0 ? x0 : 0, xb = x0 + PW < W ? x0 + PW : W;
+          const int e0 = xa - x0, e1 = xb - x0;                 // entries [e0, e1) of a row lie inside the image
+          const int y = dil < R ? y0 - dil + s : y0 + (ky - 1) * dil + rr;
+          const bool row_in = mine && (unsigned)y < (unsigned)H;
+          const uint32_t bytes = (uint32_t)__popc(__ballot_sync(0xffffffffu, row_in)) * (uint32_t)(e1 - e0) * 16u;
           for (int c = wk.cb; c < wk.ce; ++c) {
             if (wrapped) mbar_wait(a_empty + 8 * as, aph ^ 1);
-            const uint32_t bar = a_full + 8 * as, dst = s_base + as * (uint32_t)sm.a_stage;
+            const uint32_t bar = a_full + 8 * as;
             if (dbg & 16) {
-              mbar_arrive(bar);
+              if (lane == 0) mbar_arrive(bar);
             } else {
-              mbar_arrive_expect_tx(bar, (uint32_t)sm.a_stage);
-              const int g = gb + 2 * c;
-              if (dil < R) {
-                tma_load_4d(dst, &tmx, 0, x0, y0 - dil, g, bar);
-                if constexpr (P == 2) tma_load_4d(dst + (uint32_t)sm.a_lo, &tmx, 0, x0, y0 - dil, g + xs.in_Cg, bar);
-              } else if constexpr (P == 1) {
-#pragma unroll 1
-                for (int k = 0; k < 6; ++k) {    // (kernel row ky, group kc), hi plane only
-                  const int ky = k >> 1, kc = k & 1;
-                  tma_load_4d(dst + (uint32_t)((kc * E + ky * R * PW) * 16), &tmx, 0, x0, y0 + (ky - 1) * dil, g + kc, bar);
-                }
-              } else {
-#pragma unroll 1
-                for (int k = 0; k < 12; ++k) {   // (kernel row ky, group kc, plane)
-                  const int ky = k >> 2, kc = (k >> 1) & 1, pl = k & 1;
-                  tma_load_4d(dst + (uint32_t)(pl * sm.a_lo + (kc * E + ky * R * PW) * 16), &tmx, 0, x0, y0 + (ky - 1) * dil,
-                              g + kc + pl * xs.in_Cg, bar);
-                }
+              unsigned char* const row = smem + as * sm.a_stage + pl * sm.a_lo + (kc * E + s * PW) * 16;
+              if (mine) {
+                const int z0 = row_in ? e0 : PW;
+                for (int e = 0; e < z0; ++e) *reinterpret_cast<uint4*>(row + e * 16) = make_uint4(0u, 0u, 0u, 0u);
+                if (row_in)
+                  for (int e = e1; e < PW; ++e) *reinterpret_cast<uint4*>(row + e * 16) = make_uint4(0u, 0u, 0u, 0u);
+              }
+              asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy zeros -> tensor core
+              __syncwarp();
+              if (lane == 0) mbar_arrive_expect_tx(bar, bytes);
+              __syncwarp();
+              if (row_in) {
+                const long long src = sa::entry<P>(n, pl, xs.in_g0 + 2 * c + kc, (long long)y * W + xa, xs.in_Cg, HW);
+                bulk_g2s(smem_u32(row + e0 * 16), xs.in_buf + src, (uint32_t)(e1 - e0) * 16u, bar);
               }
             }
             if (++as == (uint32_t)AS) { as = 0; aph ^= 1; wrapped = true; }
@@ -1092,26 +1110,17 @@ int conv3x3_wgmma_launch(const float* x, long long x_bs, const unsigned char* wp
   const int grow = ext == 2 ? 8 : 2 * ext;   // ext 1: grid + 1 pixel per side; ext 2: + the six band rows / columns too
   const int OH = stride == 2 ? (H - 1) / 2 + 1 : H + grow, OW = stride == 2 ? (W - 1) / 2 + 1 : W + grow;
   const int MT = tile_width(OW, stride);
-  SplitDev xs = {0, 0, 0, nullptr, 0, 0};
+  SplitDev xs = {0, 0, 0, nullptr, nullptr, 0, 0};
   CUtensorMap tmx;
   memset(&tmx, 0, sizeof tmx);
   if (sio.in != nullptr) {
-    // the tensor copies need 128-byte aligned shared-memory destinations: every box offset is, unless an odd d >= R
+    // the row copies need 16-byte aligned rows, which every split buffer has; odd dilations >= R are not supported
+    // (no layer has one)
     if (stride != 1 || ext != 0 || sio.in_c0 % 16 != 0 || (dil >= R && dil % 2 != 0) || !aligned(sio.in, 16)) return -1;
-    EncodeTiledFn fn = encode_tiled_fn();
-    if (fn == nullptr) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
-    const int Cg = sa::groups(sio.in_C);
-    const cuuint64_t dim[4] = {8, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N * (terms == 1 ? 1 : 2) * Cg};
-    const cuuint64_t strides[3] = {16, (cuuint64_t)W * 16, (cuuint64_t)W * H * 16};
-    const cuuint32_t box[4] = {8, (cuuint32_t)row_pitch(MT, 1, dil), (cuuint32_t)(dil < R ? n_slots(1, dil) : R), dil < R ? 2u : 1u};
-    const cuuint32_t es[4] = {1, 1, 1, 1};
-    const CUresult r = fn(&tmx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(sio.in), dim, strides, box, es,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(MFN_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
     xs.in = 1;
+    xs.in_buf = static_cast<const unsigned char*>(sio.in);
     xs.in_g0 = sio.in_c0 / 8;
-    xs.in_Cg = Cg;
+    xs.in_Cg = sa::groups(sio.in_C);
   }
   if (sio.out != nullptr) {
     // whole 16-channel chunks after the prefix: pairs stay pairs, and the buffer's pad channels are never written

@@ -4,7 +4,7 @@
 // A buffer of C channels holds Cg = ceil(C / 16) * 2 groups of 8 channels as (N, 2, Cg, H, W, 8) bf16: per sample first the
 // hi image of every group, then the lo image; one 16-byte entry per (plane, group, pixel).  4 bytes per channel-pixel, as
 // fp32.  Channels C .. 16 ceil(C / 16) - 1 are ZERO (the packed weights are zero there too, and 0 * NaN would poison the
-// sum).  The convolution loads an input chunk (two groups, hi and lo) of a box of rows with one tensor copy each, and the
+// sum).  The convolution loads an input chunk (two groups, hi and lo) of a box of rows with one bulk copy per row, and the
 // value it multiplies is bit for bit the split_pair of the fp32 value, so results do not depend on the input's format.
 // Writers: the pack kernel (split_act.cu) and the wgmma convolution's epilogues, all through `entry` and split_pair;
 // ops.SplitAct is the only Python code that knows the layout.

@@ -5,12 +5,15 @@
 
 Runs one eager MaskFlownet-S forward (BASELINE configs[1]: batch 8, 1024x448, seeded inputs and weights) and records every
 convolution launch (ops.conv3x3_slices / ops.conv3x3_split) with the layer that issued it.  Each recorded launch is then replayed on its own,
-bracketed by CUDA events (median of --reps), in five variants of the profiling knob `conv_dbg` of the wgmma kernel:
+bracketed by CUDA events (median of --reps), in seven variants of the profiling knob `conv_dbg` of the wgmma kernel:
 
     full      the real kernel
     -load     producers skip their global loads (they still convert and hand over every stage)
     -input    producers skip loads, conversion and shared-memory stores (they only hand over every stage): what a free
               input path would cost
+    -wload    the weight loader issues no bulk copies (it still hands over every weight stage)
+    -feed     neither the input nor the weight stages are delivered (-input and -wload together): what the kernel would
+              take if nothing had to reach shared memory
     -store    no epilogue stores
     -mma      no tensor-core MMAs (the barrier protocol is unchanged)
 
@@ -24,7 +27,7 @@ Per launch the table prints the shape, the time, and two lower bounds:
 
 and `frac` = max(mma, hbm) / time.  --precision bf16 runs the forward in the opt-in bf16 mode (inference_precision):
 its launches issue one bf16 product per fp32 product, so the mma bound counts one (and the hbm bound reads bf16
-activations at 2 bytes per channel-pixel).  The four deltas (time minus the time without a phase) show what each phase adds to
+activations at 2 bytes per channel-pixel).  The six deltas (time minus the time without a phase) show what each phase adds to
 the critical path.  Both rates are for a 700 W part; a card with a lower power limit runs slower clocks.
 """
 from __future__ import annotations
@@ -51,7 +54,8 @@ def tile_width(ow: int, stride: int) -> int:
     return 64 if ow <= 64 or stride == 2 else 128
 
 
-MODES = (("full", 0), ("-load", 2), ("-input", 16), ("-store", 4), ("-mma", 8))
+MODES = (("full", 0), ("-load", 2), ("-input", 16), ("-wload", 32), ("-feed", 48), ("-store", 4), ("-mma", 8))
+DELTAS = ("-load", "-input", "-wload", "-feed", "-store", "-mma")
 
 
 def cout_pad(cin: int, cout: int) -> int:
@@ -200,9 +204,10 @@ def main():
           f"times in us (median of {args.reps}); bounds at 989 TFLOP/s bf16 and 3.35 TB/s, {terms} product(s) per MAC")
     want = {int(x) for x in args.levels.split(",") if x.strip()}
     hdr = (f"{'layer':16s} {'N':>2s} {'Cin':>4s} {'Cout':>4s} {'H':>4s} {'W':>5s} s d {'time':>8s} {'mma':>8s} {'hbm':>7s} "
-           f"{'frac':>5s} {'load':>7s} {'input':>7s} {'store':>7s} {'mma':>7s}")
+           f"{'frac':>5s} " + " ".join(f"{k[1:]:>7s}" for k in DELTAS))
     print(hdr)
     per_level = collections.OrderedDict()
+    NV = 4 + len(DELTAS)   # time, mma, hbm, useful, then the deltas
     rows = []
     for c in calls:
         mma, hbm, useful = bounds(c, terms)
@@ -211,30 +216,29 @@ def main():
         lvl = 2 if c["layer"].startswith("dc_conv") else (int(m.group()) if m else 0)
         kind = "pyramid" if re.fullmatch(r"conv\d[abc]", c["layer"]) else "decoder"
         grp = f"{kind} L{lvl}"
-        d = {k: c["full"] - c[k] for k in ("-load", "-input", "-store", "-mma")}
+        d = {k: c["full"] - c[k] for k in DELTAS}
         row = {k: v for k, v in c.items() if k not in ("args", "fn")}
         row.update(level=lvl, group=grp, mma_us=mma * 1e6, hbm_us=hbm * 1e6, useful_us=useful * 1e6,
                    frac=max(mma, hbm) / t)
         rows.append(row)
-        agg = per_level.setdefault(grp, [0.0] * 8 + [0])
-        for i, v in enumerate((c["full"], mma * 1e3, hbm * 1e3, useful * 1e3, d["-load"], d["-input"], d["-store"],
-                               d["-mma"])):
+        agg = per_level.setdefault(grp, [0.0] * NV + [0])
+        for i, v in enumerate((c["full"], mma * 1e3, hbm * 1e3, useful * 1e3) + tuple(d[k] for k in DELTAS)):
             agg[i] += v
-        agg[8] += 1
+        agg[NV] += 1
         if want and lvl not in want:
             continue
         print(f"{c['layer']:16s} {c['N']:2d} {c['Cin']:4d} {c['Cout']:4d} {c['H']:4d} {c['W']:5d} {c['stride']} "
               f"{c['dil']:<2d}{c['full'] * 1e3:7.0f} {mma * 1e6:8.0f} {hbm * 1e6:7.0f} {max(mma, hbm) / t:5.2f} "
-              f"{d['-load'] * 1e3:7.0f} {d['-input'] * 1e3:7.0f} {d['-store'] * 1e3:7.0f} {d['-mma'] * 1e3:7.0f}")
+              + " ".join(f"{d[k] * 1e3:7.0f}" for k in DELTAS))
     print(f"\n{'group':12s} {'calls':>5s} {'time':>8s} {'mma':>8s} {'useful':>8s} {'hbm':>7s} {'frac':>5s} "
-          f"{'load':>7s} {'input':>7s} {'store':>7s} {'mma':>7s}   (us; frac = mma bound / time)")
-    tot = [0.0] * 8 + [0]
+          + " ".join(f"{k[1:]:>7s}" for k in DELTAS) + "   (us; frac = mma bound / time)")
+    tot = [0.0] * NV + [0]
     for grp, v in sorted(per_level.items(), key=lambda kv: -kv[1][0]):
         tot = [x + y for x, y in zip(tot, v)]
-        print(f"{grp:12s} {v[8]:5d} {v[0] * 1e3:8.0f} {v[1] * 1e3:8.0f} {v[3] * 1e3:8.0f} {v[2] * 1e3:7.0f} "
-              f"{v[1] / v[0]:5.2f} {v[4] * 1e3:7.0f} {v[5] * 1e3:7.0f} {v[6] * 1e3:7.0f} {v[7] * 1e3:7.0f}")
-    print(f"{'all':12s} {tot[8]:5d} {tot[0] * 1e3:8.0f} {tot[1] * 1e3:8.0f} {tot[3] * 1e3:8.0f} {tot[2] * 1e3:7.0f} "
-          f"{tot[1] / tot[0]:5.2f} {tot[4] * 1e3:7.0f} {tot[5] * 1e3:7.0f} {tot[6] * 1e3:7.0f} {tot[7] * 1e3:7.0f}")
+        print(f"{grp:12s} {v[NV]:5d} {v[0] * 1e3:8.0f} {v[1] * 1e3:8.0f} {v[3] * 1e3:8.0f} {v[2] * 1e3:7.0f} "
+              f"{v[1] / v[0]:5.2f} " + " ".join(f"{x * 1e3:7.0f}" for x in v[4:NV]))
+    print(f"{'all':12s} {tot[NV]:5d} {tot[0] * 1e3:8.0f} {tot[1] * 1e3:8.0f} {tot[3] * 1e3:8.0f} {tot[2] * 1e3:7.0f} "
+          f"{tot[1] / tot[0]:5.2f} " + " ".join(f"{x * 1e3:7.0f}" for x in tot[4:NV]))
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"device": dev, "precision": args.precision, "eager_forward_ms": step, "rows": rows}, f, indent=1)
