@@ -36,7 +36,8 @@ strictly inside (0, 1) and both decisions are reached.  hd8 runs once more in bf
 
 Not checked here: frames larger than 1088x1920; the kernels of the video tools that follow this forward (interpolation,
 tracking, stabilisation and motion segmentation): test_video_chain_launches.py checks every one of their launches in
-the tools' chains against float64 at batch 8 on 1080p, and which pair each frame reads.
+the tools' chains against float64 at batch 8 on 1080p, and which pair each frame reads; test_denoise_chain_launches.py
+does the same for video denoising (network.denoise_video and VideoDenoiser's ring).
 """
 import time
 

@@ -47,6 +47,9 @@ reset), the last frame from pair P - 2, advance k against pair k's flows, seed k
 camera path from fits shifted by one pair.  test_shared_chain_wiring_restatements_on_host runs the same recorder and
 wiring checks on the CPU, with the oracles standing in for the kernels and hand-made per-pair flows, at B = 3 and P = 7:
 the right assignment passes and every wiring control fails.
+
+Not checked here: video denoising, whose chain (network.denoise_video, and VideoDenoiser's ring of frames and flows)
+test_denoise_chain_launches.py checks launch by launch and wire by wire in the same way.
 """
 import os
 import time
